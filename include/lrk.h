@@ -18,6 +18,8 @@
  *                       <- (none; sums the film of src/films/color.cpp:107-130 over ranks)  SURVEY.md §8e
  *   lrk_film_clear      <- Film::Instance::prepare / clear                      src/films/color.cpp:132-144
  *   lrk_render          <- ProgressiveIntegrator::Instance::_render_one_camera  src/integrators/wave_path.cpp:220-567
+ *   lrk_render_adaptive / lrk_download_sample_counts / lrk_download_film_variance
+ *                       <- (none: an extension, the reference has no adaptive sampling)  DESIGN.md §4 (Adaptive sampling)
  *   lrk_download_film   <- Film::Instance::download (convert_image + copy)      src/films/color.cpp:87-105
  *   lrk_download_film_raw / lrk_film_device_ptr
  *                       <- the raw (sum rgb, sum weight) float4 film buffer     src/films/color.cpp:107-130
@@ -39,7 +41,7 @@
 extern "C" {
 #endif
 
-#define LRK_ABI_VERSION 6u /* 6: lrk_comm_* / lrk_reduce_film, lrk_stats::reduce_ms, hashed lrk_tile_owner */
+#define LRK_ABI_VERSION 7u /* 7: lrk_render_adaptive, lrk_download_sample_counts, lrk_download_film_variance */
 
 typedef enum lrk_status {
     LRK_OK = 0,
@@ -555,6 +557,34 @@ int lrk_film_clear(lrk_ctx *ctx);
 /* Render sample indices [spp_begin, spp_end) of every pixel of this ctx's shard and add
  * them to the film.  Asynchronous work is synchronised before returning. */
 int lrk_render(lrk_ctx *ctx, uint32_t spp_begin, uint32_t spp_end);
+
+/* Adaptive sampling (an extension: the reference has none; DESIGN.md §4 (Adaptive sampling)).  lrk_render_adaptive clears the film and renders
+ * every pixel of this ctx's shard with a sample count of its own, n_p: sample indices [0, n_p), exactly the samples lrk_render(ctx,
+ * 0, n_p) would add to that pixel, so the pixel's raw film entry is bit-identical to it.
+ *   Rounds: every pixel gets [0, min_spp); after each round the pixels still active get [c, min(2c, max_spp)), c = their count.
+ *           The render ends when no pixel is active or c == max_spp; a pixel that stops never restarts.  Counts are therefore
+ *           min_spp * 2^k or max_spp.  Passes are sized like lrk_render's, for the active pixels.
+ *   Error:  per pixel, from the film weight n (the samples the film kept, see the NaN / Inf filter) and the moments S1 = sum Y,
+ *           S2 = sum Y^2 of those samples, Y = 0.2126 r + 0.7152 g + 0.0722 b of the clamped contribution times film.scale:
+ *           m = S1 / n, v = max(S2 / n - m^2, 0) / (n - 1), e = sqrt(v) / max(m, 0.01) in IEEE fp32 (e = v = +inf when n < 2).
+ *   Rule:   the unit is the 8x4 pixel block of the shard's pixel order (smaller at tile edges; blocks never cross tiles): a block
+ *           stops when the maximum e over its pixels is strictly below `threshold`.  threshold = 0 never stops a block before
+ *           max_spp, even one without any noise.  Decisions depend on the block's own pixels only, so a sharded, reduced render
+ *           equals a single-GPU one bit for bit.
+ * LRK_ERR_INVALID_ARGUMENT: min_spp < 2, max_spp < min_spp, a negative or non-finite threshold.  lrk_stats::samples counts the
+ * samples rendered.  The moments buffer (8 B per pixel) and the count buffer are allocated by the first call. */
+typedef struct lrk_adaptive {
+    uint32_t min_spp, max_spp;
+    float threshold;
+    uint32_t reserved;
+} lrk_adaptive;
+int lrk_render_adaptive(lrk_ctx *ctx, const lrk_adaptive *p);
+/* The sample count n_p of every pixel of the last adaptive render: W*H uint32, 0 outside this ctx's shard.
+ * LRK_ERR_INVALID_ARGUMENT when no adaptive render ran since the last lrk_film_clear / lrk_upload_scene / lrk_render. */
+int lrk_download_sample_counts(lrk_ctx *ctx, uint32_t *counts);
+/* v above (the variance of the pixel's mean luminance: a noise map) for every pixel of the last adaptive render: W*H float,
+ * 0 outside this ctx's shard.  Same error as lrk_download_sample_counts. */
+int lrk_download_film_variance(lrk_ctx *ctx, float *v);
 
 /* rgba = (sum_rgb / max(sum_w, 1)) * scale, a = 1 : W*H float4 (src/films/color.cpp:87-93) */
 int lrk_download_film(lrk_ctx *ctx, float *rgba);

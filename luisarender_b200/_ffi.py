@@ -13,7 +13,7 @@ PKG_DIR = Path(__file__).resolve().parent
 REPO_DIR = PKG_DIR.parent
 LIB_DIR = PKG_DIR / "lib"
 
-LRK_ABI_VERSION = 6
+LRK_ABI_VERSION = 7
 TEX_ADDRESS_EDGE, TEX_ADDRESS_REPEAT, TEX_ADDRESS_MIRROR, TEX_ADDRESS_ZERO = 0, 1, 2, 3
 TEX_FILTER_POINT, TEX_FILTER_LINEAR = 0, 1
 TEX_ENCODING_LINEAR, TEX_ENCODING_SRGB, TEX_ENCODING_GAMMA = 0, 1, 2
@@ -143,6 +143,10 @@ class Stats(C.Structure):
                 ("other_ms", f64), ("reduce_ms", f64)]
 
 
+class Adaptive(C.Structure):
+    _fields_ = [("min_spp", u32), ("max_spp", u32), ("threshold", f32), ("reserved", u32)]
+
+
 class SceneInfo(C.Structure):
     _fields_ = [("unique_triangles", u64), ("instanced_triangles", u64), ("vertices", u64), ("bvh_nodes", u64),
                 ("meshes", u32), ("instances", u32), ("surfaces", u32), ("lights", u32), ("cameras", u32),
@@ -154,6 +158,7 @@ LRK_SYMBOLS = [
     "lrk_set_option", "lrk_film_clear", "lrk_render", "lrk_download_film", "lrk_download_film_raw",
     "lrk_film_device_ptr", "lrk_film_normalize_to_host", "lrk_trace", "lrk_trace_device", "lrk_get_stats",
     "lrk_stream", "lrk_comm_unique_id", "lrk_comm_init", "lrk_reduce_film", "lrk_balance_shards", "lrk_assign_tiles",
+    "lrk_render_adaptive", "lrk_download_sample_counts", "lrk_download_film_variance",
 ]
 LRH_SYMBOLS = [
     "lrh_last_error", "lrh_scene_load", "lrh_scene_load_source", "lrh_scene_destroy", "lrh_scene_get_info",
@@ -223,5 +228,8 @@ def device_lib() -> C.CDLL:
         lib.lrk_reduce_film.argtypes = [C.c_void_p, u32]
         lib.lrk_balance_shards.argtypes = [C.c_void_p, u32, u32, u32, u32]
         lib.lrk_assign_tiles.argtypes = [C.c_void_p, u32, u32, C.c_void_p]
+        lib.lrk_render_adaptive.argtypes = [C.c_void_p, C.POINTER(Adaptive)]
+        lib.lrk_download_sample_counts.argtypes = [C.c_void_p, C.c_void_p]
+        lib.lrk_download_film_variance.argtypes = [C.c_void_p, C.c_void_p]
         lib._lrk_typed = True
     return lib

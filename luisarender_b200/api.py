@@ -144,6 +144,26 @@ class Renderer:
     def render(self, spp_begin: int, spp_end: int):
         self._check(self._lib.lrk_render(self._ctx, spp_begin, spp_end), "lrk_render")
 
+    def render_adaptive(self, threshold: float, min_spp: int, max_spp: int):
+        """lrk_render_adaptive: clear the film, then render every pixel until the 8x4 block around it has a relative standard error
+        below `threshold` (rounds of min_spp, 2 min_spp, 4 min_spp, ... samples, at most max_spp; include/lrk.h)."""
+        p = F.Adaptive(min_spp, max_spp, threshold, 0)
+        self._check(self._lib.lrk_render_adaptive(self._ctx, C.byref(p)), "lrk_render_adaptive")
+
+    def sample_counts(self) -> np.ndarray:
+        """The samples every pixel got in the last adaptive render, [H, W] uint32 (0 outside this context's shard)."""
+        w, h = self._res
+        out = np.empty((h, w), dtype=np.uint32)
+        self._check(self._lib.lrk_download_sample_counts(self._ctx, out.ctypes.data), "lrk_download_sample_counts")
+        return out
+
+    def film_variance(self) -> np.ndarray:
+        """The variance of every pixel's mean luminance after the last adaptive render, [H, W] float32 (0 outside the shard)."""
+        w, h = self._res
+        out = np.empty((h, w), dtype=np.float32)
+        self._check(self._lib.lrk_download_film_variance(self._ctx, out.ctypes.data), "lrk_download_film_variance")
+        return out
+
     def film(self, raw: bool = False, out: np.ndarray | None = None) -> np.ndarray:
         """The film as [H, W, 4] float32: normalised like the reference's convert_image, or the raw sums (raw=True).
         `out`: destination to reuse (with the option pin_host_buffers the library page-locks it once)."""

@@ -274,9 +274,13 @@ __global__ void __launch_bounds__(kTraceBlock) trace_volume_nee_kernel(DeviceSce
 // ---- film ---------------------------------------------------------------------------------------------------
 // One thread per pixel of the chunk: adds the S samples of this pass in sample order (deterministic).
 // Per-sample clamp / NaN filter: src/films/color.cpp:107-130 with effective_spp = 1.
+// MOMENTS (the adaptive mode, adaptive.cuh): also adds Y and Y^2 of every sample the film keeps to moments[pixel], where Y is the
+// display luminance of the clamped contribution times film.scale.
+template<bool MOMENTS>
 __global__ void __launch_bounds__(kBlock) accumulate_kernel(DeviceScene sc, const float4 *__restrict__ li, float4 *__restrict__ film,
                                                             const uint32_t *__restrict__ pixel_list, uint32_t pixel_offset, uint32_t npix,
-                                                            uint32_t spp, const uint32_t *__restrict__ counts, unsigned long long *stats) {
+                                                            uint32_t spp, const uint32_t *__restrict__ counts, unsigned long long *stats,
+                                                            float2 *__restrict__ moments) {
     uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k == 0u) {// ray totals of this pass = sum of the per-depth queue sizes
         unsigned long long closest = 0ull, shadow = 0ull;
@@ -292,6 +296,7 @@ __global__ void __launch_bounds__(kBlock) accumulate_kernel(DeviceScene sc, cons
     uint32_t px = pixel & 0xffffu, py = pixel >> 16u;
     size_t pid = static_cast<size_t>(py) * sc.width + px;
     float4 acc = film[pid];
+    float2 mom = MOMENTS ? moments[pid] : make_float2(0.f, 0.f);
     const float threshold = sc.film_clamp * fmaxf(1.f, 1.f);
     for (uint32_t s = 0; s < spp; s++) {
         float4 v = li[static_cast<size_t>(s) * npix + k];
@@ -306,8 +311,14 @@ __global__ void __launch_bounds__(kBlock) accumulate_kernel(DeviceScene sc, cons
             acc.z += c.z;
         }
         acc.w += 1.f;
+        if (MOMENTS) {
+            const float y = 0.2126f * (c.x * sc.film_scale[0]) + 0.7152f * (c.y * sc.film_scale[1]) + 0.0722f * (c.z * sc.film_scale[2]);
+            mom.x += y;
+            mom.y += y * y;
+        }
     }
     film[pid] = acc;
+    if (MOMENTS) moments[pid] = mom;
 }
 
 // convert_image: src/films/color.cpp:87-93

@@ -3,6 +3,7 @@
 // no host synchronisation inside a pass, queue sizes stay on the device.
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <limits>
@@ -14,6 +15,8 @@
 #include "shade_launch.h"
 #include "bvh_build.cuh"
 #include "comm.cuh"
+#include "adaptive.cuh"
+#include <cub/device/device_scan.cuh>
 
 using namespace lrk;
 
@@ -87,6 +90,17 @@ struct lrk_ctx {
     int grid_vgeneral{0};
     uint64_t volume_capacity{0};
     int grid_vshade[2][3]{}, grid_vmedium[2]{0, 0}, grid_vshadow{0};
+    // adaptive mode (lrk_render_adaptive); the device buffers are allocated on its first call
+    std::vector<uint32_t> block_start;// offsets of the 8x4 pixel blocks in the pixel list, closed by npix_owned (build_pixel_list)
+    float2 *pass_moments{nullptr};// set while lrk_render_adaptive runs: the film accumulation also adds the luminance moments here
+    float2 *d_moments{nullptr};
+    uint32_t *d_sample_counts{nullptr};
+    uint32_t *d_active[2]{nullptr, nullptr};// ping-pong active pixel lists of the rounds after the first
+    uint32_t *d_block_start[3]{nullptr, nullptr, nullptr};// [0]: block_start; [1], [2]: the ping-pong lists' blocks
+    unsigned long long *d_keep{nullptr};// keep words and their exclusive scan (adaptive.cuh), 2 x (blocks + 1)
+    void *d_scan_temp{nullptr};
+    size_t scan_temp_bytes{0}, adaptive_pixels{0}, adaptive_list{0}, adaptive_blocks{0};// capacities of the buffers above
+    bool adaptive_valid{false};// the film is the result of an adaptive render: sample counts and variance can be downloaded
 };
 
 namespace {
@@ -222,6 +236,7 @@ int build_pixel_list(lrk_ctx *ctx) {
     const uint32_t tiles_x = (W + ts - 1u) / ts, tiles_y = (H + ts - 1u) / ts;
     std::vector<uint32_t> list;
     list.reserve(static_cast<size_t>(W) * H / ctx->world + 1024u);
+    ctx->block_start.clear();
     for (uint32_t ty = 0; ty < tiles_y; ty++) {
         for (uint32_t tx = 0; tx < tiles_x; tx++) {
             uint32_t tile_id = ty * tiles_x + tx;
@@ -230,11 +245,14 @@ int build_pixel_list(lrk_ctx *ctx) {
             uint32_t x0 = tx * ts, y0 = ty * ts;
             uint32_t x1 = std::min(W, x0 + ts), y1 = std::min(H, y0 + ts);
             for (uint32_t by = y0; by < y1; by += 4u)
-                for (uint32_t bx = x0; bx < x1; bx += 8u)
+                for (uint32_t bx = x0; bx < x1; bx += 8u) {
+                    ctx->block_start.push_back(static_cast<uint32_t>(list.size()));
                     for (uint32_t y = by; y < std::min(y1, by + 4u); y++)
                         for (uint32_t x = bx; x < std::min(x1, bx + 8u); x++) list.push_back(x | (y << 16u));
+                }
         }
     }
+    ctx->block_start.push_back(static_cast<uint32_t>(list.size()));
     if (ctx->d_pixel_list) {
         cudaFree(ctx->d_pixel_list);
         ctx->d_pixel_list = nullptr;
@@ -288,10 +306,21 @@ void launch_query(lrk_ctx *ctx, int g, bool any_hit, const float4 *d_rays, uint4
     else any_hit ? launch(trace_query_kernel<true, false>) : launch(trace_query_kernel<false, false>);
 }
 
-int render_pass(lrk_ctx *ctx, uint32_t pixel_offset, uint32_t npix, uint32_t spp_begin, uint32_t spp) {
+// The film accumulation of a pass; with the adaptive mode's moments while lrk_render_adaptive runs.
+void launch_accumulate(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp) {
+    ScopedTimer t{ctx, CAT_OTHER};
+    auto launch = [&](auto kernel) {
+        kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->scene, ctx->pb.li, ctx->d_film, pixel_list, pixel_offset, npix, spp,
+                                                                        ctx->pb.counts, ctx->pb.stats, ctx->pass_moments);
+    };
+    ctx->pass_moments != nullptr ? launch(accumulate_kernel<true>) : launch(accumulate_kernel<false>);
+}
+
+// One pass: sample indices [spp_begin, spp_begin + spp) of the pixels pixel_list[pixel_offset .. pixel_offset + npix).
+int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp_begin, uint32_t spp) {
     const uint64_t n = static_cast<uint64_t>(npix) * spp;
     auto &pb = ctx->pb;
-    pb.pass_pixel_list = ctx->d_pixel_list;
+    pb.pass_pixel_list = pixel_list;
     pb.pass_pixel_offset = pixel_offset;
     pb.pass_npix = npix;
     pb.pass_spp_begin = spp_begin;
@@ -302,7 +331,7 @@ int render_pass(lrk_ctx *ctx, uint32_t pixel_offset, uint32_t npix, uint32_t spp
     {
         ScopedTimer t{ctx, CAT_OTHER};
         generate_rays_kernel<<<static_cast<unsigned>((n + kBlock - 1u) / kBlock), kBlock, 0, ctx->stream>>>(
-            sc, pb, ctx->d_pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
+            sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
     }
     ctx->stats.kernel_launches++;
     // upper bound of the live queue at depth d is n; launch persistent-size grids and let kernels read *count
@@ -347,11 +376,7 @@ int render_pass(lrk_ctx *ctx, uint32_t pixel_offset, uint32_t npix, uint32_t spp
         ctx->stats.kernel_launches += 4u + (ctx->has_kind[1] ? 1u : 0u) + (ctx->has_kind[2] ? 1u : 0u) + (ctx->has_kind[3] ? 1u : 0u) + (ctx->has_kind[4] ? 1u : 0u) +
                                       (ctx->has_kind[5] ? 1u : 0u) + (ctx->has_kind[6] ? 1u : 0u) + (ctx->has_kind[7] ? 1u : 0u) + (ctx->has_kind[8] ? 1u : 0u);
     }
-    {
-        ScopedTimer t{ctx, CAT_OTHER};
-        accumulate_kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(sc, pb.li, ctx->d_film, ctx->d_pixel_list, pixel_offset,
-                                                                                  npix, spp, pb.counts, pb.stats);
-    }
+    launch_accumulate(ctx, pixel_list, pixel_offset, npix, spp);
     ctx->stats.kernel_launches++;
     ctx->stats.passes++;
     LRK_CUDA(cudaGetLastError());
@@ -360,7 +385,7 @@ int render_pass(lrk_ctx *ctx, uint32_t pixel_offset, uint32_t npix, uint32_t spp
 
 // One pass of the volume path integrator (config C4); schedule described in kernels.cuh.
 // the general volume path: one thread per camera sample (volume_general.cuh), then the common film accumulation
-int render_pass_volume_general(lrk_ctx *ctx, uint32_t pixel_offset, uint32_t npix, uint32_t spp_begin, uint32_t spp) {
+int render_pass_volume_general(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp_begin, uint32_t spp) {
     const uint64_t n = static_cast<uint64_t>(npix) * spp;
     auto &pb = ctx->pb;
     const auto &sc = ctx->scene;
@@ -368,30 +393,26 @@ int render_pass_volume_general(lrk_ctx *ctx, uint32_t pixel_offset, uint32_t npi
         ScopedTimer t{ctx, CAT_SHADE};
         const unsigned blocks = static_cast<unsigned>((n + kGeneralBlock - 1u) / kGeneralBlock);
         auto launch = [&](auto kernel) {
-            kernel<<<blocks, kGeneralBlock, 0, ctx->stream>>>(sc, pb, ctx->d_pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
+            kernel<<<blocks, kGeneralBlock, 0, ctx->stream>>>(sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
         };
         ctx->any_non_opaque ? launch(volume_general_kernel<true>) : launch(volume_general_kernel<false>);
     }
-    {
-        ScopedTimer t{ctx, CAT_OTHER};
-        accumulate_kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(sc, pb.li, ctx->d_film, ctx->d_pixel_list, pixel_offset,
-                                                                                  npix, spp, pb.counts, pb.stats);
-    }
+    launch_accumulate(ctx, pixel_list, pixel_offset, npix, spp);
     ctx->stats.kernel_launches += 2u;
     ctx->stats.passes++;
     LRK_CUDA(cudaGetLastError());
     return LRK_OK;
 }
 
-int render_pass_volume(lrk_ctx *ctx, uint32_t pixel_offset, uint32_t npix, uint32_t spp_begin, uint32_t spp) {
-    if (ctx->volume_general) return render_pass_volume_general(ctx, pixel_offset, npix, spp_begin, spp);
+int render_pass_volume(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp_begin, uint32_t spp) {
+    if (ctx->volume_general) return render_pass_volume_general(ctx, pixel_list, pixel_offset, npix, spp_begin, spp);
     const uint64_t n = static_cast<uint64_t>(npix) * spp;
     auto &pb = ctx->pb;
     const auto &sc = ctx->scene;
     {
         ScopedTimer t{ctx, CAT_OTHER};
         generate_rays_volume_kernel<<<static_cast<unsigned>((n + kBlock - 1u) / kBlock), kBlock, 0, ctx->stream>>>(
-            sc, pb, ctx->d_pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
+            sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
     }
     ctx->stats.kernel_launches++;
     for (uint32_t depth = 0; depth < sc.max_depth; depth++) {
@@ -439,11 +460,7 @@ int render_pass_volume(lrk_ctx *ctx, uint32_t pixel_offset, uint32_t npix, uint3
         }
         ctx->stats.kernel_launches += 5u + (ctx->has_kind[1] ? 1u : 0u) + (ctx->has_kind[2] ? 1u : 0u);
     }
-    {
-        ScopedTimer t{ctx, CAT_OTHER};
-        accumulate_kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(sc, pb.li, ctx->d_film, ctx->d_pixel_list, pixel_offset,
-                                                                                  npix, spp, pb.counts, pb.stats);
-    }
+    launch_accumulate(ctx, pixel_list, pixel_offset, npix, spp);
     ctx->stats.kernel_launches++;
     ctx->stats.passes++;
     LRK_CUDA(cudaGetLastError());
@@ -632,6 +649,10 @@ void lrk_destroy(lrk_ctx *ctx) {
     if (ctx->d_film) cudaFree(ctx->d_film);
     if (ctx->d_film_out) cudaFree(ctx->d_film_out);
     if (ctx->d_query_cursor) cudaFree(ctx->d_query_cursor);
+    for (void *p : {static_cast<void *>(ctx->d_moments), static_cast<void *>(ctx->d_sample_counts), static_cast<void *>(ctx->d_active[0]),
+                    static_cast<void *>(ctx->d_active[1]), static_cast<void *>(ctx->d_block_start[0]), static_cast<void *>(ctx->d_block_start[1]),
+                    static_cast<void *>(ctx->d_block_start[2]), static_cast<void *>(ctx->d_keep), ctx->d_scan_temp})
+        if (p) cudaFree(p);
     for (auto &t : ctx->timed) {
         cudaEventDestroy(t.start);
         cudaEventDestroy(t.stop);
@@ -1042,41 +1063,51 @@ int lrk_film_clear(lrk_ctx *ctx) {
     if (ctx->pb.stats) LRK_CUDA(cudaMemsetAsync(ctx->pb.stats, 0, 8u * sizeof(unsigned long long), ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     ctx->stats = lrk_stats{};
+    ctx->adaptive_valid = false;
     return LRK_OK;
 }
 
-int lrk_render(lrk_ctx *ctx, uint32_t spp_begin, uint32_t spp_end) {
-    if (!ctx || !ctx->has_scene) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_render: no scene");
-    if (spp_end < spp_begin) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_render: spp_end < spp_begin");
-    LRK_CUDA(cudaSetDevice(ctx->device));
-    const uint32_t npix = ctx->npix_owned;
-    if (npix == 0u || spp_end == spp_begin) return LRK_OK;
+// Pass sizing of a render over npix pixels: chunks of whole pixels, one sample each, when the pixels alone exceed
+// max_paths_per_pass; else all the pixels with as many samples per pixel as fit.
+struct PassShape {
+    uint32_t chunk_pix, spp_per_pass;
+};
+
+static PassShape pass_shape(const lrk_ctx *ctx, uint32_t npix, uint32_t total_spp) {
     const uint64_t max_paths = std::max<uint64_t>(ctx->max_paths, 1024u);
+    PassShape sh{npix, 1u};
+    if (npix > max_paths) sh.chunk_pix = static_cast<uint32_t>(max_paths);
+    else sh.spp_per_pass = static_cast<uint32_t>(std::min<uint64_t>(total_spp, max_paths / npix));
+    return sh;
+}
+
+// Sample indices [spp_begin, spp_end) of the pixels list[0 .. npix), in passes of the given shape (path state already allocated).
+static int render_passes(lrk_ctx *ctx, const uint32_t *list, uint32_t npix, uint32_t spp_begin, uint32_t spp_end, PassShape sh) {
     const uint32_t total_spp = spp_end - spp_begin;
-    uint32_t chunk_pix = npix, spp_per_pass = 1u;
-    if (npix > max_paths) chunk_pix = static_cast<uint32_t>(max_paths);
-    else spp_per_pass = static_cast<uint32_t>(std::min<uint64_t>(total_spp, max_paths / npix));
-    int rc = alloc_paths(ctx, static_cast<uint64_t>(chunk_pix) * spp_per_pass);
-    if (rc) return rc;
-    LRK_CUDA(cudaEventRecord(ctx->ev_begin, ctx->stream));
-    for (uint32_t s = 0; s < total_spp; s += spp_per_pass) {
-        uint32_t spp = std::min(spp_per_pass, total_spp - s);
-        for (uint32_t p = 0; p < npix; p += chunk_pix) {
-            uint32_t np = std::min(chunk_pix, npix - p);
-            rc = ctx->volume ? render_pass_volume(ctx, p, np, spp_begin + s, spp) : render_pass(ctx, p, np, spp_begin + s, spp);
+    for (uint32_t s = 0; s < total_spp; s += sh.spp_per_pass) {
+        uint32_t spp = std::min(sh.spp_per_pass, total_spp - s);
+        for (uint32_t p = 0; p < npix; p += sh.chunk_pix) {
+            uint32_t np = std::min(sh.chunk_pix, npix - p);
+            int rc = ctx->volume ? render_pass_volume(ctx, list, p, np, spp_begin + s, spp) : render_pass(ctx, list, p, np, spp_begin + s, spp);
             if (rc) return rc;
         }
     }
+    return LRK_OK;
+}
+
+// The end of a render timed from ctx->ev_begin: waits for the stream, reports the kernels' overflow flags, and adds the device
+// time, the kernel-category times and the samples to the stats.
+static int finish_render(lrk_ctx *ctx, const std::string &what, uint64_t samples) {
     LRK_CUDA(cudaEventRecord(ctx->ev_end, ctx->stream));
     LRK_CUDA(cudaMemcpyAsync(&ctx->h_overflow, ctx->scene.traversal_overflow, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     LRK_CUDA(cudaGetLastError());
-    if (ctx->h_overflow & 2u) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_render: a path was inside more than 8 media at once (medium tracker overflow)");
-    if (ctx->h_overflow != 0u) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_render: traversal stack overflow (BVH deeper than the kernels support)");
+    if (ctx->h_overflow & 2u) return fail(ctx, LRK_ERR_UNSUPPORTED, what + ": a path was inside more than 8 media at once (medium tracker overflow)");
+    if (ctx->h_overflow != 0u) return fail(ctx, LRK_ERR_UNSUPPORTED, what + ": traversal stack overflow (BVH deeper than the kernels support)");
     float ms = 0.f;
     LRK_CUDA(cudaEventElapsedTime(&ms, ctx->ev_begin, ctx->ev_end));
     ctx->stats.render_ms += ms;
-    ctx->stats.samples += static_cast<uint64_t>(npix) * total_spp;
+    ctx->stats.samples += samples;
     for (auto &t : ctx->timed) {
         float kms = 0.f;
         cudaEventElapsedTime(&kms, t.start, t.stop);
@@ -1089,6 +1120,142 @@ int lrk_render(lrk_ctx *ctx, uint32_t spp_begin, uint32_t spp_end) {
         ctx->event_pool.push_back(t.stop);
     }
     ctx->timed.clear();
+    return LRK_OK;
+}
+
+int lrk_render(lrk_ctx *ctx, uint32_t spp_begin, uint32_t spp_end) {
+    if (!ctx || !ctx->has_scene) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_render: no scene");
+    if (spp_end < spp_begin) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_render: spp_end < spp_begin");
+    LRK_CUDA(cudaSetDevice(ctx->device));
+    const uint32_t npix = ctx->npix_owned;
+    if (npix == 0u || spp_end == spp_begin) return LRK_OK;
+    ctx->adaptive_valid = false;// the film no longer holds what the sample counts describe
+    const PassShape sh = pass_shape(ctx, npix, spp_end - spp_begin);
+    int rc = alloc_paths(ctx, static_cast<uint64_t>(sh.chunk_pix) * sh.spp_per_pass);
+    if (rc) return rc;
+    LRK_CUDA(cudaEventRecord(ctx->ev_begin, ctx->stream));
+    if ((rc = render_passes(ctx, ctx->d_pixel_list, npix, spp_begin, spp_end, sh))) return rc;
+    return finish_render(ctx, "lrk_render", static_cast<uint64_t>(npix) * (spp_end - spp_begin));
+}
+
+// Buffers of the adaptive mode, grown to the film / pixel list / block count of this context; clears the moments and counts.
+static int alloc_adaptive(lrk_ctx *ctx) {
+    const size_t pixels = ctx->film_pixels, list = std::max<size_t>(ctx->npix_owned, 1u), blocks = ctx->block_start.size();
+    auto grow = [&](void **p, size_t &have, size_t need, size_t bytes_each) -> int {
+        if (*p != nullptr && have >= need) return LRK_OK;
+        if (*p) cudaFree(*p);
+        *p = nullptr;
+        LRK_CUDA(cudaMalloc(p, need * bytes_each));
+        return LRK_OK;
+    };
+    int rc;
+    size_t have = ctx->adaptive_pixels;
+    if ((rc = grow(reinterpret_cast<void **>(&ctx->d_moments), have, pixels, sizeof(float2)))) return rc;
+    if ((rc = grow(reinterpret_cast<void **>(&ctx->d_sample_counts), have, pixels, sizeof(uint32_t)))) return rc;
+    ctx->adaptive_pixels = std::max(have, pixels);
+    have = ctx->adaptive_list;
+    for (auto &p : ctx->d_active)
+        if ((rc = grow(reinterpret_cast<void **>(&p), have, list, sizeof(uint32_t)))) return rc;
+    ctx->adaptive_list = std::max(have, list);
+    have = ctx->adaptive_blocks;
+    for (auto &p : ctx->d_block_start)
+        if ((rc = grow(reinterpret_cast<void **>(&p), have, blocks, sizeof(uint32_t)))) return rc;
+    if ((rc = grow(reinterpret_cast<void **>(&ctx->d_keep), have, blocks, 2u * sizeof(unsigned long long)))) return rc;
+    ctx->adaptive_blocks = std::max(have, blocks);
+    size_t temp = 0u;
+    cub::DeviceScan::ExclusiveSum(nullptr, temp, ctx->d_keep, ctx->d_keep + blocks, static_cast<int>(blocks), ctx->stream);
+    if ((rc = grow(&ctx->d_scan_temp, ctx->scan_temp_bytes, temp, 1u))) return rc;
+    ctx->scan_temp_bytes = std::max(ctx->scan_temp_bytes, temp);
+    LRK_CUDA(cudaMemsetAsync(ctx->d_moments, 0, pixels * sizeof(float2), ctx->stream));
+    LRK_CUDA(cudaMemsetAsync(ctx->d_sample_counts, 0, pixels * sizeof(uint32_t), ctx->stream));
+    LRK_CUDA(cudaMemcpyAsync(ctx->d_block_start[0], ctx->block_start.data(), blocks * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));// block_start is pageable host memory
+    return LRK_OK;
+}
+
+// Schedule and rule: include/lrk.h and DESIGN.md §4 (Adaptive sampling).  Every round renders [c, next) for the active list (pass sizing of
+// lrk_render, applied to the active pixel count), then adaptive_test_kernel stops the blocks below the threshold and the rest are
+// compacted into the next list; one 8-byte read-back per round tells the host how many pixels and blocks are left.
+int lrk_render_adaptive(lrk_ctx *ctx, const lrk_adaptive *p) {
+    if (!ctx || !ctx->has_scene) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_render_adaptive: no scene");
+    if (!p || p->min_spp < 2u || p->max_spp < p->min_spp || !(p->threshold >= 0.f) || !std::isfinite(p->threshold))
+        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_render_adaptive: needs 2 <= min_spp <= max_spp and a finite threshold >= 0");
+    int rc = lrk_film_clear(ctx);
+    if (rc) return rc;
+    if ((rc = alloc_adaptive(ctx))) return rc;
+    const uint32_t npix = ctx->npix_owned;
+    if (npix == 0u) {
+        ctx->adaptive_valid = true;
+        return LRK_OK;
+    }
+    struct MomentsOn {// the film accumulation adds the moments for the duration of this call only
+        lrk_ctx *ctx;
+        ~MomentsOn() { ctx->pass_moments = nullptr; }
+    } moments_on{ctx};
+    ctx->pass_moments = ctx->d_moments;
+    const uint32_t *list = ctx->d_pixel_list;
+    const uint32_t *blocks = ctx->d_block_start[0];
+    uint32_t active = npix, nblocks = static_cast<uint32_t>(ctx->block_start.size() - 1u), c = 0u, next = p->min_spp;
+    unsigned long long *keep = ctx->d_keep, *offsets = ctx->d_keep + ctx->adaptive_blocks;
+    uint64_t samples = 0u;
+    bool timing = false;
+    for (uint32_t round = 0u;; round++) {
+        const PassShape sh = pass_shape(ctx, active, next - c);
+        if ((rc = alloc_paths(ctx, static_cast<uint64_t>(sh.chunk_pix) * sh.spp_per_pass))) return rc;
+        if (!timing) {
+            LRK_CUDA(cudaEventRecord(ctx->ev_begin, ctx->stream));
+            timing = true;
+        }
+        if ((rc = render_passes(ctx, list, active, c, next, sh))) return rc;
+        samples += static_cast<uint64_t>(active) * (next - c);
+        c = next;
+        const bool last = c >= p->max_spp;
+        const unsigned grid = static_cast<unsigned>((static_cast<uint64_t>(nblocks + 1u) * 32u + kAdaptiveBlock - 1u) / kAdaptiveBlock);
+        adaptive_test_kernel<<<grid, kAdaptiveBlock, 0, ctx->stream>>>(ctx->scene.width, ctx->d_film, ctx->d_moments, list, blocks, nblocks, p->threshold,
+                                                                        c, last, ctx->d_sample_counts, keep);
+        ctx->stats.kernel_launches++;
+        if (last) break;
+        size_t temp = ctx->scan_temp_bytes;
+        LRK_CUDA(cub::DeviceScan::ExclusiveSum(ctx->d_scan_temp, temp, keep, offsets, static_cast<int>(nblocks + 1u), ctx->stream));
+        uint32_t *list_out = ctx->d_active[round & 1u], *blocks_out = ctx->d_block_start[1u + (round & 1u)];
+        adaptive_compact_kernel<<<grid, kAdaptiveBlock, 0, ctx->stream>>>(list, blocks, nblocks, keep, offsets, list_out, blocks_out);
+        ctx->stats.kernel_launches += 2u;
+        LRK_CUDA(cudaGetLastError());
+        unsigned long long total = 0ull;
+        LRK_CUDA(cudaMemcpyAsync(&total, offsets + nblocks, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
+        LRK_CUDA(cudaStreamSynchronize(ctx->stream));
+        active = static_cast<uint32_t>(total >> 32u);
+        nblocks = static_cast<uint32_t>(total);
+        if (active == 0u) break;
+        list = list_out;
+        blocks = blocks_out;
+        next = static_cast<uint32_t>(std::min<uint64_t>(2ull * c, p->max_spp));
+    }
+    LRK_CUDA(cudaGetLastError());
+    if ((rc = finish_render(ctx, "lrk_render_adaptive", samples))) return rc;
+    ctx->adaptive_valid = true;
+    return LRK_OK;
+}
+
+int lrk_download_sample_counts(lrk_ctx *ctx, uint32_t *counts) {
+    if (!ctx || !ctx->has_scene || !counts) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_download_sample_counts: no scene / null buffer");
+    if (!ctx->adaptive_valid) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_download_sample_counts: no adaptive render since the last film clear");
+    LRK_CUDA(cudaSetDevice(ctx->device));
+    LRK_CUDA(cudaMemcpyAsync(counts, ctx->d_sample_counts, ctx->film_pixels * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));
+    return LRK_OK;
+}
+
+int lrk_download_film_variance(lrk_ctx *ctx, float *v) {
+    if (!ctx || !ctx->has_scene || !v) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_download_film_variance: no scene / null buffer");
+    if (!ctx->adaptive_valid) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_download_film_variance: no adaptive render since the last film clear");
+    LRK_CUDA(cudaSetDevice(ctx->device));
+    const uint32_t n = static_cast<uint32_t>(ctx->film_pixels);
+    float *out = reinterpret_cast<float *>(ctx->d_film_out);// the staging buffer of lrk_download_film
+    adaptive_variance_kernel<<<(n + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->d_film, ctx->d_moments, ctx->d_sample_counts, out, n);
+    LRK_CUDA(cudaGetLastError());
+    LRK_CUDA(cudaMemcpyAsync(v, out, static_cast<size_t>(n) * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     return LRK_OK;
 }
 

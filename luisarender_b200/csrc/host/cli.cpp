@@ -9,12 +9,16 @@
 // or mpirun launch of the plain command works too) and waits for them.  Every rank parses the scene, renders the tiles it owns
 // (lrk_balance_shards), and one lrk_reduce_film (NCCL) sums the raw films on rank 0, which writes the image.  The NCCL unique id
 // travels through a file (LRK_COMM_ID_FILE, default /tmp/lrk_comm_<MASTER_PORT>.id): rank 0 writes it, the others wait for it.
+//
+// Adaptive sampling (an extension; the reference has none): `--adaptive <threshold>` renders with lrk_render_adaptive, from
+// `--adaptive-min-spp` samples per pixel (default 16, at most the camera's spp) up to the camera's spp.
 #include <sys/stat.h>
 #include <sys/wait.h>
 #include <unistd.h>
 
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -33,6 +37,8 @@ void usage() {
                 "      --scene <file>           Path to scene description file\n"
                 "  -D, --define <key>=<value>   Parameter definitions to override scene description macros.\n"
                 "      --gpus <n>               Render on n GPUs, one process each (tiles sharded, films summed on GPU 0)\n"
+                "      --adaptive <threshold>   Adaptive sampling: stop 8x4 pixel blocks whose relative error is below threshold\n"
+                "      --adaptive-min-spp <n>   Samples per pixel of the first adaptive round (default 16, at most the camera's spp)\n"
                 "  -h, --help                   Display this help message\n");
 }
 
@@ -122,6 +128,7 @@ int launch_ranks(int gpus, int argc, char *argv[]) {
 int main(int argc, char *argv[]) {
     std::string backend, scene_path;
     int device = -1, gpus = 1;
+    std::string adaptive_arg, min_spp_arg;
     std::vector<std::string> keys, values;
     auto add_macro = [&](const std::string &d) {
         auto p = d.find('=');
@@ -158,6 +165,10 @@ int main(int argc, char *argv[]) {
         else if (a == "--scene") scene_path = need("file");
         else if (a == "--gpus") gpus = std::atoi(need("count").c_str());
         else if (a.rfind("--gpus=", 0) == 0) gpus = std::atoi(a.substr(7).c_str());
+        else if (a == "--adaptive") adaptive_arg = need("threshold");
+        else if (a.rfind("--adaptive=", 0) == 0) adaptive_arg = a.substr(11);
+        else if (a == "--adaptive-min-spp") min_spp_arg = need("count");
+        else if (a.rfind("--adaptive-min-spp=", 0) == 0) min_spp_arg = a.substr(19);
         else if (a == "-D" || a == "--define") add_macro(need("definition"));
         else if (a.rfind("-D", 0) == 0) add_macro(a.substr(2));
         else if (!a.empty() && a[0] == '-') std::fprintf(stderr, "[warning] Unrecognized options: %s\n", a.c_str());
@@ -172,6 +183,27 @@ int main(int argc, char *argv[]) {
         std::fprintf(stderr, "[warning] Failed to parse command line arguments: Option 'backend' has no value.\n");
         usage();
         return -1;
+    }
+    // the adaptive options are checked here, before the scene is read or a device is touched
+    const bool adaptive = !adaptive_arg.empty();
+    float threshold = 0.f;
+    uint32_t min_spp = 16u;
+    if (adaptive) {
+        char *end = nullptr;
+        threshold = std::strtof(adaptive_arg.c_str(), &end);
+        if (end == adaptive_arg.c_str() || *end != '\0' || !std::isfinite(threshold) || threshold < 0.f) {
+            std::fprintf(stderr, "[error] --adaptive takes a finite threshold >= 0, not '%s'.\n", adaptive_arg.c_str());
+            return -1;
+        }
+    }
+    if (!min_spp_arg.empty()) {
+        char *end = nullptr;
+        const unsigned long v = std::strtoul(min_spp_arg.c_str(), &end, 10);
+        if (!adaptive || end == min_spp_arg.c_str() || *end != '\0' || min_spp_arg[0] == '-' || v < 2ul || v > 0xffffffffull) {
+            std::fprintf(stderr, "[error] --adaptive-min-spp takes a count >= 2 and needs --adaptive, not '%s'.\n", min_spp_arg.c_str());
+            return -1;
+        }
+        min_spp = static_cast<uint32_t>(v);
     }
     for (auto &c : backend) c = static_cast<char>(std::tolower(static_cast<unsigned char>(c)));
     if (backend != "cuda") die("Backend '" + backend + "' is not available: this build ships the sm_90a CUDA backend only (-b cuda).");
@@ -226,10 +258,27 @@ int main(int argc, char *argv[]) {
         const uint32_t w = desc.camera.resolution[0], h = desc.camera.resolution[1], spp = desc.camera.spp;
         std::printf("[info] Wavefront path tracing configurations: resolution = %ux%u, spp = %u.\n", w, h, spp);
         std::printf("[info] Rendering started.\n");
-        if (lrk_render(ctx, 0u, spp) != 0) die(lrk_last_error(ctx));
+        const lrk_adaptive ap{std::min(min_spp, spp), spp, threshold, 0u};
+        if (adaptive ? lrk_render_adaptive(ctx, &ap) != 0 : lrk_render(ctx, 0u, spp) != 0) die(lrk_last_error(ctx));
         if (world > 1u && lrk_reduce_film(ctx, 0u) != 0) die(lrk_last_error(ctx));
         lrk_stats st{};
         lrk_get_stats(ctx, &st);
+        if (adaptive) {// this rank's pixels: samples against a uniform render, and the rounds it took (counts are min_spp * 2^k or spp)
+            std::vector<uint32_t> counts(static_cast<size_t>(w) * h);
+            if (lrk_download_sample_counts(ctx, counts.data()) != 0) die(lrk_last_error(ctx));
+            uint64_t owned = 0u;
+            uint32_t top = 0u;
+            for (uint32_t c : counts) {
+                owned += c != 0u ? 1u : 0u;
+                top = std::max(top, c);
+            }
+            uint32_t rounds = 1u;
+            for (uint32_t level = ap.min_spp; level < top; level = static_cast<uint32_t>(std::min<uint64_t>(2ull * level, spp))) rounds++;
+            const std::string who = world > 1u ? "Rank " + std::to_string(rank) + ": a" : "A";
+            std::printf("[info] %sdaptive sampling (threshold %g, %u to %u spp): %llu samples, %.2f %% of a uniform render, %u rounds.\n", who.c_str(),
+                        static_cast<double>(threshold), ap.min_spp, spp, static_cast<unsigned long long>(st.samples),
+                        owned != 0u ? 100.0 * static_cast<double>(st.samples) / (static_cast<double>(owned) * spp) : 0.0, rounds);
+        }
         if (world > 1u) std::printf("[info] Rank %u rendered its tiles in %.3f ms (film reduce %.3f ms).\n", rank, st.render_ms, st.reduce_ms);
         if (!root) continue;
         std::printf("[info] Rendering finished in %.3f ms.\n", st.render_ms + st.reduce_ms);
