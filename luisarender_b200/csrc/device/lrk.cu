@@ -7,7 +7,9 @@
 #include <cstdio>
 #include <cstring>
 #include <limits>
+#include <memory>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -22,9 +24,42 @@ using namespace lrk;
 
 namespace {
 
+// Owner of one device allocation of the context, sized exactly to the largest request so far.  reserve() keeps the allocation when
+// it is large enough; otherwise it frees it before allocating the new size, so that growing a buffer never holds both (the path
+// state of one pass is tens of GB).
+class DeviceBuffer {
+public:
+    DeviceBuffer() = default;
+    DeviceBuffer(DeviceBuffer &&o) noexcept : ptr_{o.ptr_}, bytes_{o.bytes_} {
+        o.ptr_ = nullptr;
+        o.bytes_ = 0u;
+    }
+    ~DeviceBuffer() { release(); }
+    cudaError_t reserve(size_t bytes) {
+        if (ptr_ != nullptr && bytes_ >= bytes) return cudaSuccess;
+        release();
+        const cudaError_t e = cudaMalloc(&ptr_, bytes);
+        if (e != cudaSuccess) ptr_ = nullptr;
+        else bytes_ = bytes;
+        return e;
+    }
+    void release() {
+        if (ptr_ != nullptr) cudaFree(ptr_);
+        ptr_ = nullptr;
+        bytes_ = 0u;
+    }
+    template<typename T = void>
+    T *get() const { return static_cast<T *>(ptr_); }
+    size_t bytes() const { return bytes_; }
+
+private:
+    void *ptr_{nullptr};
+    size_t bytes_{0u};
+};
+
 struct DeviceArrays {
-    void *vertices{}, *triangles{}, *alias{}, *pdf{}, *meshes{}, *inst_handles{}, *inst_kind{}, *inst_o2w{}, *inst_xform{}, *bvh_nodes{}, *traversal_overflow{}, *sobol{}, *vdc{}, *vdc_inv{}, *pmj{}, *blue_noise{}, *pmj_pixels{}, *zsobol_hash{}, *sampler{}, *build_scratch{}, *mesh_bounds{}, *inst_mesh{}, *visible_ids{}, *scene_copy{}, *media{}, *textures{}, *texels{}, *env_alias{}, *env_pdf{},
-        *tri_verts{}, *surfaces{}, *lights{}, *light_handles{}, *camera{};
+    DeviceBuffer vertices, triangles, alias, pdf, meshes, inst_handles, inst_kind, inst_o2w, inst_xform, bvh_nodes, traversal_overflow, sobol, vdc, vdc_inv, pmj, blue_noise, pmj_pixels, zsobol_hash, sampler, build_scratch, mesh_bounds, inst_mesh, visible_ids, scene_copy, media, textures, texels, env_alias, env_pdf,
+        tri_verts, surfaces, lights, light_handles, camera;
 };
 
 enum KernelCategory { CAT_TRACE_CLOSEST = 0, CAT_TRACE_SHADOW = 1, CAT_SHADE = 2, CAT_OTHER = 3, CAT_COUNT = 4 };
@@ -47,23 +82,21 @@ struct lrk_ctx {
     uint32_t spp_hint{0};
     // sharding
     uint32_t rank{0}, world{1}, tile_size{32};
-    uint32_t *d_pixel_list{nullptr};
+    DeviceBuffer d_pixel_list;
     uint32_t npix_owned{0};
     uint32_t pixel_list_key[6]{0, 0, 0, 0, 0, 0};// width, height, rank, world, tile size, owner-table version of the cached list
     uint32_t tile_owner_version{0};// bumped whenever tile_owner changes
     uint32_t *probe_cost{nullptr};// device counters of a running lrk_balance_shards probe
     std::vector<uint32_t> tile_owner;// lrk_balance_shards: owner of every tile (empty: the static lrk_tile_owner map)
-    std::unordered_map<void **, size_t> array_bytes;// capacity of each scene array allocation
     bool textured{false};// some surface has image-textured parameters or a normal map: the shade kernels' TEXTURED variants run
     bool any_non_opaque{false};// some instance carries LRK_SHAPE_MAYBE_NON_OPAQUE: traversal runs its alpha-testing variants
     size_t film_pixels{0};
     // path state
     uint64_t max_paths{0}, capacity{0};
     PathBuffers pb{};
-    std::vector<void *> path_allocs;
-    float4 *d_film{nullptr};
-    float4 *d_film_out{nullptr};
-    uint32_t *d_query_cursor{nullptr};
+    std::vector<DeviceBuffer> path_allocs;// one allocation per array of pb
+    DeviceBuffer d_film, d_film_out;
+    DeviceBuffer d_query_cursor;
     // options
     bool count_traversal{false}, time_kernels{false};
     bool device_bvh{false};// option device_bvh: build the hierarchy on the GPU (bvh_build.cuh) instead of uploading the host's
@@ -93,14 +126,15 @@ struct lrk_ctx {
     // adaptive mode (lrk_render_adaptive); the device buffers are allocated on its first call
     std::vector<uint32_t> block_start;// offsets of the 8x4 pixel blocks in the pixel list, closed by npix_owned (build_pixel_list)
     float2 *pass_moments{nullptr};// set while lrk_render_adaptive runs: the film accumulation also adds the luminance moments here
-    float2 *d_moments{nullptr};
-    uint32_t *d_sample_counts{nullptr};
-    uint32_t *d_active[2]{nullptr, nullptr};// ping-pong active pixel lists of the rounds after the first
-    uint32_t *d_block_start[3]{nullptr, nullptr, nullptr};// [0]: block_start; [1], [2]: the ping-pong lists' blocks
-    unsigned long long *d_keep{nullptr};// keep words and their exclusive scan (adaptive.cuh), 2 x (blocks + 1)
-    void *d_scan_temp{nullptr};
-    size_t scan_temp_bytes{0}, adaptive_pixels{0}, adaptive_list{0}, adaptive_blocks{0};// capacities of the buffers above
+    DeviceBuffer d_moments;
+    DeviceBuffer d_sample_counts;
+    DeviceBuffer d_active[2];// ping-pong active pixel lists of the rounds after the first
+    DeviceBuffer d_block_start[3];// [0]: block_start; [1], [2]: the ping-pong lists' blocks
+    DeviceBuffer d_keep;// keep words and their exclusive scan (adaptive.cuh), 2 x (blocks + 1)
+    DeviceBuffer d_scan_temp;
     bool adaptive_valid{false};// the film is the result of an adaptive render: sample counts and variance can be downloaded
+
+    ~lrk_ctx();
 };
 
 namespace {
@@ -143,84 +177,61 @@ void unpin_all(lrk_ctx *ctx) {
 // Host -> device copy of one scene array.  The allocation is kept across uploads when it is large enough, so
 // re-uploading a scene of the same shape (the end-to-end path of bench.py, animation frames) costs only the copy.
 template<typename T>
-int upload(lrk_ctx *ctx, void **dst, const T *src, size_t count) {
-    size_t bytes = std::max<size_t>(count * sizeof(T), 16u);
-    size_t &have = ctx->array_bytes[dst];
-    if (*dst == nullptr || have < bytes) {
-        if (*dst) {
-            cudaFree(*dst);
-            *dst = nullptr;
-        }
-        LRK_CUDA(cudaMalloc(dst, bytes));
-        have = bytes;
-    }
+int upload(lrk_ctx *ctx, DeviceBuffer &dst, const T *src, size_t count) {
+    LRK_CUDA(dst.reserve(std::max<size_t>(count * sizeof(T), 16u)));
     if (count) {
         pin_range(ctx, src, count * sizeof(T));
-        LRK_CUDA(cudaMemcpyAsync(*dst, src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+        LRK_CUDA(cudaMemcpyAsync(dst.get(), src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
     }
     return LRK_OK;
-}
-
-void free_arrays(DeviceArrays &a) {
-    void **p = reinterpret_cast<void **>(&a);
-    for (size_t i = 0; i < sizeof(DeviceArrays) / sizeof(void *); i++) {
-        if (p[i]) cudaFree(p[i]);
-        p[i] = nullptr;
-    }
-}
-
-void free_paths(lrk_ctx *ctx) {
-    for (auto p : ctx->path_allocs) cudaFree(p);
-    ctx->path_allocs.clear();
-    ctx->pb = PathBuffers{};// no dangling pointers: lrk_film_clear / lrk_get_stats look at pb.stats
-    ctx->capacity = 0;
-    ctx->volume_capacity = 0;
-    ctx->allocated_kinds = 0u;
 }
 
 int alloc_paths(lrk_ctx *ctx, uint64_t capacity) {
     uint32_t kinds = 0u;
     for (int k = 0; k < static_cast<int>(kHitKinds); k++) if (k < 3 || ctx->has_kind[k]) kinds |= 1u << k;// buckets 3..10 only for scenes that use them
     if (ctx->capacity >= capacity && (!ctx->volume || ctx->volume_capacity >= capacity) && (ctx->allocated_kinds & kinds) == kinds) return LRK_OK;
-    free_paths(ctx);
-    auto alloc = [&](void **p, size_t bytes) -> cudaError_t {
-        cudaError_t e = cudaMalloc(p, bytes);
-        if (e == cudaSuccess) ctx->path_allocs.push_back(*p);
+    // all of the old path state is freed before any of the new one is allocated
+    ctx->path_allocs.clear();
+    ctx->pb = PathBuffers{};// no dangling pointers: lrk_film_clear / lrk_get_stats look at pb.stats
+    ctx->capacity = 0;
+    ctx->volume_capacity = 0;
+    ctx->allocated_kinds = 0u;
+    auto alloc = [&](auto *&p, size_t count) {
+        ctx->path_allocs.emplace_back();
+        const cudaError_t e = ctx->path_allocs.back().reserve(count * sizeof(*p));
+        p = ctx->path_allocs.back().get<std::remove_reference_t<decltype(*p)>>();
         return e;
     };
     auto &pb = ctx->pb;
     for (int k = 0; k < 2; k++) {
-        LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.ray_o[k]), capacity * sizeof(float4)));
-        LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.ray_d[k]), capacity * sizeof(float4)));
-        LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.beta_pdf[k]), capacity * sizeof(float4)));
-        LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.id_rng[k]), capacity * sizeof(uint2)));
+        LRK_CUDA(alloc(pb.ray_o[k], capacity));
+        LRK_CUDA(alloc(pb.ray_d[k], capacity));
+        LRK_CUDA(alloc(pb.beta_pdf[k], capacity));
+        LRK_CUDA(alloc(pb.id_rng[k], capacity));
     }
-    LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.hit), capacity * sizeof(uint4)));
-    for (int k = 0; k < static_cast<int>(kHitKinds); k++) {
-        pb.hit_index[k] = nullptr;
-        if (kinds & (1u << k)) LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.hit_index[k]), capacity * sizeof(uint32_t)));
-    }
+    LRK_CUDA(alloc(pb.hit, capacity));
+    for (int k = 0; k < static_cast<int>(kHitKinds); k++)
+        if (kinds & (1u << k)) LRK_CUDA(alloc(pb.hit_index[k], capacity));
     ctx->allocated_kinds = kinds;
-    LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.sray_o), capacity * sizeof(float4)));
-    LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.sray_d), capacity * sizeof(float4)));
-    LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.scontrib), capacity * sizeof(float4)));
-    LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.li), capacity * sizeof(float4)));
-    LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.counts), kCountSlots * kMaxDepthSlots * sizeof(uint32_t)));
+    LRK_CUDA(alloc(pb.sray_o, capacity));
+    LRK_CUDA(alloc(pb.sray_d, capacity));
+    LRK_CUDA(alloc(pb.scontrib, capacity));
+    LRK_CUDA(alloc(pb.li, capacity));
+    LRK_CUDA(alloc(pb.counts, kCountSlots * kMaxDepthSlots));
     pb.capacity = static_cast<uint32_t>(capacity);
-    LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.stats), 8u * sizeof(unsigned long long)));
+    LRK_CUDA(alloc(pb.stats, 8u));
     LRK_CUDA(cudaMemsetAsync(pb.stats, 0, 8u * sizeof(unsigned long long), ctx->stream));
     ctx->capacity = capacity;
-    ctx->volume_capacity = 0;
     if (ctx->volume) {
         for (int k = 0; k < 2; k++) {
-            LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.pcg[k]), capacity * sizeof(ulonglong2)));
-            LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.u_rr[k]), capacity * sizeof(float)));
-            LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.occl2[k]), capacity * sizeof(uint32_t)));
+            LRK_CUDA(alloc(pb.pcg[k], capacity));
+            LRK_CUDA(alloc(pb.u_rr[k], capacity));
+            LRK_CUDA(alloc(pb.occl2[k], capacity));
         }
-        LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.s1ray_o), capacity * sizeof(float4)));
-        LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.s1ray_d), capacity * sizeof(float4)));
-        LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.occl1), capacity * sizeof(uint32_t)));
-        LRK_CUDA(alloc(reinterpret_cast<void **>(&pb.s2_target), capacity * sizeof(uint32_t)));
+        LRK_CUDA(alloc(pb.s1ray_o, capacity));
+        LRK_CUDA(alloc(pb.s1ray_d, capacity));
+        LRK_CUDA(alloc(pb.occl1, capacity));
+        LRK_CUDA(alloc(pb.s2_target, capacity));
         ctx->volume_capacity = capacity;
     }
     return LRK_OK;
@@ -231,7 +242,7 @@ int alloc_paths(lrk_ctx *ctx, uint64_t capacity) {
 int build_pixel_list(lrk_ctx *ctx) {
     const uint32_t W = ctx->scene.width, H = ctx->scene.height, ts = ctx->tile_size;
     const uint32_t key[6]{W, H, ctx->rank, ctx->world, ts, ctx->tile_owner.empty() ? 0u : ctx->tile_owner_version};
-    if (ctx->d_pixel_list != nullptr && std::memcmp(key, ctx->pixel_list_key, sizeof(key)) == 0) return LRK_OK;
+    if (ctx->d_pixel_list.get() != nullptr && std::memcmp(key, ctx->pixel_list_key, sizeof(key)) == 0) return LRK_OK;
     std::memcpy(ctx->pixel_list_key, key, sizeof(key));
     const uint32_t tiles_x = (W + ts - 1u) / ts, tiles_y = (H + ts - 1u) / ts;
     std::vector<uint32_t> list;
@@ -253,13 +264,9 @@ int build_pixel_list(lrk_ctx *ctx) {
         }
     }
     ctx->block_start.push_back(static_cast<uint32_t>(list.size()));
-    if (ctx->d_pixel_list) {
-        cudaFree(ctx->d_pixel_list);
-        ctx->d_pixel_list = nullptr;
-    }
     ctx->npix_owned = static_cast<uint32_t>(list.size());
-    LRK_CUDA(cudaMalloc(reinterpret_cast<void **>(&ctx->d_pixel_list), std::max<size_t>(list.size(), 4u) * sizeof(uint32_t)));
-    LRK_CUDA(cudaMemcpyAsync(ctx->d_pixel_list, list.data(), list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    LRK_CUDA(ctx->d_pixel_list.reserve(std::max<size_t>(list.size(), 4u) * sizeof(uint32_t)));
+    LRK_CUDA(cudaMemcpyAsync(ctx->d_pixel_list.get(), list.data(), list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     return LRK_OK;
 }
@@ -300,20 +307,39 @@ int blocks_for(lrk_ctx *ctx, uint64_t n, int persistent_grid) {
     return static_cast<int>(std::max<uint64_t>(1u, std::min<uint64_t>(need, static_cast<uint64_t>(persistent_grid))));
 }
 
+// Every traversal kernel family is launched from one place, which also picks its instantiation: traversal counters (option
+// count_traversal) or any-hit queries x the stochastic alpha test (scenes with non-opaque surfaces).  The kernels are named directly
+// rather than through a generic lambda, so that they are instantiated in source order and the cubin's function order stays put.
 void launch_query(lrk_ctx *ctx, int g, bool any_hit, const float4 *d_rays, uint4 *d_hits, uint32_t n) {
-    auto launch = [&](auto kernel) { kernel<<<g, kTraceBlock, 0, ctx->stream>>>(ctx->scene, d_rays, d_hits, n, ctx->d_query_cursor); };
-    if (ctx->any_non_opaque) any_hit ? launch(trace_query_kernel<true, true>) : launch(trace_query_kernel<false, true>);
-    else any_hit ? launch(trace_query_kernel<true, false>) : launch(trace_query_kernel<false, false>);
+    const auto kernel = ctx->any_non_opaque ? (any_hit ? trace_query_kernel<true, true> : trace_query_kernel<false, true>)
+                                            : (any_hit ? trace_query_kernel<true, false> : trace_query_kernel<false, false>);
+    kernel<<<g, kTraceBlock, 0, ctx->stream>>>(ctx->scene, d_rays, d_hits, n, ctx->d_query_cursor.get<uint32_t>());
 }
+
+// stats.kernel_launches counts the kernels of lrk_render and lrk_render_adaptive (a cub call counts as one): each launch there adds
+// itself where it is issued.
 
 // The film accumulation of a pass; with the adaptive mode's moments while lrk_render_adaptive runs.
 void launch_accumulate(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp) {
     ScopedTimer t{ctx, CAT_OTHER};
-    auto launch = [&](auto kernel) {
-        kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->scene, ctx->pb.li, ctx->d_film, pixel_list, pixel_offset, npix, spp,
-                                                                        ctx->pb.counts, ctx->pb.stats, ctx->pass_moments);
-    };
-    ctx->pass_moments != nullptr ? launch(accumulate_kernel<true>) : launch(accumulate_kernel<false>);
+    const auto kernel = ctx->pass_moments != nullptr ? accumulate_kernel<true> : accumulate_kernel<false>;
+    kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->scene, ctx->pb.li, ctx->d_film.get<float4>(), pixel_list, pixel_offset, npix, spp,
+                                                                    ctx->pb.counts, ctx->pb.stats, ctx->pass_moments);
+    ctx->stats.kernel_launches++;
+}
+
+// Closest-hit traversal of the path queue of `depth`.  The volume pass launches it with alpha = false: the volume integrator rejects
+// non-opaque surfaces at upload.
+void launch_trace_closest(lrk_ctx *ctx, bool alpha, uint64_t n, uint32_t depth) {
+    ScopedTimer t{ctx, CAT_TRACE_CLOSEST};
+    const auto &pb = ctx->pb;
+    const bool count = ctx->count_traversal;
+    const auto kernel = alpha ? (count ? trace_closest_kernel<true, true> : trace_closest_kernel<false, true>)
+                              : (count ? trace_closest_kernel<true, false> : trace_closest_kernel<false, false>);
+    const int in = depth & 1u;
+    kernel<<<blocks_for(ctx, n, ctx->grid_trace), kTraceBlock, 0, ctx->stream>>>(ctx->scene, pb.ray_o[in], pb.ray_d[in], pb.hit, pb.counts + depth,
+                                                                                 pb.counts + 2u * kMaxDepthSlots + depth, pb.stats);
+    ctx->stats.kernel_launches++;
 }
 
 // One pass: sample indices [spp_begin, spp_begin + spp) of the pixels pixel_list[pixel_offset .. pixel_offset + npix).
@@ -332,26 +358,19 @@ int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset,
         ScopedTimer t{ctx, CAT_OTHER};
         generate_rays_kernel<<<static_cast<unsigned>((n + kBlock - 1u) / kBlock), kBlock, 0, ctx->stream>>>(
             sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
+        ctx->stats.kernel_launches++;
     }
-    ctx->stats.kernel_launches++;
     // upper bound of the live queue at depth d is n; launch persistent-size grids and let kernels read *count
     for (uint32_t depth = 0; depth < sc.max_depth; depth++) {
-        const int in = depth & 1u;
-        {
-            ScopedTimer t{ctx, CAT_TRACE_CLOSEST};
-            int g = blocks_for(ctx, n, ctx->grid_trace);
-            // four instantiations: traversal counters on/off x stochastic alpha test on/off (scenes with non-opaque surfaces)
-            auto launch = [&](auto kernel) {
-                kernel<<<g, kTraceBlock, 0, ctx->stream>>>(sc, pb.ray_o[in], pb.ray_d[in], pb.hit, pb.counts + depth,
-                                                      pb.counts + 2u * kMaxDepthSlots + depth, pb.stats);
-            };
-            if (ctx->any_non_opaque) ctx->count_traversal ? launch(trace_closest_kernel<true, true>) : launch(trace_closest_kernel<false, true>);
-            else ctx->count_traversal ? launch(trace_closest_kernel<true, false>) : launch(trace_closest_kernel<false, false>);
-        }
+        launch_trace_closest(ctx, ctx->any_non_opaque, n, depth);
         {
             ScopedTimer t{ctx, CAT_SHADE};
-            if (sc.env_present) shade_miss_kernel<<<blocks_for(ctx, n, ctx->grid_classify), kBlock, 0, ctx->stream>>>(sc, pb, depth);
+            if (sc.env_present) {
+                shade_miss_kernel<<<blocks_for(ctx, n, ctx->grid_classify), kBlock, 0, ctx->stream>>>(sc, pb, depth);
+                ctx->stats.kernel_launches++;
+            }
             classify_hits_kernel<<<blocks_for(ctx, n, ctx->grid_classify), kBlock, 0, ctx->stream>>>(sc, pb, depth);
+            ctx->stats.kernel_launches++;
             // one kernel per closure kind over its own hit bucket (shade.cu); TEXTURED variants only for scenes with image-textured
             // parameters / normal maps
             for (uint32_t kind = 0; kind < kHitKinds; kind++) {
@@ -362,22 +381,20 @@ int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset,
                 const int blocks = blocks_for(ctx, n, ctx->grid_shade[strict ? 1 : 0][kind]);
                 if (strict) strict::launch_shade(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
                 else fast::launch_shade(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
+                ctx->stats.kernel_launches++;
             }
         }
         {
             ScopedTimer t{ctx, CAT_TRACE_SHADOW};
-            int g = blocks_for(ctx, n, ctx->grid_shadow);
-            auto launch = [&](auto kernel) {
-                kernel<<<g, kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + kMaxDepthSlots + depth, pb.counts + 3u * kMaxDepthSlots + depth);
-            };
-            if (ctx->any_non_opaque) ctx->count_traversal ? launch(trace_shadow_kernel<true, true>) : launch(trace_shadow_kernel<false, true>);
-            else ctx->count_traversal ? launch(trace_shadow_kernel<true, false>) : launch(trace_shadow_kernel<false, false>);
+            const bool count = ctx->count_traversal;
+            const auto kernel = ctx->any_non_opaque ? (count ? trace_shadow_kernel<true, true> : trace_shadow_kernel<false, true>)
+                                                    : (count ? trace_shadow_kernel<true, false> : trace_shadow_kernel<false, false>);
+            kernel<<<blocks_for(ctx, n, ctx->grid_shadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + kMaxDepthSlots + depth,
+                                                                                         pb.counts + 3u * kMaxDepthSlots + depth);
+            ctx->stats.kernel_launches++;
         }
-        ctx->stats.kernel_launches += 4u + (ctx->has_kind[1] ? 1u : 0u) + (ctx->has_kind[2] ? 1u : 0u) + (ctx->has_kind[3] ? 1u : 0u) + (ctx->has_kind[4] ? 1u : 0u) +
-                                      (ctx->has_kind[5] ? 1u : 0u) + (ctx->has_kind[6] ? 1u : 0u) + (ctx->has_kind[7] ? 1u : 0u) + (ctx->has_kind[8] ? 1u : 0u);
     }
     launch_accumulate(ctx, pixel_list, pixel_offset, npix, spp);
-    ctx->stats.kernel_launches++;
     ctx->stats.passes++;
     LRK_CUDA(cudaGetLastError());
     return LRK_OK;
@@ -392,13 +409,11 @@ int render_pass_volume_general(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_
     {
         ScopedTimer t{ctx, CAT_SHADE};
         const unsigned blocks = static_cast<unsigned>((n + kGeneralBlock - 1u) / kGeneralBlock);
-        auto launch = [&](auto kernel) {
-            kernel<<<blocks, kGeneralBlock, 0, ctx->stream>>>(sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
-        };
-        ctx->any_non_opaque ? launch(volume_general_kernel<true>) : launch(volume_general_kernel<false>);
+        const auto kernel = ctx->any_non_opaque ? volume_general_kernel<true> : volume_general_kernel<false>;
+        kernel<<<blocks, kGeneralBlock, 0, ctx->stream>>>(sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
+        ctx->stats.kernel_launches++;
     }
     launch_accumulate(ctx, pixel_list, pixel_offset, npix, spp);
-    ctx->stats.kernel_launches += 2u;
     ctx->stats.passes++;
     LRK_CUDA(cudaGetLastError());
     return LRK_OK;
@@ -413,55 +428,41 @@ int render_pass_volume(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_
         ScopedTimer t{ctx, CAT_OTHER};
         generate_rays_volume_kernel<<<static_cast<unsigned>((n + kBlock - 1u) / kBlock), kBlock, 0, ctx->stream>>>(
             sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
+        ctx->stats.kernel_launches++;
     }
-    ctx->stats.kernel_launches++;
     for (uint32_t depth = 0; depth < sc.max_depth; depth++) {
-        const int in = depth & 1u, out = in ^ 1;
+        const int out = (depth & 1u) ^ 1;
         {
             ScopedTimer t{ctx, CAT_TRACE_SHADOW};
-            int g = blocks_for(ctx, n, ctx->grid_vshadow);
             // the in-medium shadow rays share the depth's path-queue size; their cursor lives in the shadow-cursor region + 32
-            if (ctx->count_traversal)
-                trace_medium_shadow_kernel<true><<<g, kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + depth, pb.counts + 3u * kMaxDepthSlots + 32u + depth);
-            else
-                trace_medium_shadow_kernel<false><<<g, kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + depth, pb.counts + 3u * kMaxDepthSlots + 32u + depth);
+            const auto kernel = ctx->count_traversal ? trace_medium_shadow_kernel<true> : trace_medium_shadow_kernel<false>;
+            kernel<<<blocks_for(ctx, n, ctx->grid_vshadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + depth, pb.counts + 3u * kMaxDepthSlots + 32u + depth);
+            ctx->stats.kernel_launches++;
         }
-        {
-            ScopedTimer t{ctx, CAT_TRACE_CLOSEST};
-            int g = blocks_for(ctx, n, ctx->grid_trace);
-            if (ctx->count_traversal)
-                trace_closest_kernel<true, false><<<g, kTraceBlock, 0, ctx->stream>>>(sc, pb.ray_o[in], pb.ray_d[in], pb.hit, pb.counts + depth,
-                                                                                 pb.counts + 2u * kMaxDepthSlots + depth, pb.stats);
-            else
-                trace_closest_kernel<false, false><<<g, kTraceBlock, 0, ctx->stream>>>(sc, pb.ray_o[in], pb.ray_d[in], pb.hit, pb.counts + depth,
-                                                                                  pb.counts + 2u * kMaxDepthSlots + depth, pb.stats);
-        }
+        launch_trace_closest(ctx, false, n, depth);
         {
             ScopedTimer t{ctx, CAT_SHADE};
             const int v = ctx->strict_math ? 1 : 0;
             if (v) strict::launch_volume_medium(blocks_for(ctx, n, ctx->grid_vmedium[v]), ctx->stream, sc, pb, depth);
             else fast::launch_volume_medium(blocks_for(ctx, n, ctx->grid_vmedium[v]), ctx->stream, sc, pb, depth);
+            ctx->stats.kernel_launches++;
             for (uint32_t kind = 0; kind < 3u; kind++) {
                 if (kind != 0u && !ctx->has_kind[kind]) continue;
                 const int blocks = blocks_for(ctx, n, ctx->grid_vshade[v][kind]);
                 if (v) strict::launch_volume_surface(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
                 else fast::launch_volume_surface(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
+                ctx->stats.kernel_launches++;
             }
         }
         {
             ScopedTimer t{ctx, CAT_TRACE_SHADOW};
-            int g = blocks_for(ctx, n, ctx->grid_vshadow);
-            if (ctx->count_traversal)
-                trace_volume_nee_kernel<true><<<g, kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + kMaxDepthSlots + depth,
-                                                                             pb.counts + 3u * kMaxDepthSlots + depth, pb.occl2[out]);
-            else
-                trace_volume_nee_kernel<false><<<g, kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + kMaxDepthSlots + depth,
-                                                                              pb.counts + 3u * kMaxDepthSlots + depth, pb.occl2[out]);
+            const auto kernel = ctx->count_traversal ? trace_volume_nee_kernel<true> : trace_volume_nee_kernel<false>;
+            kernel<<<blocks_for(ctx, n, ctx->grid_vshadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + kMaxDepthSlots + depth,
+                                                                                         pb.counts + 3u * kMaxDepthSlots + depth, pb.occl2[out]);
+            ctx->stats.kernel_launches++;
         }
-        ctx->stats.kernel_launches += 5u + (ctx->has_kind[1] ? 1u : 0u) + (ctx->has_kind[2] ? 1u : 0u);
     }
     launch_accumulate(ctx, pixel_list, pixel_offset, npix, spp);
-    ctx->stats.kernel_launches++;
     ctx->stats.passes++;
     LRK_CUDA(cudaGetLastError());
     return LRK_OK;
@@ -490,22 +491,11 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
     nodes += std::max<uint64_t>(visible.size(), 2u) - 1u;
     if (nodes >= 0x7fffffffull || s->triangle_count >= (1ull << 28)) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: scene too large for the BVH encoding");
     int rc;
-    if ((rc = upload(ctx, &a.bvh_nodes, static_cast<const lrk_bvh_node *>(nullptr), 0u))) return rc;
-    auto ensure = [&](void **p, size_t bytes) -> int {
-        size_t &have = ctx->array_bytes[p];
-        if (*p == nullptr || have < bytes) {
-            if (*p) cudaFree(*p);
-            *p = nullptr;
-            LRK_CUDA(cudaMalloc(p, bytes));
-            have = bytes;
-        }
-        return LRK_OK;
-    };
-    if ((rc = ensure(&a.bvh_nodes, nodes * 64u))) return rc;
-    if ((rc = ensure(&a.tri_verts, std::max<uint64_t>(s->triangle_count, 1u) * 48u))) return rc;
-    if ((rc = ensure(&a.mesh_bounds, std::max<uint64_t>(s->mesh_count, 1u) * sizeof(BuildBox)))) return rc;
-    if ((rc = upload(ctx, &a.inst_mesh, inst_mesh.data(), inst_mesh.size()))) return rc;
-    if ((rc = upload(ctx, &a.visible_ids, visible.data(), visible.size()))) return rc;
+    LRK_CUDA(a.bvh_nodes.reserve(nodes * 64u));
+    LRK_CUDA(a.tri_verts.reserve(std::max<uint64_t>(s->triangle_count, 1u) * 48u));
+    LRK_CUDA(a.mesh_bounds.reserve(std::max<uint64_t>(s->mesh_count, 1u) * sizeof(BuildBox)));
+    if ((rc = upload(ctx, a.inst_mesh, inst_mesh.data(), inst_mesh.size()))) return rc;
+    if ((rc = upload(ctx, a.visible_ids, visible.data(), visible.size()))) return rc;
     // scratch: boxes, node boxes, keys / values (double buffered), radix nodes, leaf parents, visit counters, whole-set bounds, cub
     size_t cub_bytes = 0u;
     cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, static_cast<const uint32_t *>(nullptr), static_cast<uint32_t *>(nullptr),
@@ -515,22 +505,22 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
                  off_keys2 = off_keys + n8 * 4u, off_vals = off_keys2 + n8 * 4u, off_vals2 = off_vals + n8 * 4u, off_radix = off_vals2 + n8 * 4u,
                  off_leaf_parent = off_radix + n8 * sizeof(RadixNode), off_visits = off_leaf_parent + n8 * 4u, off_whole = off_visits + n8 * 4u,
                  off_cub = off_whole + 64u, total = off_cub + cub_bytes;
-    if ((rc = ensure(&a.build_scratch, total))) return rc;
-    auto base = static_cast<char *>(a.build_scratch);
+    LRK_CUDA(a.build_scratch.reserve(total));
+    auto base = a.build_scratch.get<char>();
     auto boxes = reinterpret_cast<BuildBox *>(base + off_boxes), node_boxes = reinterpret_cast<BuildBox *>(base + off_node_boxes);
     auto keys = reinterpret_cast<uint32_t *>(base + off_keys), keys2 = reinterpret_cast<uint32_t *>(base + off_keys2);
     auto vals = reinterpret_cast<uint32_t *>(base + off_vals), vals2 = reinterpret_cast<uint32_t *>(base + off_vals2);
     auto radix = reinterpret_cast<RadixNode *>(base + off_radix);
     auto leaf_parent = reinterpret_cast<uint32_t *>(base + off_leaf_parent), visits = reinterpret_cast<uint32_t *>(base + off_visits);
     auto whole = reinterpret_cast<uint32_t *>(base + off_whole);
-    auto out_nodes = static_cast<float4 *>(a.bvh_nodes);
+    auto out_nodes = a.bvh_nodes.get<float4>();
     auto stream = ctx->stream;
     static const uint32_t whole_init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
     auto blocks = [](uint64_t n) { return static_cast<unsigned>((n + 255u) / 256u); };
     // common tail: sort, radix tree, fit, emit
     auto hierarchy = [&](uint32_t n, bool tlas, uint32_t node_base, uint32_t slot_base) -> int {
         if (n == 1u) {
-            if (tlas) build_single_kernel<true><<<1, 1, 0, stream>>>(boxes, whole, static_cast<const uint32_t *>(a.visible_ids), node_base, slot_base, out_nodes);
+            if (tlas) build_single_kernel<true><<<1, 1, 0, stream>>>(boxes, whole, a.visible_ids.get<const uint32_t>(), node_base, slot_base, out_nodes);
             else build_single_kernel<false><<<1, 1, 0, stream>>>(boxes, whole, nullptr, node_base, slot_base, out_nodes);
             LRK_CUDA(cudaMemsetAsync(vals2, 0, 4u, stream));// sorted order of one primitive
             return LRK_OK;
@@ -542,7 +532,7 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
         build_radix_tree_kernel<<<blocks(n - 1u), 256, 0, stream>>>(keys2, static_cast<int>(n), radix, leaf_parent);
         build_fit_kernel<<<blocks(n), 256, 0, stream>>>(radix, leaf_parent, vals2, boxes, static_cast<int>(n), node_boxes, visits);
         if (tlas) build_emit_kernel<true><<<blocks(n - 1u), 256, 0, stream>>>(radix, vals2, boxes, node_boxes, static_cast<int>(n), whole,
-                                                                               static_cast<const uint32_t *>(a.visible_ids), node_base, slot_base, out_nodes);
+                                                                               a.visible_ids.get<const uint32_t>(), node_base, slot_base, out_nodes);
         else build_emit_kernel<false><<<blocks(n - 1u), 256, 0, stream>>>(radix, vals2, boxes, node_boxes, static_cast<int>(n), whole, nullptr, node_base,
                                                                           slot_base, out_nodes);
         LRK_CUDA(cudaGetLastError());
@@ -552,13 +542,13 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
     for (uint32_t m = 0; m < s->mesh_count; m++) {
         const auto &mesh = s->meshes[m];
         const uint32_t n = mesh.triangle_count;
-        auto verts = static_cast<const lrk_vertex *>(a.vertices) + mesh.vertex_offset;
-        auto tris = static_cast<const lrk_triangle *>(a.triangles) + mesh.triangle_offset;
+        auto verts = a.vertices.get<const lrk_vertex>() + mesh.vertex_offset;
+        auto tris = a.triangles.get<const lrk_triangle>() + mesh.triangle_offset;
         LRK_CUDA(cudaMemcpyAsync(whole, whole_init, sizeof(whole_init), cudaMemcpyHostToDevice, stream));
         build_triangle_bounds_kernel<<<blocks(n), 256, 0, stream>>>(verts, tris, n, boxes, whole);
-        build_store_mesh_bounds_kernel<<<1, 1, 0, stream>>>(whole, static_cast<BuildBox *>(a.mesh_bounds), m);
+        build_store_mesh_bounds_kernel<<<1, 1, 0, stream>>>(whole, a.mesh_bounds.get<BuildBox>(), m);
         if ((rc = hierarchy(n, false, mesh_root[m], slot_base))) return rc;
-        build_tri_verts_kernel<<<blocks(n), 256, 0, stream>>>(verts, tris, vals2, n, static_cast<float4 *>(a.tri_verts) + static_cast<size_t>(slot_base) * 3u);
+        build_tri_verts_kernel<<<blocks(n), 256, 0, stream>>>(verts, tris, vals2, n, a.tri_verts.get<float4>() + static_cast<size_t>(slot_base) * 3u);
         slot_base += n;
     }
     const uint32_t nv = static_cast<uint32_t>(visible.size());
@@ -570,9 +560,8 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
         LRK_CUDA(cudaMemcpyAsync(out_nodes + static_cast<size_t>(tlas_root) * 4u, &root, sizeof(root), cudaMemcpyHostToDevice, stream));
     } else {
         LRK_CUDA(cudaMemcpyAsync(whole, whole_init, sizeof(whole_init), cudaMemcpyHostToDevice, stream));
-        build_instance_bounds_kernel<<<blocks(nv), 256, 0, stream>>>(static_cast<const float4 *>(a.inst_o2w), static_cast<const uint32_t *>(a.inst_mesh),
-                                                                    static_cast<const uint32_t *>(a.visible_ids), nv,
-                                                                    static_cast<const BuildBox *>(a.mesh_bounds), boxes, whole);
+        build_instance_bounds_kernel<<<blocks(nv), 256, 0, stream>>>(a.inst_o2w.get<const float4>(), a.inst_mesh.get<const uint32_t>(),
+                                                                    a.visible_ids.get<const uint32_t>(), nv, a.mesh_bounds.get<const BuildBox>(), boxes, whole);
         if ((rc = hierarchy(nv, true, tlas_root, 0u))) return rc;
     }
     LRK_CUDA(cudaStreamSynchronize(stream));// host vectors (visible, inst_mesh) and the static init block are done with
@@ -581,6 +570,25 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
 }
 
 }// namespace
+
+// The one teardown of a context, run with its device current and its stream idle (lrk_destroy, or a failed lrk_create).  The device
+// buffers release themselves after this body.
+lrk_ctx::~lrk_ctx() {
+    unpin_all(this);
+    for (auto &t : timed) {
+        cudaEventDestroy(t.start);
+        cudaEventDestroy(t.stop);
+    }
+    for (auto e : event_pool) cudaEventDestroy(e);
+    if (comm != nullptr) {
+        lrk::nccl_api().comm_destroy(comm);
+        cudaEventDestroy(ev_reduce_begin);
+        cudaEventDestroy(ev_reduce_end);
+    }
+    if (ev_begin != nullptr) cudaEventDestroy(ev_begin);
+    if (ev_end != nullptr) cudaEventDestroy(ev_end);
+    if (stream != nullptr) cudaStreamDestroy(stream);
+}
 
 extern "C" {
 
@@ -591,30 +599,21 @@ int lrk_create(const lrk_device_cfg *cfg, lrk_ctx **out) {
     *out = nullptr;
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) return LRK_ERR_NO_DEVICE;
-    auto ctx = new lrk_ctx;
     int dev = cfg ? cfg->device_index : -1;
     if (dev < 0) {
         if (cudaGetDevice(&dev) != cudaSuccess) dev = 0;
     }
-    if (dev >= count || cudaSetDevice(dev) != cudaSuccess) {
-        delete ctx;
-        return LRK_ERR_NO_DEVICE;
-    }
+    if (dev >= count || cudaSetDevice(dev) != cudaSuccess) return LRK_ERR_NO_DEVICE;
+    auto ctx = std::make_unique<lrk_ctx>();// a failed creation releases what it made in ~lrk_ctx
     ctx->device = dev;
     cudaDeviceProp prop{};
     cudaGetDeviceProperties(&prop, dev);
     ctx->sm_count = prop.multiProcessorCount;
     ctx->max_paths = cfg && cfg->max_paths_per_pass ? cfg->max_paths_per_pass : (136ull << 20);
-    if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {
-        delete ctx;
-        return LRK_ERR_CUDA;
-    }
+    if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) return LRK_ERR_CUDA;
     cudaEventCreate(&ctx->ev_begin);
     cudaEventCreate(&ctx->ev_end);
-    if (cudaMalloc(reinterpret_cast<void **>(&ctx->d_query_cursor), 64u * sizeof(uint32_t)) != cudaSuccess) {
-        delete ctx;
-        return LRK_ERR_OUT_OF_MEMORY;
-    }
+    if (ctx->d_query_cursor.reserve(64u * sizeof(uint32_t)) != cudaSuccess) return LRK_ERR_OUT_OF_MEMORY;
     auto grid_for = [&](const void *fn, int block = kBlock) {
         int per_sm = 0;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, block, 0);
@@ -634,7 +633,7 @@ int lrk_create(const lrk_device_cfg *cfg, lrk_ctx **out) {
         ctx->grid_vshade[1][kind] = strict::volume_surface_grid(kind, ctx->sm_count);
     }
     ctx->grid_vshadow = grid_for(reinterpret_cast<const void *>(trace_volume_nee_kernel<false>), kTraceBlock);
-    *out = ctx;
+    *out = ctx.release();
     return LRK_OK;
 }
 
@@ -642,30 +641,6 @@ void lrk_destroy(lrk_ctx *ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    unpin_all(ctx);
-    free_paths(ctx);
-    free_arrays(ctx->arrays);
-    if (ctx->d_pixel_list) cudaFree(ctx->d_pixel_list);
-    if (ctx->d_film) cudaFree(ctx->d_film);
-    if (ctx->d_film_out) cudaFree(ctx->d_film_out);
-    if (ctx->d_query_cursor) cudaFree(ctx->d_query_cursor);
-    for (void *p : {static_cast<void *>(ctx->d_moments), static_cast<void *>(ctx->d_sample_counts), static_cast<void *>(ctx->d_active[0]),
-                    static_cast<void *>(ctx->d_active[1]), static_cast<void *>(ctx->d_block_start[0]), static_cast<void *>(ctx->d_block_start[1]),
-                    static_cast<void *>(ctx->d_block_start[2]), static_cast<void *>(ctx->d_keep), ctx->d_scan_temp})
-        if (p) cudaFree(p);
-    for (auto &t : ctx->timed) {
-        cudaEventDestroy(t.start);
-        cudaEventDestroy(t.stop);
-    }
-    for (auto e : ctx->event_pool) cudaEventDestroy(e);
-    if (ctx->comm != nullptr) {
-        lrk::nccl_api().comm_destroy(ctx->comm);
-        cudaEventDestroy(ctx->ev_reduce_begin);
-        cudaEventDestroy(ctx->ev_reduce_end);
-    }
-    cudaEventDestroy(ctx->ev_begin);
-    cudaEventDestroy(ctx->ev_end);
-    cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
 
@@ -772,56 +747,56 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     LRK_CUDA(cudaSetDevice(ctx->device));
     auto &a = ctx->arrays;
     int rc;
-    if ((rc = upload(ctx, &a.vertices, s->vertices, s->vertex_count))) return rc;
-    if ((rc = upload(ctx, &a.triangles, s->triangles, s->triangle_count))) return rc;
-    if ((rc = upload(ctx, &a.alias, s->alias, s->triangle_count))) return rc;
-    if ((rc = upload(ctx, &a.pdf, s->pdf, s->triangle_count))) return rc;
-    if ((rc = upload(ctx, &a.meshes, s->meshes, s->mesh_count))) return rc;
+    if ((rc = upload(ctx, a.vertices, s->vertices, s->vertex_count))) return rc;
+    if ((rc = upload(ctx, a.triangles, s->triangles, s->triangle_count))) return rc;
+    if ((rc = upload(ctx, a.alias, s->alias, s->triangle_count))) return rc;
+    if ((rc = upload(ctx, a.pdf, s->pdf, s->triangle_count))) return rc;
+    if ((rc = upload(ctx, a.meshes, s->meshes, s->mesh_count))) return rc;
     if (!ctx->device_bvh)
-        if ((rc = upload(ctx, &a.bvh_nodes, s->bvh_nodes, s->bvh_node_count))) return rc;
+        if ((rc = upload(ctx, a.bvh_nodes, s->bvh_nodes, s->bvh_node_count))) return rc;
     {
         static const uint32_t zero = 0u;
-        if ((rc = upload(ctx, &a.traversal_overflow, &zero, 1u))) return rc;
+        if ((rc = upload(ctx, a.traversal_overflow, &zero, 1u))) return rc;
     }
     if (!ctx->device_bvh)
-        if ((rc = upload(ctx, &a.tri_verts, s->tri_verts, s->tri_slot_count * 12u))) return rc;
-    if ((rc = upload(ctx, &a.surfaces, s->surfaces, s->surface_count))) return rc;
-    if ((rc = upload(ctx, &a.textures, s->textures, s->texture_count))) return rc;
+        if ((rc = upload(ctx, a.tri_verts, s->tri_verts, s->tri_slot_count * 12u))) return rc;
+    if ((rc = upload(ctx, a.surfaces, s->surfaces, s->surface_count))) return rc;
+    if ((rc = upload(ctx, a.textures, s->textures, s->texture_count))) return rc;
     {
         const auto &e = s->environment;
         const bool mapped = e.present && e.emission_tex != 0u;
         const size_t cells = mapped ? static_cast<size_t>(e.map_width) * e.map_height : 0u;
-        if ((rc = upload(ctx, &a.env_alias, e.alias, mapped ? cells + e.map_height : 0u))) return rc;
-        if ((rc = upload(ctx, &a.env_pdf, e.pdf, cells))) return rc;
+        if ((rc = upload(ctx, a.env_alias, e.alias, mapped ? cells + e.map_height : 0u))) return rc;
+        if ((rc = upload(ctx, a.env_pdf, e.pdf, cells))) return rc;
     }
-    if ((rc = upload(ctx, &a.texels, s->texels, s->texel_count * 4u))) return rc;
-    if ((rc = upload(ctx, &a.lights, s->lights, s->light_count))) return rc;
-    if ((rc = upload(ctx, &a.light_handles, s->light_handles, s->light_count))) return rc;
-    if ((rc = upload(ctx, &a.camera, &s->camera, 1))) return rc;
+    if ((rc = upload(ctx, a.texels, s->texels, s->texel_count * 4u))) return rc;
+    if ((rc = upload(ctx, a.lights, s->lights, s->light_count))) return rc;
+    if ((rc = upload(ctx, a.light_handles, s->light_handles, s->light_count))) return rc;
+    if ((rc = upload(ctx, a.camera, &s->camera, 1))) return rc;
     if (s->sampler.type != LRK_SAMPLER_INDEPENDENT) {
         // the static tables (213 KB / 2.6 MB / 1.5 MB) cross the bus once per context: same host address = same table
         const auto &q = s->sampler;
         if (ctx->sampler_table_src[0] != q.sobol_matrices) {
-            if ((rc = upload(ctx, &a.sobol, q.sobol_matrices, 1024u * 52u))) return rc;
+            if ((rc = upload(ctx, a.sobol, q.sobol_matrices, 1024u * 52u))) return rc;
             ctx->sampler_table_src[0] = q.sobol_matrices;
         }
         if (q.type == LRK_SAMPLER_PMJ02BN) {
             if (ctx->sampler_table_src[1] != q.pmj_samples) {
-                if ((rc = upload(ctx, &a.pmj, q.pmj_samples, 5u * 65536u * 2u))) return rc;
+                if ((rc = upload(ctx, a.pmj, q.pmj_samples, 5u * 65536u * 2u))) return rc;
                 ctx->sampler_table_src[1] = q.pmj_samples;
             }
             if (ctx->sampler_table_src[2] != q.blue_noise) {
-                if ((rc = upload(ctx, &a.blue_noise, q.blue_noise, 48u * 128u * 128u))) return rc;
+                if ((rc = upload(ctx, a.blue_noise, q.blue_noise, 48u * 128u * 128u))) return rc;
                 ctx->sampler_table_src[2] = q.blue_noise;
             }
-            if ((rc = upload(ctx, &a.pmj_pixels, q.pmj_pixel_samples, q.pmj_pixel_sample_count * 2u))) return rc;
+            if ((rc = upload(ctx, a.pmj_pixels, q.pmj_pixel_samples, q.pmj_pixel_sample_count * 2u))) return rc;
         }
         if (q.type == LRK_SAMPLER_SOBOL) {
-            if ((rc = upload(ctx, &a.vdc, q.vdc, 52u))) return rc;
-            if ((rc = upload(ctx, &a.vdc_inv, q.vdc_inv, 52u))) return rc;
+            if ((rc = upload(ctx, a.vdc, q.vdc, 52u))) return rc;
+            if ((rc = upload(ctx, a.vdc_inv, q.vdc_inv, 52u))) return rc;
         }
         if (q.type == LRK_SAMPLER_ZSOBOL)
-            if ((rc = upload(ctx, &a.zsobol_hash, q.zsobol_hash, 2048u))) return rc;
+            if ((rc = upload(ctx, a.zsobol_hash, q.zsobol_hash, 2048u))) return rc;
     }
     std::vector<uint32_t> handles(static_cast<size_t>(s->instance_count) * 4u), kinds(s->instance_count);
     for (int k = 1; k < static_cast<int>(kHitKinds); k++) ctx->has_kind[k] = false;
@@ -850,9 +825,9 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         std::memcpy(&xform[i * 16u], inst.world_to_object, 48);
         xform[i * 16u + 12u] = xform[i * 16u + 13u] = xform[i * 16u + 14u] = xform[i * 16u + 15u] = 0.f;
     }
-    if ((rc = upload(ctx, &a.inst_handles, handles.data(), handles.size()))) return rc;
-    if ((rc = upload(ctx, &a.inst_kind, kinds.data(), kinds.size()))) return rc;
-    if ((rc = upload(ctx, &a.inst_o2w, o2w.data(), o2w.size()))) return rc;
+    if ((rc = upload(ctx, a.inst_handles, handles.data(), handles.size()))) return rc;
+    if ((rc = upload(ctx, a.inst_kind, kinds.data(), kinds.size()))) return rc;
+    if ((rc = upload(ctx, a.inst_o2w, o2w.data(), o2w.size()))) return rc;
     // the hierarchy: the host's (the parity path: the oracle walks the same nodes) or one built here on the device
     std::vector<uint32_t> mesh_root(s->mesh_count);
     uint32_t tlas_root = s->tlas_root;
@@ -864,26 +839,26 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         for (uint32_t m = 0; m < s->mesh_count; m++) mesh_root[m] = s->meshes[m].bvh_root;
     }
     for (uint32_t i = 0; i < s->instance_count; i++) std::memcpy(&xform[i * 16u + 12u], &mesh_root[s->instances[i].mesh], 4);
-    if ((rc = upload(ctx, &a.inst_xform, xform.data(), xform.size()))) return rc;
+    if ((rc = upload(ctx, a.inst_xform, xform.data(), xform.size()))) return rc;
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
 
     auto &sc = ctx->scene;
-    sc.vertices = static_cast<const lrk_vertex *>(a.vertices);
-    sc.triangles = static_cast<const lrk_triangle *>(a.triangles);
-    sc.alias = static_cast<const lrk_alias_entry *>(a.alias);
-    sc.pdf = static_cast<const float *>(a.pdf);
-    sc.meshes = static_cast<const lrk_mesh *>(a.meshes);
-    sc.inst_handles = static_cast<const uint4 *>(a.inst_handles);
-    sc.inst_kind = static_cast<const uint32_t *>(a.inst_kind);
-    sc.inst_o2w = static_cast<const float4 *>(a.inst_o2w);
-    sc.inst_xform = static_cast<const float4 *>(a.inst_xform);
-    sc.bvh_nodes = static_cast<const float4 *>(a.bvh_nodes);
-    sc.traversal_overflow = static_cast<uint32_t *>(a.traversal_overflow);
-    sc.tri_verts = static_cast<const float4 *>(a.tri_verts);
-    sc.surfaces = static_cast<const lrk_surface *>(a.surfaces);
-    sc.textures = static_cast<const lrk_texture *>(a.textures);
-    sc.env_alias = static_cast<const lrk_alias_entry *>(a.env_alias);
-    sc.env_pdf = static_cast<const float *>(a.env_pdf);
+    sc.vertices = a.vertices.get<const lrk_vertex>();
+    sc.triangles = a.triangles.get<const lrk_triangle>();
+    sc.alias = a.alias.get<const lrk_alias_entry>();
+    sc.pdf = a.pdf.get<const float>();
+    sc.meshes = a.meshes.get<const lrk_mesh>();
+    sc.inst_handles = a.inst_handles.get<const uint4>();
+    sc.inst_kind = a.inst_kind.get<const uint32_t>();
+    sc.inst_o2w = a.inst_o2w.get<const float4>();
+    sc.inst_xform = a.inst_xform.get<const float4>();
+    sc.bvh_nodes = a.bvh_nodes.get<const float4>();
+    sc.traversal_overflow = a.traversal_overflow.get<uint32_t>();
+    sc.tri_verts = a.tri_verts.get<const float4>();
+    sc.surfaces = a.surfaces.get<const lrk_surface>();
+    sc.textures = a.textures.get<const lrk_texture>();
+    sc.env_alias = a.env_alias.get<const lrk_alias_entry>();
+    sc.env_pdf = a.env_pdf.get<const float>();
     sc.env_present = s->environment.present ? 1u : 0u;
     sc.env_emission_tex = s->environment.present ? s->environment.emission_tex : 0u;
     sc.env_map_width = s->environment.map_width;
@@ -892,10 +867,10 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     sc.env_prob = s->environment.present ? s->environment.env_prob : 0.f;
     for (int k = 0; k < 3; k++) sc.env_emission[k] = s->environment.emission[k];
     for (int k = 0; k < 9; k++) sc.env_to_world[k] = s->environment.to_world[k];
-    sc.texels = static_cast<const float4 *>(a.texels);
-    sc.lights = static_cast<const lrk_light *>(a.lights);
-    sc.light_handles = static_cast<const lrk_light_handle *>(a.light_handles);
-    sc.camera = static_cast<const lrk_camera *>(a.camera);
+    sc.texels = a.texels.get<const float4>();
+    sc.lights = a.lights.get<const lrk_light>();
+    sc.light_handles = a.light_handles.get<const lrk_light_handle>();
+    sc.camera = a.camera.get<const lrk_camera>();
     sc.tlas_root = tlas_root;
     sc.light_count = s->light_count;
     sc.instance_count = s->instance_count;
@@ -906,17 +881,17 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     sc.sampler_seed = s->integrator.sampler_seed;
     {// the sampler record in device memory, its table pointers replaced by the device copies
         lrk_sampler rec = s->sampler;
-        rec.sobol_matrices = static_cast<const uint32_t *>(a.sobol);
-        rec.vdc = static_cast<const uint64_t *>(a.vdc);
-        rec.vdc_inv = static_cast<const uint64_t *>(a.vdc_inv);
-        rec.pmj_samples = static_cast<const uint32_t *>(a.pmj);
-        rec.blue_noise = static_cast<const uint16_t *>(a.blue_noise);
-        rec.pmj_pixel_samples = static_cast<const float *>(a.pmj_pixels);
-        rec.zsobol_hash = static_cast<const uint32_t *>(a.zsobol_hash);
-        if ((rc = upload(ctx, &a.sampler, &rec, 1))) return rc;
+        rec.sobol_matrices = a.sobol.get<const uint32_t>();
+        rec.vdc = a.vdc.get<const uint64_t>();
+        rec.vdc_inv = a.vdc_inv.get<const uint64_t>();
+        rec.pmj_samples = a.pmj.get<const uint32_t>();
+        rec.blue_noise = a.blue_noise.get<const uint16_t>();
+        rec.pmj_pixel_samples = a.pmj_pixels.get<const float>();
+        rec.zsobol_hash = a.zsobol_hash.get<const uint32_t>();
+        if ((rc = upload(ctx, a.sampler, &rec, 1))) return rc;
         LRK_CUDA(cudaStreamSynchronize(ctx->stream));// `rec` is a stack object
         sc.sampler_type = rec.type;
-        sc.sampler = static_cast<const lrk_sampler *>(a.sampler);
+        sc.sampler = a.sampler.get<const lrk_sampler>();
     }
     sc.film_clamp = s->film.clamp;
     for (int i = 0; i < 3; i++) sc.film_scale[i] = s->film.scale[i];
@@ -933,32 +908,20 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     sc.medium_g = s->environment_medium.g;
     sc.medium_priority = s->environment_medium.priority;
     ctx->volume_general = volume_general;
-    if ((rc = upload(ctx, &a.media, s->media, s->medium_count))) return rc;
-    sc.media = static_cast<const lrk_medium *>(a.media);
+    if ((rc = upload(ctx, a.media, s->media, s->medium_count))) return rc;
+    sc.media = a.media.get<const lrk_medium>();
     sc.medium_count = s->medium_count;
     sc.env_medium_tag = s->environment_medium_tag;
 
     const size_t npix = static_cast<size_t>(sc.width) * sc.height;
-    if (ctx->film_pixels != npix) {
-        if (ctx->d_film) cudaFree(ctx->d_film);
-        if (ctx->d_film_out) cudaFree(ctx->d_film_out);
-        ctx->d_film = ctx->d_film_out = nullptr;
-        ctx->film_pixels = 0;
-        LRK_CUDA(cudaMalloc(reinterpret_cast<void **>(&ctx->d_film), npix * sizeof(float4)));
-        LRK_CUDA(cudaMalloc(reinterpret_cast<void **>(&ctx->d_film_out), npix * sizeof(float4)));
-        ctx->film_pixels = npix;
-    }
+    ctx->film_pixels = 0;
+    LRK_CUDA(ctx->d_film.reserve(npix * sizeof(float4)));
+    LRK_CUDA(ctx->d_film_out.reserve(npix * sizeof(float4)));
+    ctx->film_pixels = npix;
     {// the scene record itself in device memory, for the out-of-line device functions (DeviceScene::self)
-        if ((rc = upload(ctx, &a.scene_copy, static_cast<const DeviceScene *>(nullptr), 0u))) return rc;
-        size_t &have = ctx->array_bytes[&a.scene_copy];
-        if (have < sizeof(DeviceScene)) {
-            cudaFree(a.scene_copy);
-            a.scene_copy = nullptr;
-            LRK_CUDA(cudaMalloc(&a.scene_copy, sizeof(DeviceScene)));
-            have = sizeof(DeviceScene);
-        }
-        sc.self = static_cast<const DeviceScene *>(a.scene_copy);
-        LRK_CUDA(cudaMemcpyAsync(a.scene_copy, &sc, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
+        LRK_CUDA(a.scene_copy.reserve(sizeof(DeviceScene)));
+        sc.self = a.scene_copy.get<const DeviceScene>();
+        LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get(), &sc, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
         LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     }
     ctx->has_scene = true;
@@ -999,15 +962,14 @@ int lrk_balance_shards(lrk_ctx *ctx, uint32_t rank, uint32_t world, uint32_t til
     if (rc) return rc;
     const uint32_t tiles_x = (ctx->scene.width + tile_size - 1u) / tile_size, tiles_y = (ctx->scene.height + tile_size - 1u) / tile_size;
     const uint32_t tile_count = tiles_x * tiles_y;
-    uint32_t *d_cost = nullptr;
-    LRK_CUDA(cudaMalloc(reinterpret_cast<void **>(&d_cost), static_cast<size_t>(tile_count) * sizeof(uint32_t)));
-    cudaMemsetAsync(d_cost, 0, static_cast<size_t>(tile_count) * sizeof(uint32_t), ctx->stream);
-    ctx->probe_cost = d_cost;
+    DeviceBuffer d_cost;
+    LRK_CUDA(d_cost.reserve(static_cast<size_t>(tile_count) * sizeof(uint32_t)));
+    cudaMemsetAsync(d_cost.get(), 0, static_cast<size_t>(tile_count) * sizeof(uint32_t), ctx->stream);
+    ctx->probe_cost = d_cost.get<uint32_t>();
     rc = lrk_render(ctx, 0u, probe_spp);
     ctx->probe_cost = nullptr;
     std::vector<uint32_t> cost(tile_count);
-    if (rc == LRK_OK && cudaMemcpy(cost.data(), d_cost, static_cast<size_t>(tile_count) * sizeof(uint32_t), cudaMemcpyDeviceToHost) != cudaSuccess) rc = LRK_ERR_CUDA;
-    cudaFree(d_cost);
+    if (rc == LRK_OK && cudaMemcpy(cost.data(), d_cost.get(), static_cast<size_t>(tile_count) * sizeof(uint32_t), cudaMemcpyDeviceToHost) != cudaSuccess) rc = LRK_ERR_CUDA;
     if (rc) return rc;
     std::vector<uint32_t> owner(tile_count);
     lrk_assign_tiles(cost.data(), tile_count, world, owner.data());
@@ -1046,8 +1008,8 @@ int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value) {
     } else if (n == "max_paths_per_pass") ctx->max_paths = value > 0 ? static_cast<uint64_t>(value) : ctx->max_paths;
     else if (n == "refill_below" || n == "inner_min") {
         (n == "refill_below" ? ctx->scene.refill_below : ctx->scene.inner_min) = static_cast<uint32_t>(std::min<int64_t>(std::max<int64_t>(value, 1), 32));
-        if (ctx->has_scene && ctx->arrays.scene_copy) {// keep DeviceScene::self in step
-            LRK_CUDA(cudaMemcpyAsync(ctx->arrays.scene_copy, &ctx->scene, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
+        if (ctx->has_scene && ctx->arrays.scene_copy.get() != nullptr) {// keep DeviceScene::self in step
+            LRK_CUDA(cudaMemcpyAsync(ctx->arrays.scene_copy.get(), &ctx->scene, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
             LRK_CUDA(cudaStreamSynchronize(ctx->stream));
         }
     }
@@ -1059,7 +1021,7 @@ int lrk_film_clear(lrk_ctx *ctx) {
     if (!ctx || !ctx->has_scene) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_film_clear: no scene");
     LRK_CUDA(cudaSetDevice(ctx->device));
     const size_t npix = static_cast<size_t>(ctx->scene.width) * ctx->scene.height;
-    LRK_CUDA(cudaMemsetAsync(ctx->d_film, 0, npix * sizeof(float4), ctx->stream));
+    LRK_CUDA(cudaMemsetAsync(ctx->d_film.get(), 0, npix * sizeof(float4), ctx->stream));
     if (ctx->pb.stats) LRK_CUDA(cudaMemsetAsync(ctx->pb.stats, 0, 8u * sizeof(unsigned long long), ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     ctx->stats = lrk_stats{};
@@ -1134,41 +1096,25 @@ int lrk_render(lrk_ctx *ctx, uint32_t spp_begin, uint32_t spp_end) {
     int rc = alloc_paths(ctx, static_cast<uint64_t>(sh.chunk_pix) * sh.spp_per_pass);
     if (rc) return rc;
     LRK_CUDA(cudaEventRecord(ctx->ev_begin, ctx->stream));
-    if ((rc = render_passes(ctx, ctx->d_pixel_list, npix, spp_begin, spp_end, sh))) return rc;
+    if ((rc = render_passes(ctx, ctx->d_pixel_list.get<uint32_t>(), npix, spp_begin, spp_end, sh))) return rc;
     return finish_render(ctx, "lrk_render", static_cast<uint64_t>(npix) * (spp_end - spp_begin));
 }
 
 // Buffers of the adaptive mode, grown to the film / pixel list / block count of this context; clears the moments and counts.
 static int alloc_adaptive(lrk_ctx *ctx) {
     const size_t pixels = ctx->film_pixels, list = std::max<size_t>(ctx->npix_owned, 1u), blocks = ctx->block_start.size();
-    auto grow = [&](void **p, size_t &have, size_t need, size_t bytes_each) -> int {
-        if (*p != nullptr && have >= need) return LRK_OK;
-        if (*p) cudaFree(*p);
-        *p = nullptr;
-        LRK_CUDA(cudaMalloc(p, need * bytes_each));
-        return LRK_OK;
-    };
-    int rc;
-    size_t have = ctx->adaptive_pixels;
-    if ((rc = grow(reinterpret_cast<void **>(&ctx->d_moments), have, pixels, sizeof(float2)))) return rc;
-    if ((rc = grow(reinterpret_cast<void **>(&ctx->d_sample_counts), have, pixels, sizeof(uint32_t)))) return rc;
-    ctx->adaptive_pixels = std::max(have, pixels);
-    have = ctx->adaptive_list;
-    for (auto &p : ctx->d_active)
-        if ((rc = grow(reinterpret_cast<void **>(&p), have, list, sizeof(uint32_t)))) return rc;
-    ctx->adaptive_list = std::max(have, list);
-    have = ctx->adaptive_blocks;
-    for (auto &p : ctx->d_block_start)
-        if ((rc = grow(reinterpret_cast<void **>(&p), have, blocks, sizeof(uint32_t)))) return rc;
-    if ((rc = grow(reinterpret_cast<void **>(&ctx->d_keep), have, blocks, 2u * sizeof(unsigned long long)))) return rc;
-    ctx->adaptive_blocks = std::max(have, blocks);
+    LRK_CUDA(ctx->d_moments.reserve(pixels * sizeof(float2)));
+    LRK_CUDA(ctx->d_sample_counts.reserve(pixels * sizeof(uint32_t)));
+    for (auto &b : ctx->d_active) LRK_CUDA(b.reserve(list * sizeof(uint32_t)));
+    for (auto &b : ctx->d_block_start) LRK_CUDA(b.reserve(blocks * sizeof(uint32_t)));
+    LRK_CUDA(ctx->d_keep.reserve(blocks * 2u * sizeof(unsigned long long)));
     size_t temp = 0u;
-    cub::DeviceScan::ExclusiveSum(nullptr, temp, ctx->d_keep, ctx->d_keep + blocks, static_cast<int>(blocks), ctx->stream);
-    if ((rc = grow(&ctx->d_scan_temp, ctx->scan_temp_bytes, temp, 1u))) return rc;
-    ctx->scan_temp_bytes = std::max(ctx->scan_temp_bytes, temp);
-    LRK_CUDA(cudaMemsetAsync(ctx->d_moments, 0, pixels * sizeof(float2), ctx->stream));
-    LRK_CUDA(cudaMemsetAsync(ctx->d_sample_counts, 0, pixels * sizeof(uint32_t), ctx->stream));
-    LRK_CUDA(cudaMemcpyAsync(ctx->d_block_start[0], ctx->block_start.data(), blocks * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    auto keep = ctx->d_keep.get<unsigned long long>();
+    cub::DeviceScan::ExclusiveSum(nullptr, temp, keep, keep + blocks, static_cast<int>(blocks), ctx->stream);
+    LRK_CUDA(ctx->d_scan_temp.reserve(temp));
+    LRK_CUDA(cudaMemsetAsync(ctx->d_moments.get(), 0, pixels * sizeof(float2), ctx->stream));
+    LRK_CUDA(cudaMemsetAsync(ctx->d_sample_counts.get(), 0, pixels * sizeof(uint32_t), ctx->stream));
+    LRK_CUDA(cudaMemcpyAsync(ctx->d_block_start[0].get(), ctx->block_start.data(), blocks * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));// block_start is pageable host memory
     return LRK_OK;
 }
@@ -1192,11 +1138,11 @@ int lrk_render_adaptive(lrk_ctx *ctx, const lrk_adaptive *p) {
         lrk_ctx *ctx;
         ~MomentsOn() { ctx->pass_moments = nullptr; }
     } moments_on{ctx};
-    ctx->pass_moments = ctx->d_moments;
-    const uint32_t *list = ctx->d_pixel_list;
-    const uint32_t *blocks = ctx->d_block_start[0];
+    ctx->pass_moments = ctx->d_moments.get<float2>();
+    const uint32_t *list = ctx->d_pixel_list.get<uint32_t>();
+    const uint32_t *blocks = ctx->d_block_start[0].get<uint32_t>();
     uint32_t active = npix, nblocks = static_cast<uint32_t>(ctx->block_start.size() - 1u), c = 0u, next = p->min_spp;
-    unsigned long long *keep = ctx->d_keep, *offsets = ctx->d_keep + ctx->adaptive_blocks;
+    unsigned long long *keep = ctx->d_keep.get<unsigned long long>(), *offsets = keep + ctx->block_start.size();
     uint64_t samples = 0u;
     bool timing = false;
     for (uint32_t round = 0u;; round++) {
@@ -1211,15 +1157,16 @@ int lrk_render_adaptive(lrk_ctx *ctx, const lrk_adaptive *p) {
         c = next;
         const bool last = c >= p->max_spp;
         const unsigned grid = static_cast<unsigned>((static_cast<uint64_t>(nblocks + 1u) * 32u + kAdaptiveBlock - 1u) / kAdaptiveBlock);
-        adaptive_test_kernel<<<grid, kAdaptiveBlock, 0, ctx->stream>>>(ctx->scene.width, ctx->d_film, ctx->d_moments, list, blocks, nblocks, p->threshold,
-                                                                        c, last, ctx->d_sample_counts, keep);
+        adaptive_test_kernel<<<grid, kAdaptiveBlock, 0, ctx->stream>>>(ctx->scene.width, ctx->d_film.get<float4>(), ctx->d_moments.get<float2>(), list, blocks,
+                                                                        nblocks, p->threshold, c, last, ctx->d_sample_counts.get<uint32_t>(), keep);
         ctx->stats.kernel_launches++;
         if (last) break;
-        size_t temp = ctx->scan_temp_bytes;
-        LRK_CUDA(cub::DeviceScan::ExclusiveSum(ctx->d_scan_temp, temp, keep, offsets, static_cast<int>(nblocks + 1u), ctx->stream));
-        uint32_t *list_out = ctx->d_active[round & 1u], *blocks_out = ctx->d_block_start[1u + (round & 1u)];
+        size_t temp = ctx->d_scan_temp.bytes();
+        LRK_CUDA(cub::DeviceScan::ExclusiveSum(ctx->d_scan_temp.get(), temp, keep, offsets, static_cast<int>(nblocks + 1u), ctx->stream));
+        ctx->stats.kernel_launches++;
+        uint32_t *list_out = ctx->d_active[round & 1u].get<uint32_t>(), *blocks_out = ctx->d_block_start[1u + (round & 1u)].get<uint32_t>();
         adaptive_compact_kernel<<<grid, kAdaptiveBlock, 0, ctx->stream>>>(list, blocks, nblocks, keep, offsets, list_out, blocks_out);
-        ctx->stats.kernel_launches += 2u;
+        ctx->stats.kernel_launches++;
         LRK_CUDA(cudaGetLastError());
         unsigned long long total = 0ull;
         LRK_CUDA(cudaMemcpyAsync(&total, offsets + nblocks, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1241,7 +1188,7 @@ int lrk_download_sample_counts(lrk_ctx *ctx, uint32_t *counts) {
     if (!ctx || !ctx->has_scene || !counts) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_download_sample_counts: no scene / null buffer");
     if (!ctx->adaptive_valid) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_download_sample_counts: no adaptive render since the last film clear");
     LRK_CUDA(cudaSetDevice(ctx->device));
-    LRK_CUDA(cudaMemcpyAsync(counts, ctx->d_sample_counts, ctx->film_pixels * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    LRK_CUDA(cudaMemcpyAsync(counts, ctx->d_sample_counts.get(), ctx->film_pixels * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     return LRK_OK;
 }
@@ -1251,8 +1198,9 @@ int lrk_download_film_variance(lrk_ctx *ctx, float *v) {
     if (!ctx->adaptive_valid) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_download_film_variance: no adaptive render since the last film clear");
     LRK_CUDA(cudaSetDevice(ctx->device));
     const uint32_t n = static_cast<uint32_t>(ctx->film_pixels);
-    float *out = reinterpret_cast<float *>(ctx->d_film_out);// the staging buffer of lrk_download_film
-    adaptive_variance_kernel<<<(n + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->d_film, ctx->d_moments, ctx->d_sample_counts, out, n);
+    float *out = ctx->d_film_out.get<float>();// the staging buffer of lrk_download_film
+    adaptive_variance_kernel<<<(n + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->d_film.get<float4>(), ctx->d_moments.get<float2>(),
+                                                                                    ctx->d_sample_counts.get<uint32_t>(), out, n);
     LRK_CUDA(cudaGetLastError());
     LRK_CUDA(cudaMemcpyAsync(v, out, static_cast<size_t>(n) * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1261,10 +1209,10 @@ int lrk_download_film_variance(lrk_ctx *ctx, float *v) {
 
 static int convert_and_copy(lrk_ctx *ctx, const float4 *raw, float *rgba) {
     const uint32_t npix = ctx->scene.width * ctx->scene.height;
-    convert_film_kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->scene, raw, ctx->d_film_out, npix);
+    convert_film_kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->scene, raw, ctx->d_film_out.get<float4>(), npix);
     LRK_CUDA(cudaGetLastError());
     pin_range(ctx, rgba, static_cast<size_t>(npix) * sizeof(float4));
-    LRK_CUDA(cudaMemcpyAsync(rgba, ctx->d_film_out, static_cast<size_t>(npix) * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
+    LRK_CUDA(cudaMemcpyAsync(rgba, ctx->d_film_out.get(),static_cast<size_t>(npix) * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     return LRK_OK;
 }
@@ -1272,7 +1220,7 @@ static int convert_and_copy(lrk_ctx *ctx, const float4 *raw, float *rgba) {
 int lrk_download_film(lrk_ctx *ctx, float *rgba) {
     if (!ctx || !ctx->has_scene || !rgba) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_download_film: no scene / null buffer");
     LRK_CUDA(cudaSetDevice(ctx->device));
-    return convert_and_copy(ctx, ctx->d_film, rgba);
+    return convert_and_copy(ctx, ctx->d_film.get<float4>(), rgba);
 }
 
 int lrk_download_film_raw(lrk_ctx *ctx, float *rgba) {
@@ -1280,14 +1228,14 @@ int lrk_download_film_raw(lrk_ctx *ctx, float *rgba) {
     LRK_CUDA(cudaSetDevice(ctx->device));
     const size_t npix = static_cast<size_t>(ctx->scene.width) * ctx->scene.height;
     pin_range(ctx, rgba, npix * sizeof(float4));
-    LRK_CUDA(cudaMemcpyAsync(rgba, ctx->d_film, npix * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
+    LRK_CUDA(cudaMemcpyAsync(rgba, ctx->d_film.get(), npix * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     return LRK_OK;
 }
 
 int lrk_film_device_ptr(lrk_ctx *ctx, void **ptr, uint64_t *bytes) {
     if (!ctx || !ctx->has_scene || !ptr || !bytes) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_film_device_ptr: no scene");
-    *ptr = ctx->d_film;
+    *ptr = ctx->d_film.get();
     *bytes = static_cast<uint64_t>(ctx->scene.width) * ctx->scene.height * sizeof(float4);
     return LRK_OK;
 }
@@ -1303,23 +1251,17 @@ int lrk_trace(lrk_ctx *ctx, const lrk_ray *rays, uint64_t n, int any_hit, lrk_hi
     if (n == 0u) return LRK_OK;
     if (!rays || !hits || n > 0xffffffffull) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_trace: bad argument");
     LRK_CUDA(cudaSetDevice(ctx->device));
-    float4 *d_rays = nullptr;
-    uint4 *d_hits = nullptr;
-    LRK_CUDA(cudaMalloc(reinterpret_cast<void **>(&d_rays), n * sizeof(lrk_ray)));
-    if (cudaMalloc(reinterpret_cast<void **>(&d_hits), n * sizeof(lrk_hit)) != cudaSuccess) {
-        cudaFree(d_rays);
-        return fail(ctx, LRK_ERR_OUT_OF_MEMORY, "lrk_trace: out of device memory");
-    }
-    cudaMemcpyAsync(d_rays, rays, n * sizeof(lrk_ray), cudaMemcpyHostToDevice, ctx->stream);
+    DeviceBuffer d_rays, d_hits;
+    LRK_CUDA(d_rays.reserve(n * sizeof(lrk_ray)));
+    if (d_hits.reserve(n * sizeof(lrk_hit)) != cudaSuccess) return fail(ctx, LRK_ERR_OUT_OF_MEMORY, "lrk_trace: out of device memory");
+    cudaMemcpyAsync(d_rays.get(), rays, n * sizeof(lrk_ray), cudaMemcpyHostToDevice, ctx->stream);
     int g = blocks_for(ctx, n, ctx->grid_trace);
-    cudaMemsetAsync(ctx->d_query_cursor, 0, sizeof(uint32_t), ctx->stream);
-    launch_query(ctx, g, any_hit != 0, d_rays, d_hits, static_cast<uint32_t>(n));
-    cudaMemcpyAsync(hits, d_hits, n * sizeof(lrk_hit), cudaMemcpyDeviceToHost, ctx->stream);
+    cudaMemsetAsync(ctx->d_query_cursor.get(), 0, sizeof(uint32_t), ctx->stream);
+    launch_query(ctx, g, any_hit != 0, d_rays.get<float4>(), d_hits.get<uint4>(), static_cast<uint32_t>(n));
+    cudaMemcpyAsync(hits, d_hits.get(), n * sizeof(lrk_hit), cudaMemcpyDeviceToHost, ctx->stream);
     cudaMemcpyAsync(&ctx->h_overflow, ctx->scene.traversal_overflow, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (e == cudaSuccess) e = cudaGetLastError();
-    cudaFree(d_rays);
-    cudaFree(d_hits);
     if (e != cudaSuccess) return fail(ctx, LRK_ERR_CUDA, std::string("lrk_trace: ") + cudaGetErrorString(e));
     if (ctx->h_overflow != 0u) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_trace: traversal stack overflow (BVH deeper than the kernels support)");
     return LRK_OK;
@@ -1332,7 +1274,7 @@ int lrk_trace_device(lrk_ctx *ctx, const void *d_rays, uint64_t n, int any_hit, 
     int g = blocks_for(ctx, n, ctx->grid_trace);
     LRK_CUDA(cudaEventRecord(ctx->ev_begin, ctx->stream));
     for (uint32_t r = 0; r < repeat; r++) {
-        LRK_CUDA(cudaMemsetAsync(ctx->d_query_cursor, 0, sizeof(uint32_t), ctx->stream));
+        LRK_CUDA(cudaMemsetAsync(ctx->d_query_cursor.get(), 0, sizeof(uint32_t), ctx->stream));
         launch_query(ctx, g, any_hit != 0, static_cast<const float4 *>(d_rays), static_cast<uint4 *>(d_hits), static_cast<uint32_t>(n));
     }
     LRK_CUDA(cudaEventRecord(ctx->ev_end, ctx->stream));
@@ -1389,7 +1331,7 @@ int lrk_reduce_film(lrk_ctx *ctx, uint32_t root) {
     auto &api = lrk::nccl_api();
     const size_t count = static_cast<size_t>(ctx->scene.width) * ctx->scene.height * 4u;
     LRK_CUDA(cudaEventRecord(ctx->ev_reduce_begin, ctx->stream));
-    ncclResult_t r = api.reduce(ctx->d_film, ctx->d_film, count, ncclFloat, ncclSum, static_cast<int>(root), ctx->comm, ctx->stream);
+    ncclResult_t r = api.reduce(ctx->d_film.get(), ctx->d_film.get(), count, ncclFloat, ncclSum, static_cast<int>(root), ctx->comm, ctx->stream);
     if (r != ncclSuccess) return fail(ctx, LRK_ERR_CUDA, std::string("lrk_reduce_film: ncclReduce: ") + api.error_string(r));
     LRK_CUDA(cudaEventRecord(ctx->ev_reduce_end, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));

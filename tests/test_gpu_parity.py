@@ -214,6 +214,55 @@ def test_render_is_deterministic_and_independent_of_scheduling(cornell_small, gp
     assert st["closest_xforms"] + st["shadow_xforms"] <= cnt["xforms"]
 
 
+SURFACE_DISNEY, SURFACE_LAYERED, SURFACE_DISNEY_THIN, INTEGRATOR_VOLUME_PATH = 1, 7, 64, 1  # include/lrk.h
+
+
+def _hit_buckets(d):
+    """The hit buckets 1..10 the instances of a scene description use: the closure kind lrk_upload_scene gives each instance."""
+    from luisarender_b200 import _ffi as F
+    used = set()
+    for inst in d.instances[:d.instance_count]:
+        if inst.handle[0] & F.SHAPE_HAS_SURFACE:
+            s = d.surfaces[(inst.handle[1] >> 12) & 4095]
+            kind = s.type + 1  # Matte 1, Disney 2, Mirror 3, Glass 4, Plastic 5, Metal 6, Mix 7
+            if s.type == SURFACE_DISNEY and s.flags & F.SURFACE_DISNEY_TRANSMISSIVE:
+                kind = 8
+            if s.type == SURFACE_LAYERED:
+                kind = 9
+            if s.type == SURFACE_DISNEY and s.flags & SURFACE_DISNEY_THIN:
+                kind = 10
+            used.add(kind)
+    return used
+
+
+@pytest.mark.parametrize("name", ["environment", "layered", "disney_thin", "c4_medium"])
+def test_kernel_launch_count_follows_the_scene(name, gpu_renderer):
+    """stats()["kernel_launches"] restated from the scene.  Surface path, per pass: ray generation and film accumulation, and per depth
+    closest hit, classification, bucket 0's shade kernel, the shadow rays, the miss kernel when an environment light is present, and
+    one shade kernel per further hit bucket in use.  Volume path (C4), per depth: in-medium shadow rays, closest hit, the medium step,
+    bucket 0's surface step, the surface NEE rays, and the surface steps of buckets 1 and 2 when used."""
+    if name in ("disney_thin", "c4_medium"):  # the reference-render fixtures' scene texts (tests/test_ref_render.py)
+        key = {"disney_thin": "spheres_disney_thin", "c4_medium": "config_c4_full_scene"}[name]
+        src = bytes(np.load(REPO / "tests" / "golden" / "ref_renders.npz")[f"{key}/scene"]).decode()
+    else:
+        src = scenes.environment_scene() if name == "environment" else scenes.layered_box()
+    scene = Scene.from_source(src, REPO)
+    d = scene.desc()
+    buckets, depth = _hit_buckets(d), d.integrator.max_depth
+    volume = d.integrator.type == INTEGRATOR_VOLUME_PATH
+    # each scene exercises what it is here for
+    assert {"environment": d.environment.present, "layered": 9 in buckets, "disney_thin": 10 in buckets, "c4_medium": volume}[name]
+    if volume:
+        per_pass = 2 + depth * (5 + (1 in buckets) + (2 in buckets))
+    else:
+        per_pass = 2 + depth * (4 + bool(d.environment.present) + len(buckets))
+    gpu_renderer.upload(d)
+    gpu_renderer.render(0, d.camera.spp)
+    st = gpu_renderer.stats()
+    assert st["passes"] >= 1
+    assert st["kernel_launches"] == st["passes"] * per_pass
+
+
 def test_pixel_tile_sharding_is_bit_identical(spheres_small, gpu_renderer):
     d = spheres_small.desc()
     gpu_renderer.upload(d)
