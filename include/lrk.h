@@ -20,6 +20,8 @@
  *   lrk_render          <- ProgressiveIntegrator::Instance::_render_one_camera  src/integrators/wave_path.cpp:220-567
  *   lrk_render_adaptive / lrk_download_sample_counts / lrk_download_film_variance
  *                       <- (none: an extension, the reference has no adaptive sampling)  DESIGN.md §4 (Adaptive sampling)
+ *   option "gbuffer" / lrk_download_gbuffer / lrk_denoise
+ *                       <- (none: an extension, the reference has no G-buffer and no denoiser)  DESIGN.md §4 (G-buffer and denoiser)
  *   lrk_download_film   <- Film::Instance::download (convert_image + copy)      src/films/color.cpp:87-105
  *   lrk_download_film_raw / lrk_film_device_ptr
  *                       <- the raw (sum rgb, sum weight) float4 film buffer     src/films/color.cpp:107-130
@@ -41,7 +43,8 @@
 extern "C" {
 #endif
 
-#define LRK_ABI_VERSION 7u /* 7: lrk_render_adaptive, lrk_download_sample_counts, lrk_download_film_variance */
+#define LRK_ABI_VERSION 8u /* 7: lrk_render_adaptive, lrk_download_sample_counts, lrk_download_film_variance;
+                              8: option "gbuffer", lrk_download_gbuffer, lrk_denoise */
 
 typedef enum lrk_status {
     LRK_OK = 0,
@@ -549,7 +552,13 @@ int lrk_reduce_film(lrk_ctx *ctx, uint32_t root);
  *   "pin_host_buffers" (0/1)  the caller promises that the host arrays it passes to lrk_upload_scene / lrk_download_film*
  *                             stay allocated until lrk_destroy (or until the option is cleared); the library page-locks each
  *                             of them once (cudaHostRegister), so that every later transfer of the same buffer is a
- *                             full-speed DMA: the per-frame path of an animation, and of bench.py's end-to-end leg */
+ *                             full-speed DMA: the per-frame path of an animation, and of bench.py's end-to-end leg
+ *   "gbuffer" (0/1)           G-buffer mode, for lrk_denoise and external denoisers (see lrk_download_gbuffer).  The value the
+ *                             option has at a film clear (lrk_film_clear, lrk_upload_scene, lrk_balance_shards, the start of
+ *                             lrk_render_adaptive) decides whether the renders add to the G-buffer until the next clear, so that
+ *                             every sample of a G-buffer film has its G-buffer entry.  The film itself is bit-identical either
+ *                             way.  Surface integrator only: lrk_render / lrk_render_adaptive return LRK_ERR_UNSUPPORTED for
+ *                             the volume integrator with the option on */
 int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value);
 
 int lrk_film_clear(lrk_ctx *ctx);
@@ -585,6 +594,23 @@ int lrk_download_sample_counts(lrk_ctx *ctx, uint32_t *counts);
 /* v above (the variance of the pixel's mean luminance: a noise map) for every pixel of the last adaptive render: W*H float,
  * 0 outside this ctx's shard.  Same error as lrk_download_sample_counts. */
 int lrk_download_film_variance(lrk_ctx *ctx, float *v);
+
+/* G-buffer and denoiser (an extension: the reference has neither; DESIGN.md §4 (G-buffer and denoiser)).
+ * A G-buffer film holds per pixel, over its S samples in sample order: the sums of the first hit's albedo, of its shading normal
+ * (vertex normal face-forwarded to the geometric one, before any normal map, turned against the camera ray) and of its
+ * distance from the camera, and the number H of samples that hit a surface.  A miss adds zeros.  The albedo is the colour the
+ * hit's closure scales: Matte Kd, Disney colour, Mirror colour, Glass Kt, saturate(Plastic p[0..2]), Metal Kd tint, a Mix's two
+ * children weighted as the closure weights them, a Layered surface's bottom interface, 0 for a shape without a surface;
+ * image-textured slots are evaluated at the hit.  It also holds the luminance moments of include/lrk.h's adaptive mode.
+ * lrk_download_gbuffer: per pixel, albedo_cov = (sum albedo / S, H / S) and normal_depth = (normalize(sum n) or 0, sum t / H
+ * or 0) as W*H float4 each, and variance = v of the adaptive mode (+inf below two samples) as W*H float; all 0 for pixels without
+ * samples.  LRK_ERR_INVALID_ARGUMENT without a G-buffer film. */
+int lrk_download_gbuffer(lrk_ctx *ctx, float *albedo_cov, float *normal_depth, float *variance);
+/* The denoised film as W*H float4 in lrk_download_film's layout, alpha 1: an edge-avoiding à-trous filter over the
+ * albedo-demodulated colour, guided by the G-buffer and the variance (five steps; denoise.h).  The film is not modified.
+ * LRK_ERR_INVALID_ARGUMENT without a G-buffer film, LRK_ERR_UNSUPPORTED on a sharded context (world > 1): the other ranks hold the
+ * neighbouring pixels and the G-buffer is not reduced. */
+int lrk_denoise(lrk_ctx *ctx, float *rgba);
 
 /* rgba = (sum_rgb / max(sum_w, 1)) * scale, a = 1 : W*H float4 (src/films/color.cpp:87-93) */
 int lrk_download_film(lrk_ctx *ctx, float *rgba);

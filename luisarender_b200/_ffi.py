@@ -13,7 +13,7 @@ PKG_DIR = Path(__file__).resolve().parent
 REPO_DIR = PKG_DIR.parent
 LIB_DIR = PKG_DIR / "lib"
 
-LRK_ABI_VERSION = 7
+LRK_ABI_VERSION = 8
 TEX_ADDRESS_EDGE, TEX_ADDRESS_REPEAT, TEX_ADDRESS_MIRROR, TEX_ADDRESS_ZERO = 0, 1, 2, 3
 TEX_FILTER_POINT, TEX_FILTER_LINEAR = 0, 1
 TEX_ENCODING_LINEAR, TEX_ENCODING_SRGB, TEX_ENCODING_GAMMA = 0, 1, 2
@@ -158,7 +158,7 @@ LRK_SYMBOLS = [
     "lrk_set_option", "lrk_film_clear", "lrk_render", "lrk_download_film", "lrk_download_film_raw",
     "lrk_film_device_ptr", "lrk_film_normalize_to_host", "lrk_trace", "lrk_trace_device", "lrk_get_stats",
     "lrk_stream", "lrk_comm_unique_id", "lrk_comm_init", "lrk_reduce_film", "lrk_balance_shards", "lrk_assign_tiles",
-    "lrk_render_adaptive", "lrk_download_sample_counts", "lrk_download_film_variance",
+    "lrk_render_adaptive", "lrk_download_sample_counts", "lrk_download_film_variance", "lrk_download_gbuffer", "lrk_denoise",
 ]
 LRH_SYMBOLS = [
     "lrh_last_error", "lrh_scene_load", "lrh_scene_load_source", "lrh_scene_destroy", "lrh_scene_get_info",
@@ -231,5 +231,7 @@ def device_lib() -> C.CDLL:
         lib.lrk_render_adaptive.argtypes = [C.c_void_p, C.POINTER(Adaptive)]
         lib.lrk_download_sample_counts.argtypes = [C.c_void_p, C.c_void_p]
         lib.lrk_download_film_variance.argtypes = [C.c_void_p, C.c_void_p]
+        lib.lrk_download_gbuffer.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.lrk_denoise.argtypes = [C.c_void_p, C.c_void_p]
         lib._lrk_typed = True
     return lib

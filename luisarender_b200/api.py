@@ -164,6 +164,24 @@ class Renderer:
         self._check(self._lib.lrk_download_film_variance(self._ctx, out.ctypes.data), "lrk_download_film_variance")
         return out
 
+    def gbuffer(self) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """The guides of a G-buffer film (option "gbuffer" set before the film clear; include/lrk.h): albedo_cov [H, W, 4] (mean
+        first-hit albedo, fraction of samples that hit), normal_depth [H, W, 4] (normalised sum of normals, mean hit distance) and
+        variance [H, W] (variance of the pixel's mean luminance)."""
+        w, h = self._res
+        albedo_cov, normal_depth = np.empty((h, w, 4), dtype=np.float32), np.empty((h, w, 4), dtype=np.float32)
+        variance = np.empty((h, w), dtype=np.float32)
+        self._check(self._lib.lrk_download_gbuffer(self._ctx, albedo_cov.ctypes.data, normal_depth.ctypes.data, variance.ctypes.data),
+                    "lrk_download_gbuffer")
+        return albedo_cov, normal_depth, variance
+
+    def denoise(self) -> np.ndarray:
+        """The denoised film of a G-buffer film, [H, W, 4] float32 normalised like film(); the film itself is left as it is."""
+        w, h = self._res
+        out = np.empty((h, w, 4), dtype=np.float32)
+        self._check(self._lib.lrk_denoise(self._ctx, out.ctypes.data), "lrk_denoise")
+        return out
+
     def film(self, raw: bool = False, out: np.ndarray | None = None) -> np.ndarray:
         """The film as [H, W, 4] float32: normalised like the reference's convert_image, or the raw sums (raw=True).
         `out`: destination to reuse (with the option pin_host_buffers the library page-locks it once)."""

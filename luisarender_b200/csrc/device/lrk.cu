@@ -18,6 +18,8 @@
 #include "bvh_build.cuh"
 #include "comm.cuh"
 #include "adaptive.cuh"
+#include "gbuffer.cuh"
+#include "denoise.cuh"
 #include <cub/device/device_scan.cuh>
 
 using namespace lrk;
@@ -133,6 +135,11 @@ struct lrk_ctx {
     DeviceBuffer d_keep;// keep words and their exclusive scan (adaptive.cuh), 2 x (blocks + 1)
     DeviceBuffer d_scan_temp;
     bool adaptive_valid{false};// the film is the result of an adaptive render: sample counts and variance can be downloaded
+    // G-buffer mode (option "gbuffer"): the option's value is latched into gbuffer_film at every film clear, and a G-buffer film's
+    // renders add the first-hit sums (gbuffer.cuh) and the luminance moments (d_moments) until the next clear
+    bool gbuffer_option{false}, gbuffer_film{false};
+    DeviceBuffer d_gb_albedo, d_gb_normal, d_gb_hits;// per pixel (sum albedo, S), (sum n, sum t), H
+    DeviceBuffer d_dn_albedo_cov, d_dn_normal_depth, d_dn_variance, d_dn_ping[2];// lrk_denoise / lrk_download_gbuffer scratch
 
     ~lrk_ctx();
 };
@@ -328,6 +335,17 @@ void launch_accumulate(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_
     ctx->stats.kernel_launches++;
 }
 
+// The G-buffer sums of a pass (G-buffer films only): after depth 0's closest-hit trace, while pb.hit and ray_o / ray_d[0] still hold
+// the camera samples' hits and rays.
+void launch_gbuffer(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp) {
+    ScopedTimer t{ctx, CAT_OTHER};
+    const auto &pb = ctx->pb;
+    gbuffer_kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->scene, pb.ray_o[0], pb.ray_d[0], pb.hit, pixel_list, pixel_offset, npix, spp,
+                                                                            ctx->d_gb_albedo.get<float4>(), ctx->d_gb_normal.get<float4>(),
+                                                                            ctx->d_gb_hits.get<float>());
+    ctx->stats.kernel_launches++;
+}
+
 // Closest-hit traversal of the path queue of `depth`.  The volume pass launches it with alpha = false: the volume integrator rejects
 // non-opaque surfaces at upload.
 void launch_trace_closest(lrk_ctx *ctx, bool alpha, uint64_t n, uint32_t depth) {
@@ -363,6 +381,7 @@ int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset,
     // upper bound of the live queue at depth d is n; launch persistent-size grids and let kernels read *count
     for (uint32_t depth = 0; depth < sc.max_depth; depth++) {
         launch_trace_closest(ctx, ctx->any_non_opaque, n, depth);
+        if (depth == 0u && ctx->gbuffer_film) launch_gbuffer(ctx, pixel_list, pixel_offset, npix, spp);
         {
             ScopedTimer t{ctx, CAT_SHADE};
             if (sc.env_present) {
@@ -1002,6 +1021,7 @@ int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value) {
     else if (n == "time_kernels") ctx->time_kernels = value != 0;
     else if (n == "device_bvh") ctx->device_bvh = value != 0;
     else if (n == "strict_math") ctx->strict_math = value != 0;
+    else if (n == "gbuffer") ctx->gbuffer_option = value != 0;// takes effect at the next film clear
     else if (n == "pin_host_buffers") {
         ctx->pin_host = value != 0;
         if (!ctx->pin_host) unpin_all(ctx);
@@ -1026,6 +1046,33 @@ int lrk_film_clear(lrk_ctx *ctx) {
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     ctx->stats = lrk_stats{};
     ctx->adaptive_valid = false;
+    ctx->gbuffer_film = false;
+    if (ctx->gbuffer_option) {
+        LRK_CUDA(ctx->d_gb_albedo.reserve(npix * sizeof(float4)));
+        LRK_CUDA(ctx->d_gb_normal.reserve(npix * sizeof(float4)));
+        LRK_CUDA(ctx->d_gb_hits.reserve(npix * sizeof(float)));
+        LRK_CUDA(ctx->d_moments.reserve(npix * sizeof(float2)));
+        LRK_CUDA(cudaMemsetAsync(ctx->d_gb_albedo.get(), 0, npix * sizeof(float4), ctx->stream));
+        LRK_CUDA(cudaMemsetAsync(ctx->d_gb_normal.get(), 0, npix * sizeof(float4), ctx->stream));
+        LRK_CUDA(cudaMemsetAsync(ctx->d_gb_hits.get(), 0, npix * sizeof(float), ctx->stream));
+        LRK_CUDA(cudaMemsetAsync(ctx->d_moments.get(), 0, npix * sizeof(float2), ctx->stream));
+        LRK_CUDA(cudaStreamSynchronize(ctx->stream));
+        ctx->gbuffer_film = true;
+    }
+    return LRK_OK;
+}
+
+// The film accumulation adds the luminance moments to d_moments while one of these is alive (adaptive renders, G-buffer films).
+struct PassMoments {
+    lrk_ctx *ctx;
+    explicit PassMoments(lrk_ctx *c, bool on) : ctx{c} { ctx->pass_moments = on ? ctx->d_moments.get<float2>() : nullptr; }
+    ~PassMoments() { ctx->pass_moments = nullptr; }
+};
+
+// The G-buffer is written after depth 0's trace by the surface integrator's passes only.
+static int check_gbuffer_supported(lrk_ctx *ctx, bool gbuffer, const char *what) {
+    if (gbuffer && ctx->volume) return fail(ctx, LRK_ERR_UNSUPPORTED, std::string(what) + ": the G-buffer mode does not support the volume integrator");
+    if (gbuffer && ctx->scene.max_depth == 0u) return fail(ctx, LRK_ERR_UNSUPPORTED, std::string(what) + ": the G-buffer mode needs max_depth >= 1");
     return LRK_OK;
 }
 
@@ -1091,10 +1138,12 @@ int lrk_render(lrk_ctx *ctx, uint32_t spp_begin, uint32_t spp_end) {
     LRK_CUDA(cudaSetDevice(ctx->device));
     const uint32_t npix = ctx->npix_owned;
     if (npix == 0u || spp_end == spp_begin) return LRK_OK;
+    int rc = check_gbuffer_supported(ctx, ctx->gbuffer_film, "lrk_render");
+    if (rc) return rc;
     ctx->adaptive_valid = false;// the film no longer holds what the sample counts describe
     const PassShape sh = pass_shape(ctx, npix, spp_end - spp_begin);
-    int rc = alloc_paths(ctx, static_cast<uint64_t>(sh.chunk_pix) * sh.spp_per_pass);
-    if (rc) return rc;
+    if ((rc = alloc_paths(ctx, static_cast<uint64_t>(sh.chunk_pix) * sh.spp_per_pass))) return rc;
+    PassMoments moments{ctx, ctx->gbuffer_film};
     LRK_CUDA(cudaEventRecord(ctx->ev_begin, ctx->stream));
     if ((rc = render_passes(ctx, ctx->d_pixel_list.get<uint32_t>(), npix, spp_begin, spp_end, sh))) return rc;
     return finish_render(ctx, "lrk_render", static_cast<uint64_t>(npix) * (spp_end - spp_begin));
@@ -1126,7 +1175,9 @@ int lrk_render_adaptive(lrk_ctx *ctx, const lrk_adaptive *p) {
     if (!ctx || !ctx->has_scene) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_render_adaptive: no scene");
     if (!p || p->min_spp < 2u || p->max_spp < p->min_spp || !(p->threshold >= 0.f) || !std::isfinite(p->threshold))
         return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_render_adaptive: needs 2 <= min_spp <= max_spp and a finite threshold >= 0");
-    int rc = lrk_film_clear(ctx);
+    int rc = check_gbuffer_supported(ctx, ctx->gbuffer_option, "lrk_render_adaptive");
+    if (rc) return rc;
+    if ((rc = lrk_film_clear(ctx))) return rc;
     if (rc) return rc;
     if ((rc = alloc_adaptive(ctx))) return rc;
     const uint32_t npix = ctx->npix_owned;
@@ -1134,11 +1185,7 @@ int lrk_render_adaptive(lrk_ctx *ctx, const lrk_adaptive *p) {
         ctx->adaptive_valid = true;
         return LRK_OK;
     }
-    struct MomentsOn {// the film accumulation adds the moments for the duration of this call only
-        lrk_ctx *ctx;
-        ~MomentsOn() { ctx->pass_moments = nullptr; }
-    } moments_on{ctx};
-    ctx->pass_moments = ctx->d_moments.get<float2>();
+    PassMoments moments{ctx, true};
     const uint32_t *list = ctx->d_pixel_list.get<uint32_t>();
     const uint32_t *blocks = ctx->d_block_start[0].get<uint32_t>();
     uint32_t active = npix, nblocks = static_cast<uint32_t>(ctx->block_start.size() - 1u), c = 0u, next = p->min_spp;
@@ -1203,6 +1250,58 @@ int lrk_download_film_variance(lrk_ctx *ctx, float *v) {
                                                                                     ctx->d_sample_counts.get<uint32_t>(), out, n);
     LRK_CUDA(cudaGetLastError());
     LRK_CUDA(cudaMemcpyAsync(v, out, static_cast<size_t>(n) * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));
+    return LRK_OK;
+}
+
+// The guides of lrk_download_gbuffer / lrk_denoise into the denoiser's scratch buffers.
+static int gbuffer_guides(lrk_ctx *ctx, const char *what, bool zero_empty) {
+    if (!ctx->gbuffer_film) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, std::string(what) + ": the film is not a G-buffer film (set the option \"gbuffer\" before the film clear)");
+    const size_t n = ctx->film_pixels;
+    LRK_CUDA(ctx->d_dn_albedo_cov.reserve(n * sizeof(float4)));
+    LRK_CUDA(ctx->d_dn_normal_depth.reserve(n * sizeof(float4)));
+    LRK_CUDA(ctx->d_dn_variance.reserve(n * sizeof(float)));
+    denoise_guides_kernel<<<static_cast<unsigned>((n + kBlock - 1u) / kBlock), kBlock, 0, ctx->stream>>>(
+        ctx->d_film.get<float4>(), ctx->d_moments.get<float2>(), ctx->d_gb_albedo.get<float4>(), ctx->d_gb_normal.get<float4>(), ctx->d_gb_hits.get<float>(),
+        ctx->d_dn_albedo_cov.get<DenoiseVec4>(), ctx->d_dn_normal_depth.get<DenoiseVec4>(), ctx->d_dn_variance.get<float>(), static_cast<uint32_t>(n), zero_empty);
+    LRK_CUDA(cudaGetLastError());
+    return LRK_OK;
+}
+
+int lrk_download_gbuffer(lrk_ctx *ctx, float *albedo_cov, float *normal_depth, float *variance) {
+    if (!ctx || !ctx->has_scene || !albedo_cov || !normal_depth || !variance)
+        return fail(ctx, LRK_ERR_NO_SCENE, "lrk_download_gbuffer: no scene / null buffer");
+    LRK_CUDA(cudaSetDevice(ctx->device));
+    int rc = gbuffer_guides(ctx, "lrk_download_gbuffer", true);
+    if (rc) return rc;
+    const size_t n = ctx->film_pixels;
+    LRK_CUDA(cudaMemcpyAsync(albedo_cov, ctx->d_dn_albedo_cov.get(), n * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
+    LRK_CUDA(cudaMemcpyAsync(normal_depth, ctx->d_dn_normal_depth.get(), n * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
+    LRK_CUDA(cudaMemcpyAsync(variance, ctx->d_dn_variance.get(), n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));
+    return LRK_OK;
+}
+
+// Filter and schedule: denoise.h.  The film is read, never written; the output goes through lrk_download_film's staging buffer.
+int lrk_denoise(lrk_ctx *ctx, float *rgba) {
+    if (!ctx || !ctx->has_scene || !rgba) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_denoise: no scene / null buffer");
+    LRK_CUDA(cudaSetDevice(ctx->device));
+    if (!ctx->gbuffer_film) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_denoise: the film is not a G-buffer film (set the option \"gbuffer\" before the film clear)");
+    if (ctx->world > 1u) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_denoise: a sharded context holds only its own tiles' G-buffer");
+    int rc = gbuffer_guides(ctx, "lrk_denoise", false);
+    if (rc) return rc;
+    const uint32_t w = ctx->scene.width, h = ctx->scene.height, n = w * h;
+    const unsigned grid = (n + kBlock - 1u) / kBlock;
+    for (auto &b : ctx->d_dn_ping) LRK_CUDA(b.reserve(static_cast<size_t>(n) * sizeof(float4)));
+    const auto *ac = ctx->d_dn_albedo_cov.get<const DenoiseVec4>(), *nd = ctx->d_dn_normal_depth.get<const DenoiseVec4>();
+    DenoiseVec4 *ping[2] = {ctx->d_dn_ping[0].get<DenoiseVec4>(), ctx->d_dn_ping[1].get<DenoiseVec4>()};
+    denoise_input_kernel<<<grid, kBlock, 0, ctx->stream>>>(ctx->scene, ctx->d_film.get<float4>(), ac, ctx->d_dn_variance.get<float>(), ping[0], n);
+    for (int it = 0; it < kDenoiseIterations; it++)
+        denoise_atrous_kernel<<<grid, kBlock, 0, ctx->stream>>>(ping[it & 1], ac, nd, ping[(it & 1) ^ 1], w, h, 1 << it);
+    denoise_output_kernel<<<grid, kBlock, 0, ctx->stream>>>(ping[kDenoiseIterations & 1], ac, ctx->d_film_out.get<DenoiseVec4>(), n);
+    LRK_CUDA(cudaGetLastError());
+    pin_range(ctx, rgba, static_cast<size_t>(n) * sizeof(float4));
+    LRK_CUDA(cudaMemcpyAsync(rgba, ctx->d_film_out.get(), static_cast<size_t>(n) * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     return LRK_OK;
 }

@@ -12,6 +12,9 @@
 //
 // Adaptive sampling (an extension; the reference has none): `--adaptive <threshold>` renders with lrk_render_adaptive, from
 // `--adaptive-min-spp` samples per pixel (default 16, at most the camera's spp) up to the camera's spp.
+//
+// Denoising (an extension): `--denoise` renders G-buffer films (lrk_set_option("gbuffer")) and also writes lrk_denoise's image to
+// <stem>.denoised<ext> next to the camera's file, which is written as without it.  One GPU only: the G-buffer is not reduced.
 #include <sys/stat.h>
 #include <sys/wait.h>
 #include <unistd.h>
@@ -39,6 +42,7 @@ void usage() {
                 "      --gpus <n>               Render on n GPUs, one process each (tiles sharded, films summed on GPU 0)\n"
                 "      --adaptive <threshold>   Adaptive sampling: stop 8x4 pixel blocks whose relative error is below threshold\n"
                 "      --adaptive-min-spp <n>   Samples per pixel of the first adaptive round (default 16, at most the camera's spp)\n"
+                "      --denoise                Also write the denoised image to <stem>.denoised<ext> (one GPU only)\n"
                 "  -h, --help                   Display this help message\n");
 }
 
@@ -123,11 +127,19 @@ int launch_ranks(int gpus, int argc, char *argv[]) {
     return worst;
 }
 
+// <dir>/<stem>.denoised<ext> for <dir>/<stem><ext>
+std::string denoised_path(const std::string &file) {
+    const size_t slash = file.find_last_of('/'), dot = file.find_last_of('.');
+    if (dot == std::string::npos || (slash != std::string::npos && dot < slash)) return file + ".denoised";
+    return file.substr(0, dot) + ".denoised" + file.substr(dot);
+}
+
 }// namespace
 
 int main(int argc, char *argv[]) {
     std::string backend, scene_path;
     int device = -1, gpus = 1;
+    bool denoise = false;
     std::string adaptive_arg, min_spp_arg;
     std::vector<std::string> keys, values;
     auto add_macro = [&](const std::string &d) {
@@ -169,6 +181,7 @@ int main(int argc, char *argv[]) {
         else if (a.rfind("--adaptive=", 0) == 0) adaptive_arg = a.substr(11);
         else if (a == "--adaptive-min-spp") min_spp_arg = need("count");
         else if (a.rfind("--adaptive-min-spp=", 0) == 0) min_spp_arg = a.substr(19);
+        else if (a == "--denoise") denoise = true;
         else if (a == "-D" || a == "--define") add_macro(need("definition"));
         else if (a.rfind("-D", 0) == 0) add_macro(a.substr(2));
         else if (!a.empty() && a[0] == '-') std::fprintf(stderr, "[warning] Unrecognized options: %s\n", a.c_str());
@@ -205,6 +218,10 @@ int main(int argc, char *argv[]) {
         }
         min_spp = static_cast<uint32_t>(v);
     }
+    if (denoise && (gpus > 1 || env_u32("WORLD_SIZE", 1u) > 1u)) {
+        std::fprintf(stderr, "[error] --denoise renders on one GPU: the G-buffer of sharded renders is not reduced.\n");
+        return -1;
+    }
     for (auto &c : backend) c = static_cast<char>(std::tolower(static_cast<unsigned char>(c)));
     if (backend != "cuda") die("Backend '" + backend + "' is not available: this build ships the sm_90a CUDA backend only (-b cuda).");
     if (gpus > 1) return launch_ranks(gpus, argc, argv);
@@ -235,6 +252,7 @@ int main(int argc, char *argv[]) {
     cfg.device_index = device;
     lrk_ctx *ctx = nullptr;
     if (int rc = lrk_create(&cfg, &ctx); rc != 0) die("Failed to create the CUDA device context (lrk_create = " + std::to_string(rc) + ").");
+    if (denoise && lrk_set_option(ctx, "gbuffer", 1) != 0) die(lrk_last_error(ctx));
     if (world > 1u) {
         uint8_t id[LRK_COMM_ID_BYTES];
         exchange_comm_id(rank, id);
@@ -291,6 +309,12 @@ int main(int argc, char *argv[]) {
         const char *file = lrh_scene_camera_file(scene, cam);
         if (lrh_save_image(file, pixels.data(), w, h) != 0) std::fprintf(stderr, "[warning] %s\n", lrh_last_error());
         else std::printf("[info] Saved film to '%s'.\n", file);
+        if (denoise) {
+            if (lrk_denoise(ctx, pixels.data()) != 0) die(lrk_last_error(ctx));
+            const std::string out = denoised_path(file);
+            if (lrh_save_image(out.c_str(), pixels.data(), w, h) != 0) std::fprintf(stderr, "[warning] %s\n", lrh_last_error());
+            else std::printf("[info] Saved denoised film to '%s'.\n", out.c_str());
+        }
     }
     lrk_destroy(ctx);
     lrh_scene_destroy(scene);
