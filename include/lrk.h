@@ -558,7 +558,13 @@ int lrk_reduce_film(lrk_ctx *ctx, uint32_t root);
  *                             lrk_render_adaptive) decides whether the renders add to the G-buffer until the next clear, so that
  *                             every sample of a G-buffer film has its G-buffer entry.  The film itself is bit-identical either
  *                             way.  Surface integrator only: lrk_render / lrk_render_adaptive return LRK_ERR_UNSUPPORTED for
- *                             the volume integrator with the option on */
+ *                             the volume integrator with the option on
+ *   "light_tree" (0/1)        light selection of next-event estimation from a light tree (bounds, power and normal cone per node)
+ *                             over every instance that carries a light, instead of the reference's uniform sampler over the light
+ *                             nodes.  Read at lrk_upload_scene; the tree is built there from the scene description.  Another value
+ *                             -> LRK_ERR_INVALID_ARGUMENT.  Surface integrator only: lrk_upload_scene returns LRK_ERR_UNSUPPORTED
+ *                             for the volume integrator with the option on.  A scene with one emissive instance renders bit for bit
+ *                             as without it.  LRK_ABI_VERSION stays 8: no layout or signature changed */
 int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value);
 
 int lrk_film_clear(lrk_ctx *ctx);

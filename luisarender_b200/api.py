@@ -91,9 +91,14 @@ def save_image(path: str | Path, rgba: np.ndarray) -> None:
 
 
 class Renderer:
-    """One GPU context. Fails loudly when libb200pt.so or a CUDA device is missing (no CPU fallback)."""
+    """One GPU context. Fails loudly when libb200pt.so or a CUDA device is missing (no CPU fallback).
 
-    def __init__(self, device_index: int = -1, max_paths_per_pass: int = 0):
+    ``light_tree=True`` sets the option "light_tree" (include/lrk.h): from the next upload on, next-event estimation picks its
+    lights from a light tree by power, distance and orientation instead of uniformly (surface integrator only)."""
+
+    def __init__(self, device_index: int = -1, max_paths_per_pass: int = 0, light_tree: bool = False):
+        if light_tree not in (0, 1):
+            raise ValueError(f"light_tree is False or True, not {light_tree!r}")
         self._lib = F.device_lib()
         cfg = F.DeviceCfg(device_index, 0, max_paths_per_pass)
         self._ctx = C.c_void_p()
@@ -101,6 +106,8 @@ class Renderer:
         if rc != 0:
             raise RuntimeError(f"lrk_create failed ({rc}): no usable CUDA device")
         self._res = None
+        if light_tree:
+            self.set_option("light_tree", 1)
 
     def _check(self, rc: int, what: str):
         if rc != 0:
@@ -136,6 +143,7 @@ class Renderer:
         self._check(self._lib.lrk_balance_shards(self._ctx, rank, world, tile_size, probe_spp), "lrk_balance_shards")
 
     def set_option(self, name: str, value: int):
+        """lrk_set_option; e.g. ("light_tree", 1): light-tree selection of next-event lights from the next upload on."""
         self._check(self._lib.lrk_set_option(self._ctx, name.encode(), value), f"lrk_set_option({name})")
 
     def clear(self):

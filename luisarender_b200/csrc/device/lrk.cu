@@ -61,7 +61,7 @@ private:
 
 struct DeviceArrays {
     DeviceBuffer vertices, triangles, alias, pdf, meshes, inst_handles, inst_kind, inst_o2w, inst_xform, bvh_nodes, traversal_overflow, sobol, vdc, vdc_inv, pmj, blue_noise, pmj_pixels, zsobol_hash, sampler, build_scratch, mesh_bounds, inst_mesh, visible_ids, scene_copy, media, textures, texels, env_alias, env_pdf,
-        tri_verts, surfaces, lights, light_handles, camera;
+        tri_verts, surfaces, lights, light_handles, camera, lt_nodes, lt_light_inst, lt_trail, lt_inst_light;
 };
 
 enum KernelCategory { CAT_TRACE_CLOSEST = 0, CAT_TRACE_SHADOW = 1, CAT_SHADE = 2, CAT_OTHER = 3, CAT_COUNT = 4 };
@@ -140,6 +140,10 @@ struct lrk_ctx {
     bool gbuffer_option{false}, gbuffer_film{false};
     DeviceBuffer d_gb_albedo, d_gb_normal, d_gb_hits;// per pixel (sum albedo, S), (sum n, sum t), H
     DeviceBuffer d_dn_albedo_cov, d_dn_normal_depth, d_dn_variance, d_dn_ping[2];// lrk_denoise / lrk_download_gbuffer scratch
+    // light tree (option "light_tree"): the option's value at lrk_upload_scene is latched into light_tree, which selects the shade
+    // kernels' instantiations
+    bool light_tree_option{false}, light_tree{false};
+    DeviceLightTree light_tree_rec{};// the record after the scene's device copy (scene.cuh)
 
     ~lrk_ctx();
 };
@@ -398,8 +402,8 @@ int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset,
                 // IEEE arithmetic
                 const bool strict = ctx->strict_math || (kind >= 3u && kind <= 7u) || kind >= 9u;
                 const int blocks = blocks_for(ctx, n, ctx->grid_shade[strict ? 1 : 0][kind]);
-                if (strict) strict::launch_shade(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
-                else fast::launch_shade(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
+                if (strict) strict::launch_shade(kind, ctx->textured, ctx->light_tree, blocks, ctx->stream, sc, pb, depth);
+                else fast::launch_shade(kind, ctx->textured, ctx->light_tree, blocks, ctx->stream, sc, pb, depth);
                 ctx->stats.kernel_launches++;
             }
         }
@@ -588,6 +592,53 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
     return LRK_OK;
 }
 
+// The light tree of the option "light_tree" (light_tree.h) over every instance that carries a light - not only the first light_count
+// handles - from the scene's own arrays: world-space triangles, the emission (the mean of max(texel, 0) of an image emission) and the
+// sidedness.  tree_inst: per tree light its instance; inst_light: per instance its tree light, kLightTreeNone for instances without
+// a light or without power.
+int build_light_tree(lrk_ctx *ctx, const lrk_scene_desc *s, LightTreeBuild &tree, std::vector<uint32_t> &tree_inst, std::vector<uint32_t> &inst_light) {
+    std::vector<LightTreeEmitter> emitters;
+    inst_light.assign(s->instance_count, kLightTreeNone);
+    std::vector<double> tris;
+    for (uint32_t i = 0; i < s->instance_count; i++) {
+        const auto &inst = s->instances[i];
+        if (!(inst.handle[0] & LRK_SHAPE_HAS_LIGHT)) continue;
+        const uint32_t tag = inst.handle[1] & 4095u;
+        if (tag >= s->light_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: light tag out of range");
+        const lrk_light &light = s->lights[tag];
+        double rgb[3] = {light.emission[0], light.emission[1], light.emission[2]};
+        if (light.emission_tex != 0u) {
+            const lrk_texture &t = s->textures[light.emission_tex - 1u];
+            const size_t texels = static_cast<size_t>(t.width) * t.height;
+            double sum[3] = {0.0, 0.0, 0.0};
+            for (size_t k = 0; k < texels; k++)
+                for (int c = 0; c < 3; c++) sum[c] += std::max(static_cast<double>(s->texels[(t.texel_offset + k) * 4u + c]), 0.0);
+            for (int c = 0; c < 3; c++) rgb[c] = sum[c] / static_cast<double>(texels);
+        }
+        for (double &c : rgb) c = std::max(c, 0.0);
+        const double lum = 0.2126 * rgb[0] + 0.7152 * rgb[1] + 0.0722 * rgb[2];
+        const lrk_mesh &mesh = s->meshes[inst.mesh];
+        const float *m = inst.object_to_world;// row-major 3x4
+        tris.clear();
+        for (uint32_t t = 0; t < mesh.triangle_count; t++) {
+            const lrk_triangle &tri = s->triangles[mesh.triangle_offset + t];
+            for (uint32_t v : {tri.i0, tri.i1, tri.i2}) {
+                const lrk_vertex &vx = s->vertices[mesh.vertex_offset + v];
+                for (int r = 0; r < 3; r++)
+                    tris.push_back(static_cast<double>(m[4 * r]) * vx.p[0] + static_cast<double>(m[4 * r + 1]) * vx.p[1] +
+                                   static_cast<double>(m[4 * r + 2]) * vx.p[2] + m[4 * r + 3]);
+            }
+        }
+        inst_light[i] = static_cast<uint32_t>(emitters.size());
+        tree_inst.push_back(i);
+        emitters.push_back(light_tree_emitter(tris, lum * light.scale, light.two_sided != 0u));
+    }
+    tree = light_tree_build(emitters);
+    for (uint32_t i = 0; i < s->instance_count; i++)
+        if (inst_light[i] != kLightTreeNone && !(emitters[inst_light[i]].phi > 0.0)) inst_light[i] = kLightTreeNone;
+    return LRK_OK;
+}
+
 }// namespace
 
 // The one teardown of a context, run with its device current and its stream idle (lrk_destroy, or a failed lrk_create).  The device
@@ -702,6 +753,9 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: an environment medium needs the volume path integrator (MegaVPTNaive)");
     }
     if (s->integrator.max_depth > kMaxDepthSlots - 1u) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: max depth > 63");
+    if (ctx->light_tree_option && s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
+        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: the light tree (option light_tree) serves the surface integrator only; the volume "
+                                              "integrator selects its lights uniformly");
     if (s->camera.resolution[0] > 65535u || s->camera.resolution[1] > 65535u)
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: film larger than 65535 pixels per side");
     if (s->light_count == 0u && !s->environment.present)// !pipeline().has_lighting(), wave_path.cpp:224-228
@@ -859,6 +913,15 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     }
     for (uint32_t i = 0; i < s->instance_count; i++) std::memcpy(&xform[i * 16u + 12u], &mesh_root[s->instances[i].mesh], 4);
     if ((rc = upload(ctx, a.inst_xform, xform.data(), xform.size()))) return rc;
+    LightTreeBuild tree;
+    std::vector<uint32_t> tree_inst, inst_light;
+    if (ctx->light_tree_option) {
+        if ((rc = build_light_tree(ctx, s, tree, tree_inst, inst_light))) return rc;
+        if ((rc = upload(ctx, a.lt_nodes, tree.nodes.data(), tree.nodes.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_light_inst, tree_inst.data(), tree_inst.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_trail, tree.trail.data(), tree.trail.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_inst_light, inst_light.data(), inst_light.size()))) return rc;
+    }
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
 
     auto &sc = ctx->scene;
@@ -931,16 +994,26 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     sc.media = a.media.get<const lrk_medium>();
     sc.medium_count = s->medium_count;
     sc.env_medium_tag = s->environment_medium_tag;
+    ctx->light_tree = ctx->light_tree_option;
+    {
+        auto &lt = ctx->light_tree_rec;
+        lt.nodes = ctx->light_tree && !tree.nodes.empty() ? a.lt_nodes.get<const LightTreeNode>() : nullptr;
+        lt.light_inst = ctx->light_tree ? a.lt_light_inst.get<const uint32_t>() : nullptr;
+        lt.trail = ctx->light_tree ? a.lt_trail.get<const unsigned long long>() : nullptr;
+        lt.inst_light = ctx->light_tree ? a.lt_inst_light.get<const uint32_t>() : nullptr;
+    }
 
     const size_t npix = static_cast<size_t>(sc.width) * sc.height;
     ctx->film_pixels = 0;
     LRK_CUDA(ctx->d_film.reserve(npix * sizeof(float4)));
     LRK_CUDA(ctx->d_film_out.reserve(npix * sizeof(float4)));
     ctx->film_pixels = npix;
-    {// the scene record itself in device memory, for the out-of-line device functions (DeviceScene::self)
-        LRK_CUDA(a.scene_copy.reserve(sizeof(DeviceScene)));
+    {// the scene record itself in device memory, for the out-of-line device functions (DeviceScene::self), and the light tree's after it
+        LRK_CUDA(a.scene_copy.reserve(sizeof(DeviceScene) + sizeof(DeviceLightTree)));
         sc.self = a.scene_copy.get<const DeviceScene>();
         LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get(), &sc, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
+        LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get<char>() + sizeof(DeviceScene), &ctx->light_tree_rec, sizeof(DeviceLightTree), cudaMemcpyHostToDevice,
+                                 ctx->stream));
         LRK_CUDA(cudaStreamSynchronize(ctx->stream));
     }
     ctx->has_scene = true;
@@ -1022,6 +1095,10 @@ int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value) {
     else if (n == "device_bvh") ctx->device_bvh = value != 0;
     else if (n == "strict_math") ctx->strict_math = value != 0;
     else if (n == "gbuffer") ctx->gbuffer_option = value != 0;// takes effect at the next film clear
+    else if (n == "light_tree") {// takes effect at the next lrk_upload_scene
+        if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_tree is 0 or 1");
+        ctx->light_tree_option = value != 0;
+    }
     else if (n == "pin_host_buffers") {
         ctx->pin_host = value != 0;
         if (!ctx->pin_host) unpin_all(ctx);

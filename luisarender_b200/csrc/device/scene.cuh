@@ -3,6 +3,7 @@
 #include <cstdint>
 
 #include "../../../include/lrk.h"
+#include "light_tree.h"
 #include "vecmath.cuh"
 
 namespace lrk {
@@ -67,5 +68,18 @@ struct DeviceScene {
     uint32_t medium_count;
     uint32_t env_medium_tag;// LRK_MEDIUM_INVALID_TAG: none
 };
+
+// The light tree's arrays (option "light_tree", light_tree.h), in device memory right after the record DeviceScene::self points
+// to: kept out of the kernel parameter, so that the parameter layout - and the code - of every kernel stays what it is without the
+// tree.  All null unless the option was on at lrk_upload_scene (nodes also when no emitter has power).
+struct DeviceLightTree {
+    const LightTreeNode *nodes;
+    const uint32_t *light_inst;        // per tree light: its instance
+    const unsigned long long *trail;   // per tree light: its root-to-leaf bit trail
+    const uint32_t *inst_light;        // per instance: its tree light, kLightTreeNone for none
+};
+__device__ __forceinline__ const DeviceLightTree &light_tree_of(const DeviceScene &sc) {
+    return *reinterpret_cast<const DeviceLightTree *>(sc.self + 1);
+}
 
 }// namespace lrk

@@ -30,21 +30,21 @@ int grid_of(Kernel kernel, int block, int sm_count) {
     return (per_sm > 0 ? per_sm : 1) * sm_count;
 }
 
-// calls f(kernel) with the shade kernel instantiation of (kind, textured)
-template<typename F>
+// calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection)
+template<uint32_t SEL, typename F>
 void with_shade_kernel(uint32_t kind, bool textured, F &&f) {
     switch (kind) {
-        case 0u: textured ? f(shade_kernel<0u, true>) : f(shade_kernel<0u, false>); break;// emitter-only hits: a light's image emission
-        case 1u: textured ? f(shade_kernel<1u, true>) : f(shade_kernel<1u, false>); break;
-        case 2u: textured ? f(shade_kernel<2u, true>) : f(shade_kernel<2u, false>); break;
-        case 3u: textured ? f(shade_kernel<3u, true>) : f(shade_kernel<3u, false>); break;
-        case 4u: textured ? f(shade_kernel<4u, true>) : f(shade_kernel<4u, false>); break;
-        case 5u: textured ? f(shade_kernel<5u, true>) : f(shade_kernel<5u, false>); break;
-        case 6u: textured ? f(shade_kernel<6u, true>) : f(shade_kernel<6u, false>); break;
-        case 7u: textured ? f(shade_kernel<7u, true>) : f(shade_kernel<7u, false>); break;
-        case 8u: textured ? f(shade_kernel<8u, true>) : f(shade_kernel<8u, false>); break;
-        case 9u: textured ? f(shade_kernel<9u, true>) : f(shade_kernel<9u, false>); break;
-        default: textured ? f(shade_kernel<10u, true>) : f(shade_kernel<10u, false>); break;
+        case 0u: textured ? f(shade_kernel<0u, true, SEL>) : f(shade_kernel<0u, false, SEL>); break;// emitter-only hits: a light's image emission
+        case 1u: textured ? f(shade_kernel<1u, true, SEL>) : f(shade_kernel<1u, false, SEL>); break;
+        case 2u: textured ? f(shade_kernel<2u, true, SEL>) : f(shade_kernel<2u, false, SEL>); break;
+        case 3u: textured ? f(shade_kernel<3u, true, SEL>) : f(shade_kernel<3u, false, SEL>); break;
+        case 4u: textured ? f(shade_kernel<4u, true, SEL>) : f(shade_kernel<4u, false, SEL>); break;
+        case 5u: textured ? f(shade_kernel<5u, true, SEL>) : f(shade_kernel<5u, false, SEL>); break;
+        case 6u: textured ? f(shade_kernel<6u, true, SEL>) : f(shade_kernel<6u, false, SEL>); break;
+        case 7u: textured ? f(shade_kernel<7u, true, SEL>) : f(shade_kernel<7u, false, SEL>); break;
+        case 8u: textured ? f(shade_kernel<8u, true, SEL>) : f(shade_kernel<8u, false, SEL>); break;
+        case 9u: textured ? f(shade_kernel<9u, true, SEL>) : f(shade_kernel<9u, false, SEL>); break;
+        default: textured ? f(shade_kernel<10u, true, SEL>) : f(shade_kernel<10u, false, SEL>); break;
     }
 }
 
@@ -61,7 +61,7 @@ void with_volume_surface_kernel(uint32_t kind, bool textured, F &&f) {
 
 int shade_grid(uint32_t kind, int sm_count) {
     int g = 1;
-    with_shade_kernel(kind, false, [&](auto kernel) { g = grid_of(kernel, kShadeBlock, sm_count); });
+    with_shade_kernel<kLightSelectUniform>(kind, false, [&](auto kernel) { g = grid_of(kernel, kShadeBlock, sm_count); });
     return g;
 }
 
@@ -73,8 +73,11 @@ int volume_surface_grid(uint32_t kind, int sm_count) {
     return g;
 }
 
-void launch_shade(uint32_t kind, bool textured, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth) {
-    with_shade_kernel(kind, textured, [&](auto kernel) { kernel<<<blocks, kShadeBlock, 0, stream>>>(sc, pb, depth); });
+void launch_shade(uint32_t kind, bool textured, bool light_tree, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb,
+                  uint32_t depth) {
+    const auto launch = [&](auto kernel) { kernel<<<blocks, kShadeBlock, 0, stream>>>(sc, pb, depth); };
+    if (light_tree) with_shade_kernel<kLightSelectTree>(kind, textured, launch);
+    else with_shade_kernel<kLightSelectUniform>(kind, textured, launch);
 }
 
 void launch_volume_medium(int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth) {

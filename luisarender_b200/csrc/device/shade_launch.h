@@ -15,8 +15,10 @@ namespace lrk {
     int shade_grid(uint32_t kind, int sm_count);                                                                                             \
     int volume_medium_grid(int sm_count);                                                                                                    \
     int volume_surface_grid(uint32_t kind, int sm_count);                                                                                    \
-    /* `textured`: the instantiation that evaluates image-textured parameters / normal maps */                                               \
-    void launch_shade(uint32_t kind, bool textured, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth); \
+    /* `textured`: the instantiation that evaluates image-textured parameters / normal maps; `light_tree`: the one whose next-event */      \
+    /* estimation selects lights with the light tree (option "light_tree") */                                                                \
+    void launch_shade(uint32_t kind, bool textured, bool light_tree, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, \
+                      uint32_t depth);                                                                                                       \
     void launch_volume_medium(int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth);                \
     void launch_volume_surface(uint32_t kind, bool textured, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb,  \
                                uint32_t depth);                                                                                              \

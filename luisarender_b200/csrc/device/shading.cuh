@@ -239,9 +239,32 @@ __device__ __forceinline__ LightEval diffuse_light_evaluate(const DeviceScene &s
     return e;
 }
 
-template<bool TEX = true>
-__device__ __forceinline__ LightEval evaluate_hit(const DeviceScene &sc, const Interaction &it, V3 p_from) {
+// Light selection of next-event estimation: the reference's uniform sampler over the light NODES (uniform.cpp), or the light tree
+// of the option "light_tree" over the emissive instances (light_tree.h)
+enum LightSelect : uint32_t { kLightSelectUniform = 0u, kLightSelectTree = 1u };
+
+// The descents of the light tree, out of line so that the shade kernels' register allocation does not grow with them.
+__device__ __noinline__ inline uint32_t light_tree_sample(const LightTreeNode *nodes, V3 p, float u, float &pmf) {
+    return light_tree_walk<true>(nodes, p.x, p.y, p.z, u, 0ull, pmf);
+}
+__device__ __noinline__ inline float light_tree_pmf(const LightTreeNode *nodes, const uint32_t *inst_light, const unsigned long long *trail, V3 p,
+                                                    uint32_t inst) {
+    const uint32_t l = __ldg(inst_light + inst);
+    if (l == kLightTreeNone) return 0.f;// an emitter without power
+    float pmf;
+    light_tree_walk<false>(nodes, p.x, p.y, p.z, 0.f, __ldg(trail + l), pmf);
+    return pmf;
+}
+
+// `inst`: the instance hit (used by the light tree only)
+template<bool TEX = true, uint32_t SEL = kLightSelectUniform>
+__device__ __forceinline__ LightEval evaluate_hit(const DeviceScene &sc, const Interaction &it, V3 p_from, uint32_t inst = 0u) {
     LightEval e = diffuse_light_evaluate<TEX>(sc, it, p_from);
+    if (SEL == kLightSelectTree) {
+        const DeviceLightTree &lt = light_tree_of(sc);
+        e.pdf *= (1.f - sc.env_prob) * light_tree_pmf(lt.nodes, lt.inst_light, lt.trail, p_from, inst);
+        return e;
+    }
     float n = static_cast<float>(sc.light_count);
     e.pdf *= (1.f - sc.env_prob) / n;// uniform.cpp:63 (env_prob = 0 without an environment)
     return e;
@@ -259,7 +282,7 @@ struct LightSample {
 // `p_shading`: it_from.p_shading(), the point the light's emission and pdf are evaluated from (diffuse.cpp:62-86) - the hit point
 // for a surface interaction, but the WORLD ORIGIN for the volume integrator's Interaction{ray->origin()}, whose shading point is
 // never set (mega_vpt_naive.cpp:283-285; the reference's renders carry that, so this library does too)
-template<bool TEX = true>
+template<bool TEX = true, uint32_t SEL = kLightSelectUniform>
 __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, const Interaction &it_from, V3 p_shading, float u_sel, float u0, float u1) {
     LightSample s;
     float n = static_cast<float>(sc.light_count);
@@ -268,7 +291,30 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
     bool is_env = ep == 1.f;
     uint32_t tag = 0u;
     float sel_prob = 1.f;
-    if (ep == 0.f) {
+    if (SEL == kLightSelectTree) {// the environment keeps its probability; the tree divides the rest
+        float uu = u_sel;
+        if (ep != 0.f && ep != 1.f) {
+            uu = (u_sel - ep) / (1.f - ep);
+            is_env = u_sel < ep;
+        }
+        if (is_env) {
+            sel_prob = ep;
+        } else {
+            const DeviceLightTree &lt = light_tree_of(sc);
+            const LightTreeNode *nodes = lt.nodes;
+            float pmf = 0.f;
+            const uint32_t l = nodes != nullptr ? light_tree_sample(nodes, it_from.pg, uu, pmf) : kLightTreeNone;
+            if (l == kLightTreeNone) {// no emitter can reach the point: nothing to trace
+                s.eval.L = v3(0.f);
+                s.eval.pdf = 0.f;
+                s.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
+                s.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
+                return s;
+            }
+            tag = __ldg(lt.light_inst + l);// the instance itself
+            sel_prob = ep == 0.f ? pmf : (1.f - ep) * pmf;
+        }
+    } else if (ep == 0.f) {
         tag = static_cast<uint32_t>(clampf(u_sel * n, 0.f, n - 1.f));
         sel_prob = 1.f / n;
     } else if (ep != 1.f) {
@@ -286,7 +332,9 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
         s.ray_d_tmax = make_float4(wi.x, wi.y, wi.z, kFltMax);
         return s;
     }
-    const lrk_light_handle handle = sc.light_handles[tag];
+    lrk_light_handle handle;
+    if (SEL == kLightSelectTree) handle.instance_id = tag;
+    else handle = sc.light_handles[tag];
     ShapeHandle light_inst = decode_handle(__ldg(sc.inst_handles + handle.instance_id));
     const lrk_mesh mesh = sc.meshes[light_inst.mesh];
     // sample_alias_table: src/util/sampling.h:38-50
@@ -312,9 +360,9 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
     return s;
 }
 
-template<bool TEX = true>
+template<bool TEX = true, uint32_t SEL = kLightSelectUniform>
 __device__ __forceinline__ LightSample sample_light(const DeviceScene &sc, const Interaction &it_from, float u_sel, float u0, float u1) {
-    return sample_light_from<TEX>(sc, it_from, it_from.pg, u_sel, u0, u1);
+    return sample_light_from<TEX, SEL>(sc, it_from, it_from.pg, u_sel, u0, u1);
 }
 
 // ---- image textures: src/textures/image.cpp:132-166, sampled like the reference's software sampler

@@ -15,6 +15,9 @@
 //
 // Denoising (an extension): `--denoise` renders G-buffer films (lrk_set_option("gbuffer")) and also writes lrk_denoise's image to
 // <stem>.denoised<ext> next to the camera's file, which is written as without it.  One GPU only: the G-buffer is not reduced.
+//
+// Light tree (an extension): `--light-tree` sets lrk_set_option("light_tree", 1) before the upload, so that next-event estimation
+// picks its lights by power, distance and orientation.  Surface integrator only: a volume scene fails with the library's message.
 #include <sys/stat.h>
 #include <sys/wait.h>
 #include <unistd.h>
@@ -43,6 +46,7 @@ void usage() {
                 "      --adaptive <threshold>   Adaptive sampling: stop 8x4 pixel blocks whose relative error is below threshold\n"
                 "      --adaptive-min-spp <n>   Samples per pixel of the first adaptive round (default 16, at most the camera's spp)\n"
                 "      --denoise                Also write the denoised image to <stem>.denoised<ext> (one GPU only)\n"
+                "      --light-tree             Pick next-event lights from a light tree (power, distance, orientation)\n"
                 "  -h, --help                   Display this help message\n");
 }
 
@@ -139,7 +143,7 @@ std::string denoised_path(const std::string &file) {
 int main(int argc, char *argv[]) {
     std::string backend, scene_path;
     int device = -1, gpus = 1;
-    bool denoise = false;
+    bool denoise = false, light_tree = false;
     std::string adaptive_arg, min_spp_arg;
     std::vector<std::string> keys, values;
     auto add_macro = [&](const std::string &d) {
@@ -182,6 +186,7 @@ int main(int argc, char *argv[]) {
         else if (a == "--adaptive-min-spp") min_spp_arg = need("count");
         else if (a.rfind("--adaptive-min-spp=", 0) == 0) min_spp_arg = a.substr(19);
         else if (a == "--denoise") denoise = true;
+        else if (a == "--light-tree") light_tree = true;
         else if (a == "-D" || a == "--define") add_macro(need("definition"));
         else if (a.rfind("-D", 0) == 0) add_macro(a.substr(2));
         else if (!a.empty() && a[0] == '-') std::fprintf(stderr, "[warning] Unrecognized options: %s\n", a.c_str());
@@ -253,6 +258,7 @@ int main(int argc, char *argv[]) {
     lrk_ctx *ctx = nullptr;
     if (int rc = lrk_create(&cfg, &ctx); rc != 0) die("Failed to create the CUDA device context (lrk_create = " + std::to_string(rc) + ").");
     if (denoise && lrk_set_option(ctx, "gbuffer", 1) != 0) die(lrk_last_error(ctx));
+    if (light_tree && lrk_set_option(ctx, "light_tree", 1) != 0) die(lrk_last_error(ctx));
     if (world > 1u) {
         uint8_t id[LRK_COMM_ID_BYTES];
         exchange_comm_id(rank, id);

@@ -105,11 +105,26 @@ def cornell_box(resolution=(512, 512), spp=16, depth=10, rr_depth=0, rr_threshol
 
 def instanced_spheres(resolution=(1920, 1080), spp=1024, seed=1, depth=10, rr_depth=0, rr_threshold=0.95,
                       big_subdivision=7, big_count=4, small_subdivision=3, small_count=60, medium=False,
-                      integrator=None, sampler_seed=19980810, output="spheres.exr") -> str:
+                      integrator=None, sampler_seed=19980810, output="spheres.exr", emissive=0, shared_light_node=False,
+                      emission_spread=True) -> str:
     """Configs C3 (1920x1080 @1024), C4 (+ homogeneous medium, depth 8, 3840x2160 @4096) and C5.
-    4 x 327 680 + 60 x 1 280 + 2 (ground) + 4 (lights) = 1 387 526 instanced triangles."""
+    4 x 327 680 + 60 x 1 280 + 2 (ground) + 4 (lights) = 1 387 526 instanced triangles.
+
+    ``emissive=K`` also makes the first K small spheres one-sided emitters (see ``many_lights``): each with its own Light node whose
+    emission is log-uniform over two orders of magnitude (``emission_spread``) or 4.0, or all K sharing one node of emission 4.0
+    (``shared_light_node``).  The defaults emit the scene without them, unchanged."""
     rng = np.random.default_rng(seed)
     out = []
+    emitter_of = {}
+    if emissive:
+        assert not (shared_light_node and emission_spread), "a shared light node has one emission"
+        levels = np.random.default_rng(seed + 7919).uniform(-1.0, 1.0, emissive) if emission_spread else np.zeros(emissive)
+        for i in range(emissive):
+            node = "sphere_light" if shared_light_node else f"sphere_light_{i}"
+            emitter_of[i] = node
+            if i == 0 or not shared_light_node:
+                v = 4.0 * 10.0 ** levels[i]
+                out.append(f"Light {node} : Diffuse {{ emission : Constant {{ v {{ {_fmt(v)}, {_fmt(0.8 * v)}, {_fmt(0.6 * v)} }} }} two_sided {{ false }} }}")
     # 8 Disney surfaces, parameters ~ U[0,1]
     for i in range(8):
         color = rng.uniform(0.0, 1.0, 3)
@@ -143,7 +158,7 @@ def instanced_spheres(resolution=(1920, 1080), spp=1024, seed=1, depth=10, rr_de
         out.append(f"Shape light_shape_{name} : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} light {{ @light_{name} }} }}")
         shapes.append(f"@light_shape_{name}")
 
-    def add_instance(name, base, scale_range, surface_index):
+    def add_instance(name, base, scale_range, surface_index, light=None):
         p = rng.uniform(-4.0, 4.0, 3)
         s = rng.uniform(*scale_range)
         p[1] = abs(p[1]) + s  # keep spheres above the ground plane
@@ -154,6 +169,7 @@ def instanced_spheres(resolution=(1920, 1080), spp=1024, seed=1, depth=10, rr_de
             f"Shape {name} : Instance {{\n"
             f"  shape {{ @{base} }}\n"
             f"  surface {{ @disney_{surface_index} }}\n"
+            + (f"  light {{ @{light} }}\n" if light else "") +
             f"  transform : SRT {{ scale {{ {_fmt(s)} }} rotate {{ {_fmt(axis[0])}, {_fmt(axis[1])}, {_fmt(axis[2])}, {_fmt(angle)} }} "
             f"translate {{ {_fmt(p[0])}, {_fmt(p[1])}, {_fmt(p[2])} }} }}\n"
             f"}}")
@@ -162,7 +178,7 @@ def instanced_spheres(resolution=(1920, 1080), spp=1024, seed=1, depth=10, rr_de
     for i in range(big_count):
         add_instance(f"big_{i}", "big_sphere", (0.7, 1.0), i % 8)
     for i in range(small_count):
-        add_instance(f"small_{i}", "small_sphere", (0.2, 0.5), int(rng.integers(0, 8)))
+        add_instance(f"small_{i}", "small_sphere", (0.2, 0.5), int(rng.integers(0, 8)), emitter_of.get(i))
 
     out.append(f"""Camera camera : Pinhole {{
   position {{ 0.0, 3.0, 12.0 }}
@@ -194,6 +210,15 @@ def instanced_spheres(resolution=(1920, 1080), spp=1024, seed=1, depth=10, rr_de
   shapes {{ {", ".join(shapes)} }}
 }}""")
     return "\n".join(out) + "\n"
+
+
+def many_lights(resolution=(1920, 1080), spp=64, count=48, shared_node=False, spread=True, **kw) -> str:
+    """The many-light frame of the light tree (option "light_tree"): the C3 scene with its two quad lights and ``count`` of its small
+    spheres emissive, with emission over two orders of magnitude (``spread``).  ``shared_node=True``: the spheres share one Light
+    node, which the reference's uniform sampler counts once (only the first is ever sampled by next-event estimation)."""
+    kw.setdefault("big_subdivision", 5)
+    return instanced_spheres(resolution=resolution, spp=spp, emissive=count, shared_light_node=shared_node,
+                             emission_spread=spread and not shared_node, output="many_lights.exr", **kw)
 
 
 def textured_materials(resolution=(64, 40), spp=4, depth=6, rr_depth=0, rr_threshold=0.95, seed=19980810, assets="tests/golden/assets",
