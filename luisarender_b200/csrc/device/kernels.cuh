@@ -52,9 +52,6 @@ __global__ void __launch_bounds__(kBlock) generate_rays_kernel(DeviceScene sc, P
 }
 
 // ---- traversal kernels -------------------------------------------------------------------------------
-// counts[] layout (all zeroed by generate_rays_kernel at the start of a pass), 64 slots (one per depth) each:
-//   [0] path-queue sizes  [1] shadow-queue sizes  [2] closest-hit fetch cursors  [3] shadow fetch cursors
-//   [4],[5],[6] hit-bucket sizes: light-only hits, Matte hits, Disney hits
 template<bool COUNT, bool ALPHA = false>
 __global__ void __launch_bounds__(kTraceBlock, LRK_TRACE_MIN_BLOCKS) trace_closest_kernel(DeviceScene sc, const float4 *__restrict__ ray_o,
                                                                const float4 *__restrict__ ray_d, uint4 *__restrict__ hits,
@@ -75,16 +72,9 @@ __global__ void __launch_bounds__(kTraceBlock, LRK_TRACE_MIN_BLOCKS) trace_close
 // Sorted-by-material dispatch, step 1: bucket the hits of this bounce by closure kind (the reference sorts its
 // SURFACE queue by surface tag, wave_path_v2.cpp:891-928,1255-1260, with a one-thread prefix sum; here a near-stable
 // block-aggregated partition).  Escaped rays are dropped, so the shade kernels only ever see real work; every bucket
-// keeps the ray-queue order inside a block chunk, which keeps the shade kernels' gathers coalesced.
-//   kind 0: hit has no surface (emitter only)   kind 1: Matte closure   kind 2: Disney closure
-//   kinds 3..6: Mirror, Glass, Plastic, Metal (MicrofacetFamilyClosure<type>, kind = type + 1)   kind 7: Mix
-//   kind 8: transmissive Disney closure ("disney_trans": LRK_SURFACE_DISNEY_TRANSMISSIVE records)   kind 9: Layered
-//   kind 10: thin Disney closure ("disney_thin": LRK_SURFACE_DISNEY_THIN records)
+// keeps the ray-queue order inside a block chunk, which keeps the shade kernels' gathers coalesced.  The kinds: hit_kinds.h.
 __global__ void __launch_bounds__(kBlock) classify_hits_kernel(DeviceScene sc, PathBuffers pb, uint32_t depth) {
-    __shared__ uint32_t s_warp[kHitKinds][kBlock / 32];
-    __shared__ uint32_t s_base[kHitKinds];
-    const uint32_t n = pb.counts[depth];
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5u, lane_lt = (1u << lane) - 1u;
+    const uint32_t n = *path_count(pb.counts, depth);
     for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {
         const uint32_t i = base + threadIdx.x;
         uint32_t kind = ~0u;
@@ -98,26 +88,8 @@ __global__ void __launch_bounds__(kBlock) classify_hits_kernel(DeviceScene sc, P
                 atomicAdd(pb.tile_cost + tile, inst != ~0u ? 3u : 1u);
             }
         }
-        uint32_t masks[kHitKinds];
-#pragma unroll
-        for (uint32_t k = 0; k < kHitKinds; k++) {
-            masks[k] = __ballot_sync(0xffffffffu, kind == k);
-            if (lane == 0u) s_warp[k][warp] = __popc(masks[k]);
-        }
-        __syncthreads();
-        if (threadIdx.x < kHitKinds) {
-            const uint32_t k = threadIdx.x;
-            uint32_t total = 0u;
-            for (int w = 0; w < kBlock / 32; w++) {
-                uint32_t c = s_warp[k][w];
-                s_warp[k][w] = total;
-                total += c;
-            }
-            s_base[k] = total ? atomicAdd(pb.counts + (4u + k) * kMaxDepthSlots + depth, total) : 0u;
-        }
-        __syncthreads();
-        if (kind != ~0u) pb.hit_index[kind][s_base[kind] + s_warp[kind][warp] + __popc(masks[kind] & lane_lt)] = i;
-        __syncthreads();
+        block_append<kBlock, kHitKinds>(kind != ~0u ? 1u << kind : 0u, [&](uint32_t k) { return bucket_count(pb.counts, k, depth); },
+                                        [&](uint32_t k, uint32_t slot) { pb.hit_index[k][slot] = i; });
     }
 }
 
@@ -160,7 +132,7 @@ __global__ void __launch_bounds__(kTraceBlock) trace_query_kernel(DeviceScene sc
 // scene (mega_path.cpp:68-75, UniformLightSamplerInstance::evaluate_miss uniform.cpp:67-76).  Without an environment the
 // escaped rays are simply never looked at again (classify_hits_kernel buckets hits only).
 __global__ void __launch_bounds__(kBlock) shade_miss_kernel(DeviceScene sc, PathBuffers pb, uint32_t depth) {
-    const uint32_t n = pb.counts[depth];
+    const uint32_t n = *path_count(pb.counts, depth);
     const int in = depth & 1u;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         if (pb.hit[i].x != ~0u) continue;

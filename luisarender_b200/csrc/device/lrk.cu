@@ -116,8 +116,8 @@ struct lrk_ctx {
     cudaEvent_t ev_begin{}, ev_end{};
     std::vector<TimedLaunch> timed;
     std::vector<cudaEvent_t> event_pool;
-    int grid_trace{0}, grid_shade[2][11]{}, grid_shadow{0}, grid_classify{0};// grid_shade[variant]: 0 = fast, 1 = strict arithmetic
-    bool has_kind[11]{true, false, false, false, false, false, false, false, false, false, false};
+    int grid_trace{0}, grid_shade[2][kHitKinds]{}, grid_shadow{0}, grid_classify{0};// grid_shade[variant]: 0 = fast, 1 = strict arithmetic
+    uint32_t used_kinds{1u};     // bit k: an instance of the scene has hit kind k (bit 0 always: emitter-only hits of an image emission)
     uint32_t allocated_kinds{0u};// bit k: hit_index[k] is allocated
     bool volume{false};
     bool strict_math{false};// option strict_math: every closure kernel from shade.cu's IEEE-arithmetic compilation
@@ -198,8 +198,7 @@ int upload(lrk_ctx *ctx, DeviceBuffer &dst, const T *src, size_t count) {
 }
 
 int alloc_paths(lrk_ctx *ctx, uint64_t capacity) {
-    uint32_t kinds = 0u;
-    for (int k = 0; k < static_cast<int>(kHitKinds); k++) if (k < 3 || ctx->has_kind[k]) kinds |= 1u << k;// buckets 3..10 only for scenes that use them
+    const uint32_t kinds = ctx->used_kinds | 7u;// buckets 0..2 always, the others only for scenes that use them
     if (ctx->capacity >= capacity && (!ctx->volume || ctx->volume_capacity >= capacity) && (ctx->allocated_kinds & kinds) == kinds) return LRK_OK;
     // all of the old path state is freed before any of the new one is allocated
     ctx->path_allocs.clear();
@@ -359,8 +358,8 @@ void launch_trace_closest(lrk_ctx *ctx, bool alpha, uint64_t n, uint32_t depth) 
     const auto kernel = alpha ? (count ? trace_closest_kernel<true, true> : trace_closest_kernel<false, true>)
                               : (count ? trace_closest_kernel<true, false> : trace_closest_kernel<false, false>);
     const int in = depth & 1u;
-    kernel<<<blocks_for(ctx, n, ctx->grid_trace), kTraceBlock, 0, ctx->stream>>>(ctx->scene, pb.ray_o[in], pb.ray_d[in], pb.hit, pb.counts + depth,
-                                                                                 pb.counts + 2u * kMaxDepthSlots + depth, pb.stats);
+    kernel<<<blocks_for(ctx, n, ctx->grid_trace), kTraceBlock, 0, ctx->stream>>>(ctx->scene, pb.ray_o[in], pb.ray_d[in], pb.hit, path_count(pb.counts, depth),
+                                                                                 closest_cursor(pb.counts, depth), pb.stats);
     ctx->stats.kernel_launches++;
 }
 
@@ -397,10 +396,8 @@ int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset,
             // one kernel per closure kind over its own hit bucket (shade.cu); TEXTURED variants only for scenes with image-textured
             // parameters / normal maps
             for (uint32_t kind = 0; kind < kHitKinds; kind++) {
-                if (kind != 0u && !ctx->has_kind[kind]) continue;
-                // the near-specular closures (Mirror, Glass, Plastic, Metal, Mix: buckets 3..7), Layered and thin Disney always run in
-                // IEEE arithmetic
-                const bool strict = ctx->strict_math || (kind >= 3u && kind <= 7u) || kind >= 9u;
+                if (!(ctx->used_kinds & (1u << kind))) continue;
+                const bool strict = ctx->strict_math || hit_kind_always_strict(kind);
                 const int blocks = blocks_for(ctx, n, ctx->grid_shade[strict ? 1 : 0][kind]);
                 if (strict) strict::launch_shade(kind, ctx->textured, ctx->light_tree, blocks, ctx->stream, sc, pb, depth);
                 else fast::launch_shade(kind, ctx->textured, ctx->light_tree, blocks, ctx->stream, sc, pb, depth);
@@ -412,8 +409,7 @@ int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset,
             const bool count = ctx->count_traversal;
             const auto kernel = ctx->any_non_opaque ? (count ? trace_shadow_kernel<true, true> : trace_shadow_kernel<false, true>)
                                                     : (count ? trace_shadow_kernel<true, false> : trace_shadow_kernel<false, false>);
-            kernel<<<blocks_for(ctx, n, ctx->grid_shadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + kMaxDepthSlots + depth,
-                                                                                         pb.counts + 3u * kMaxDepthSlots + depth);
+            kernel<<<blocks_for(ctx, n, ctx->grid_shadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, shadow_count(pb.counts, depth), shadow_cursor(pb.counts, depth));
             ctx->stats.kernel_launches++;
         }
     }
@@ -457,9 +453,9 @@ int render_pass_volume(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_
         const int out = (depth & 1u) ^ 1;
         {
             ScopedTimer t{ctx, CAT_TRACE_SHADOW};
-            // the in-medium shadow rays share the depth's path-queue size; their cursor lives in the shadow-cursor region + 32
+            // the in-medium shadow rays share the depth's path-queue size
             const auto kernel = ctx->count_traversal ? trace_medium_shadow_kernel<true> : trace_medium_shadow_kernel<false>;
-            kernel<<<blocks_for(ctx, n, ctx->grid_vshadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + depth, pb.counts + 3u * kMaxDepthSlots + 32u + depth);
+            kernel<<<blocks_for(ctx, n, ctx->grid_vshadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, path_count(pb.counts, depth), medium_shadow_cursor(pb.counts, depth));
             ctx->stats.kernel_launches++;
         }
         launch_trace_closest(ctx, false, n, depth);
@@ -469,8 +465,8 @@ int render_pass_volume(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_
             if (v) strict::launch_volume_medium(blocks_for(ctx, n, ctx->grid_vmedium[v]), ctx->stream, sc, pb, depth);
             else fast::launch_volume_medium(blocks_for(ctx, n, ctx->grid_vmedium[v]), ctx->stream, sc, pb, depth);
             ctx->stats.kernel_launches++;
-            for (uint32_t kind = 0; kind < 3u; kind++) {
-                if (kind != 0u && !ctx->has_kind[kind]) continue;
+            for (uint32_t kind = 0; kind <= kHitDisney; kind++) {
+                if (!(ctx->used_kinds & (1u << kind))) continue;
                 const int blocks = blocks_for(ctx, n, ctx->grid_vshade[v][kind]);
                 if (v) strict::launch_volume_surface(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
                 else fast::launch_volume_surface(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
@@ -480,8 +476,8 @@ int render_pass_volume(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_
         {
             ScopedTimer t{ctx, CAT_TRACE_SHADOW};
             const auto kernel = ctx->count_traversal ? trace_volume_nee_kernel<true> : trace_volume_nee_kernel<false>;
-            kernel<<<blocks_for(ctx, n, ctx->grid_vshadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, pb.counts + kMaxDepthSlots + depth,
-                                                                                         pb.counts + 3u * kMaxDepthSlots + depth, pb.occl2[out]);
+            kernel<<<blocks_for(ctx, n, ctx->grid_vshadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, shadow_count(pb.counts, depth), shadow_cursor(pb.counts, depth),
+                                                                                         pb.occl2[out]);
             ctx->stats.kernel_launches++;
         }
     }
@@ -872,7 +868,7 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
             if ((rc = upload(ctx, a.zsobol_hash, q.zsobol_hash, 2048u))) return rc;
     }
     std::vector<uint32_t> handles(static_cast<size_t>(s->instance_count) * 4u), kinds(s->instance_count);
-    for (int k = 1; k < static_cast<int>(kHitKinds); k++) ctx->has_kind[k] = false;
+    ctx->used_kinds = 1u;
     ctx->any_non_opaque = false;
     std::vector<float> o2w(static_cast<size_t>(s->instance_count) * 12u), xform(static_cast<size_t>(s->instance_count) * 16u);
     for (uint32_t i = 0; i < s->instance_count; i++) {
@@ -880,17 +876,13 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         std::memcpy(&handles[i * 4u], inst.handle, 16);
         {// closure kind of the instance: the bucket key of the material sort
             const uint32_t flags = inst.handle[0] & 1023u, surface_tag = (inst.handle[1] >> 12u) & 4095u;
-            uint32_t kind = 0u;
+            uint32_t kind = kHitEmitter;
             if (flags & LRK_SHAPE_HAS_SURFACE) {
                 if (surface_tag >= s->surface_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: surface tag out of range");
-                const uint32_t type = s->surfaces[surface_tag].type;
-                kind = type + 1u;// Matte 1, Disney 2, Mirror 3, Glass 4, Plastic 5, Metal 6, Mix 7
-                if (type == LRK_SURFACE_DISNEY && (s->surfaces[surface_tag].flags & LRK_SURFACE_DISNEY_TRANSMISSIVE)) kind = 8u;
-                if (type == LRK_SURFACE_LAYERED) kind = 9u;
-                if (type == LRK_SURFACE_DISNEY && (s->surfaces[surface_tag].flags & LRK_SURFACE_DISNEY_THIN)) kind = 10u;
+                kind = hit_kind_of(s->surfaces[surface_tag]);
             }
             kinds[i] = kind;
-            ctx->has_kind[kind] = true;
+            ctx->used_kinds |= 1u << kind;
             if ((flags & LRK_SHAPE_MAYBE_NON_OPAQUE) && (flags & LRK_SHAPE_HAS_SURFACE)) ctx->any_non_opaque = true;
         }
         if (inst.mesh >= s->mesh_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: mesh index out of range");

@@ -5,6 +5,7 @@
 #include <type_traits>
 #include <utility>
 
+#include "hit_kinds.h"
 #include "shading.cuh"
 
 namespace lrk {
@@ -70,6 +71,39 @@ template<bool TEXTURED>
 __device__ __forceinline__ Frame closure_frame(const DeviceScene &sc, const lrk_surface *node, const Interaction &it, V3 wo) {
     if (TEXTURED && (node->flags & LRK_SURFACE_HAS_NORMAL_MAP)) return normal_mapped_frame(sc, node, it, wo);
     return it.shading;
+}
+
+// The closure of hit bucket KIND (hit_kinds.h) at a hit seen from wo: calls f(closure, frame) with the frame the closure works in,
+// frame_of() (closure_frame, or the caller's copy of it), and returns the closure's eta scale for Russian roulette
+// (mega_path.cpp:113,133-138).  Layered's init needs the frame, so Layered alone takes the frame before init.  Emitter-only hits
+// have no closure: f is not called.
+template<uint32_t KIND> struct hit_closure { using type = MicrofacetFamilyClosure<KIND - 1u>; };// Mirror .. Metal: kind = type + 1
+template<> struct hit_closure<kHitMatte> { using type = MatteClosure; };
+template<> struct hit_closure<kHitDisney> { using type = DisneyClosure; };
+template<> struct hit_closure<kHitMix> { using type = MixClosure; };
+template<> struct hit_closure<kHitDisneyTrans> { using type = DisneyTransClosure; };
+template<> struct hit_closure<kHitDisneyThin> { using type = DisneyThinClosure; };
+
+template<uint32_t KIND, bool TEXTURED, typename FrameOf, typename F>
+__device__ __forceinline__ float with_hit_closure(const DeviceScene &sc, const lrk_surface *surf, const Interaction &it, const V3 &wo, FrameOf &&frame_of,
+                                                 F &&f) {
+    if constexpr (KIND == kHitEmitter) {
+        return 1.f;
+    } else if constexpr (KIND == kHitLayered) {
+        LayeredClosure cl;
+        const Frame fr = frame_of();
+        cl.init(*surf, sc.surfaces, it, fr, wo);
+        f(cl, fr);
+        return cl.rr_eta_scale;
+    } else {
+        typename hit_closure<KIND>::type cl;
+        if constexpr (KIND == kHitMix) cl.init(*surf, sc.surfaces);
+        else init_closure<TEXTURED>(sc, cl, surf, it);
+        f(cl, frame_of());
+        if constexpr (KIND == kHitDisneyTrans) return (surf->lobes & LRK_DISNEY_LOBE_SPEC_TRANS) ? cl.rr_eta_scale : 1.f;// disney.cpp:531-533
+        else if constexpr (KIND == kHitMatte || KIND == kHitDisney || KIND == kHitDisneyThin) return 1.f;// closure->eta() is empty
+        else return cl.rr_eta_scale;
+    }
 }
 
 // Evaluates the closure for the light sample's direction (NEE term) and for the direction the closure itself samples.

@@ -5,6 +5,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "hit_kinds.h"
 #include "scene.cuh"
 
 namespace lrk {
@@ -26,8 +27,8 @@ constexpr int kBlock = 256;
 #define LRK_SHADE_MIN_BLOCKS 2
 #endif
 constexpr int kShadeBlock = LRK_SHADE_BLOCK;// threads per block of the surface shade kernels (register-bound: see DESIGN.md)
-constexpr uint32_t kCountSlots = 16u;   // rows of 64 counters in PathBuffers::counts: 4 queue / cursor rows + one per hit bucket
-constexpr uint32_t kMaxDepthSlots = 64u;// counts[0..63]: path queue size per depth, counts[64..127]: shadow queue size
+constexpr uint32_t kCountSlots = 16u;   // rows of counters in PathBuffers::counts: 4 queue / cursor rows + one per hit bucket
+constexpr uint32_t kMaxDepthSlots = 64u;// counters per row: one per depth
 
 struct PathBuffers {
     float4 *ray_o[2];
@@ -35,7 +36,7 @@ struct PathBuffers {
     float4 *beta_pdf[2];
     uint2 *id_rng[2];
     uint4 *hit;// {inst, prim, bary} per ray of the current queue (inst == ~0u: escaped)
-    uint32_t *hit_index[11];// per closure kind: indices (into the current ray queue) of the rays that hit such a surface
+    uint32_t *hit_index[kHitKinds];// per hit kind (hit_kinds.h): indices (into the current ray queue) of the rays that hit such a surface
     float4 *sray_o;
     float4 *sray_d;
     float4 *scontrib;// rgb + path id bits
@@ -58,7 +59,54 @@ struct PathBuffers {
     uint32_t tile_cost_size, tile_cost_tiles_x;
     unsigned long long *stats;// [0] closest rays, [1] shadow rays, [2..4] closest nodes/tris/xforms, [5..7] shadow nodes/tris/xforms
 };
-constexpr uint32_t kHitKinds = 11u;// hit buckets: emitter-only, Matte, Disney, Mirror, Glass, Plastic, Metal, Mix, transmissive Disney, Layered, thin Disney
+
+// The rows of PathBuffers::counts, kMaxDepthSlots counters each (one per depth), all zeroed by the ray generation kernels at the start
+// of a pass.  Free functions of the pointer rather than members: a member call on a kernel's PathBuffers parameter takes its address,
+// which changes the shade kernels' code.
+__host__ __device__ __forceinline__ uint32_t *path_count(uint32_t *counts, uint32_t depth) { return counts + depth; }// path-queue size
+__host__ __device__ __forceinline__ uint32_t *shadow_count(uint32_t *counts, uint32_t depth) { return counts + kMaxDepthSlots + depth; }// shadow-queue size
+__host__ __device__ __forceinline__ uint32_t *closest_cursor(uint32_t *counts, uint32_t depth) { return counts + 2u * kMaxDepthSlots + depth; }// closest-hit fetch cursor
+__host__ __device__ __forceinline__ uint32_t *shadow_cursor(uint32_t *counts, uint32_t depth) { return counts + 3u * kMaxDepthSlots + depth; }// shadow fetch cursor
+// fetch cursor of the volume integrator's in-medium shadow rays: the upper half of the shadow-cursor row (its depths stay below 32)
+__host__ __device__ __forceinline__ uint32_t *medium_shadow_cursor(uint32_t *counts, uint32_t depth) { return counts + 3u * kMaxDepthSlots + 32u + depth; }
+__host__ __device__ __forceinline__ uint32_t *bucket_count(uint32_t *counts, uint32_t kind, uint32_t depth) {// size of hit bucket `kind`
+    return counts + ((4u + kind) * kMaxDepthSlots + depth);
+}
 static_assert(4u + kHitKinds <= kCountSlots, "PathBuffers::counts has one row of counters per hit bucket behind the four queue rows");
+
+#ifdef __CUDACC__
+// Block-aggregated append: every thread of the block calls it with the set of lists it appends one item to (bit l: list l < LISTS),
+// and store(l, slot) is called for each of them with the item's slot in list l.  Ballots inside the warp, a scan of the warp counts in
+// shared memory, one atomicAdd on counter(l) per list with items; the order inside a block is the thread order.  The last barrier
+// lets the next call reuse the shared counts.
+template<int BLOCK, uint32_t LISTS, typename Counter, typename Store>
+__device__ __forceinline__ void block_append(uint32_t lists, Counter &&counter, Store &&store) {
+    __shared__ uint32_t s_warp[LISTS][BLOCK / 32], s_base[LISTS];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5u;
+    uint32_t masks[LISTS];
+#pragma unroll
+    for (uint32_t l = 0; l < LISTS; l++) {
+        masks[l] = __ballot_sync(0xffffffffu, (lists >> l) & 1u);
+        if (lane == 0u) s_warp[l][warp] = __popc(masks[l]);
+    }
+    __syncthreads();
+    if (threadIdx.x < LISTS) {
+        const uint32_t l = threadIdx.x;
+        uint32_t total = 0u;
+        for (int w = 0; w < BLOCK / 32; w++) {
+            const uint32_t c = s_warp[l][w];
+            s_warp[l][w] = total;
+            total += c;
+        }
+        s_base[l] = total ? atomicAdd(counter(l), total) : 0u;
+    }
+    __syncthreads();
+    const uint32_t lane_lt = (1u << lane) - 1u;
+#pragma unroll
+    for (uint32_t l = 0; l < LISTS; l++)
+        if ((lists >> l) & 1u) store(l, s_base[l] + s_warp[l][warp] + __popc(masks[l] & lane_lt));
+    __syncthreads();
+}
+#endif
 
 }// namespace lrk

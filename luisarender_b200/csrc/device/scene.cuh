@@ -22,7 +22,7 @@ struct DeviceScene {
     const float *pdf;
     const lrk_mesh *meshes;
     const uint4 *inst_handles;
-    const uint32_t *inst_kind;// per instance: 0 = no surface, else surface type + 1 (Matte 1, Disney 2, Mirror 3, Glass 4, Plastic 5, Metal 6): bucket key of the material sort
+    const uint32_t *inst_kind;// per instance: its hit kind (hit_kinds.h), the bucket key of the material sort
     const float4 *inst_o2w;
     const float4 *inst_xform;
     const float4 *bvh_nodes;// 4 x float4 per node: {lo0.xyz,hi0.x} {hi0.yz,lo1.xy} {lo1.z,hi1.xyz} {ref0,ref1,parent,-}

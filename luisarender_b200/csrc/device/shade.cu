@@ -33,28 +33,19 @@ int grid_of(Kernel kernel, int block, int sm_count) {
 // calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection)
 template<uint32_t SEL, typename F>
 void with_shade_kernel(uint32_t kind, bool textured, F &&f) {
-    switch (kind) {
-        case 0u: textured ? f(shade_kernel<0u, true, SEL>) : f(shade_kernel<0u, false, SEL>); break;// emitter-only hits: a light's image emission
-        case 1u: textured ? f(shade_kernel<1u, true, SEL>) : f(shade_kernel<1u, false, SEL>); break;
-        case 2u: textured ? f(shade_kernel<2u, true, SEL>) : f(shade_kernel<2u, false, SEL>); break;
-        case 3u: textured ? f(shade_kernel<3u, true, SEL>) : f(shade_kernel<3u, false, SEL>); break;
-        case 4u: textured ? f(shade_kernel<4u, true, SEL>) : f(shade_kernel<4u, false, SEL>); break;
-        case 5u: textured ? f(shade_kernel<5u, true, SEL>) : f(shade_kernel<5u, false, SEL>); break;
-        case 6u: textured ? f(shade_kernel<6u, true, SEL>) : f(shade_kernel<6u, false, SEL>); break;
-        case 7u: textured ? f(shade_kernel<7u, true, SEL>) : f(shade_kernel<7u, false, SEL>); break;
-        case 8u: textured ? f(shade_kernel<8u, true, SEL>) : f(shade_kernel<8u, false, SEL>); break;
-        case 9u: textured ? f(shade_kernel<9u, true, SEL>) : f(shade_kernel<9u, false, SEL>); break;
-        default: textured ? f(shade_kernel<10u, true, SEL>) : f(shade_kernel<10u, false, SEL>); break;
-    }
+    with_hit_kind(kind, [&](auto k) {
+        constexpr uint32_t K = decltype(k)::value;
+        textured ? f(shade_kernel<K, true, SEL>) : f(shade_kernel<K, false, SEL>);
+    });
 }
 
+// the volume integrator's surface step exists for the kinds of config C4's closures: emitter-only, Matte and Disney
 template<typename F>
 void with_volume_surface_kernel(uint32_t kind, bool textured, F &&f) {
-    switch (kind) {
-        case 0u: textured ? f(volume_surface_kernel<0u, true>) : f(volume_surface_kernel<0u, false>); break;
-        case 1u: textured ? f(volume_surface_kernel<1u, true>) : f(volume_surface_kernel<1u, false>); break;
-        default: textured ? f(volume_surface_kernel<2u, true>) : f(volume_surface_kernel<2u, false>); break;
-    }
+    with_hit_kind(kind, [&](auto k) {
+        constexpr uint32_t K = decltype(k)::value;
+        if constexpr (K <= kHitDisney) textured ? f(volume_surface_kernel<K, true>) : f(volume_surface_kernel<K, false>);
+    });
 }
 
 }// namespace

@@ -43,9 +43,10 @@ __device__ __noinline__ inline BounceDraws draw_bounce_from_tables(SamplerRef sc
 // of next-event estimation (kLightSelectTree with the option "light_tree")
 template<uint32_t KIND, bool TEXTURED = false, uint32_t SEL = kLightSelectUniform>
 __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kernel(DeviceScene sc, PathBuffers pb, uint32_t depth) {
+    // the compaction is written out here rather than through block_append, which raises registers or spills of most instantiations
     __shared__ uint32_t s_warp_next[kShadeBlock / 32], s_warp_shadow[kShadeBlock / 32];
     __shared__ uint32_t s_base_next, s_base_shadow;
-    const uint32_t n = pb.counts[(4u + KIND) * kMaxDepthSlots + depth];// size of this kind's hit bucket
+    const uint32_t n = *bucket_count(pb.counts, KIND, depth);// size of this kind's hit bucket
     const int in = depth & 1u, out = in ^ 1;
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5u;
     for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {
@@ -77,7 +78,7 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                     li.z += add.z;
                     pb.li[ir.x] = li;
                 }
-                if (KIND != 0u) {// kind 0 = emitter-only hit (no surface): the path ends here (mega_path.cpp:89)
+                if (KIND != kHitEmitter) {// an emitter-only hit (no surface): the path ends here (mega_path.cpp:89)
                     // draw order is normative: mega_path.cpp:91-98
                     float u_sel, ul0, ul1, u_lobe, ub0, ub1, u_rr = 0.f;
                     if (sc.sampler_type == LRK_SAMPLER_INDEPENDENT) {// the headline path: an LCG word in a register
@@ -103,41 +104,10 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                     const lrk_surface *surf = sc.surfaces + it.shape.surface_tag;
                     V3 contrib, wi, f;
                     float pdf;
-                    float eta_scale = 1.f;// mega_path.cpp:113,133-138
-                    if (KIND == 1u) {
-                        MatteClosure cl;
-                        init_closure<TEXTURED>(sc, cl, surf, it);
-                        shade_surface<false>(cl, it, closure_frame<TEXTURED>(sc, surf, it, wo), wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
-                    } else if (KIND == 2u) {
-                        DisneyClosure cl;
-                        init_closure<TEXTURED>(sc, cl, surf, it);
-                        shade_surface<false>(cl, it, closure_frame<TEXTURED>(sc, surf, it, wo), wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
-                    } else if (KIND == 8u) {
-                        DisneyTransClosure cl;
-                        init_closure<TEXTURED>(sc, cl, surf, it);
-                        shade_surface<false>(cl, it, closure_frame<TEXTURED>(sc, surf, it, wo), wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
-                        if (surf->lobes & LRK_DISNEY_LOBE_SPEC_TRANS) eta_scale = cl.rr_eta_scale;// closure->eta() (disney.cpp:531-533)
-                    } else if (KIND == 10u) {// closure->eta() is empty (disney.cpp:779): no Russian-roulette eta scale
-                        DisneyThinClosure cl;
-                        init_closure<TEXTURED>(sc, cl, surf, it);
-                        shade_surface<false>(cl, it, closure_frame<TEXTURED>(sc, surf, it, wo), wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
-                    } else if (KIND == 9u) {
-                        LayeredClosure cl;
-                        const Frame fr = closure_frame<TEXTURED>(sc, surf, it, wo);
-                        cl.init(*surf, sc.surfaces, it, fr, wo);
+                    const float eta_scale = with_hit_closure<KIND, TEXTURED>(sc, surf, it, wo, [&] { return closure_frame<TEXTURED>(sc, surf, it, wo); },
+                                                                           [&](auto &cl, const Frame &fr) {
                         shade_surface<false>(cl, it, fr, wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
-                        eta_scale = cl.rr_eta_scale;
-                    } else if (KIND == 7u) {
-                        MixClosure cl;
-                        cl.init(*surf, sc.surfaces);
-                        shade_surface<false>(cl, it, closure_frame<TEXTURED>(sc, surf, it, wo), wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
-                        eta_scale = cl.rr_eta_scale;
-                    } else {
-                        MicrofacetFamilyClosure<(KIND >= 3u && KIND <= 6u) ? KIND - 1u : LRK_SURFACE_MIRROR> cl;// kind = surface type + 1
-                        init_closure<TEXTURED>(sc, cl, surf, it);
-                        shade_surface<false>(cl, it, closure_frame<TEXTURED>(sc, surf, it, wo), wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
-                        eta_scale = cl.rr_eta_scale;
-                    }
+                    });
                     if (contrib.x != 0.f || contrib.y != 0.f || contrib.z != 0.f) {
                         // a zero (or NaN-free zero) contribution needs no shadow ray; NaNs must reach the film filter
                         push_shadow = true;
@@ -185,8 +155,8 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                 tn += a;
                 ts += b;
             }
-            s_base_next = tn ? atomicAdd(pb.counts + depth + 1u, tn) : 0u;
-            s_base_shadow = ts ? atomicAdd(pb.counts + kMaxDepthSlots + depth, ts) : 0u;
+            s_base_next = tn ? atomicAdd(path_count(pb.counts, depth + 1u), tn) : 0u;
+            s_base_shadow = ts ? atomicAdd(shadow_count(pb.counts, depth), ts) : 0u;
         }
         __syncthreads();
         const uint32_t lt = (1u << lane) - 1u;
@@ -263,12 +233,8 @@ __device__ __forceinline__ void volume_store_next(const PathBuffers &pb, int out
 // (event 3) write their updated throughput, pdf, PCG state and the MOVED ray origin back in place and are appended to the
 // hit bucket of their closure kind - the same material sort as the surface integrator - for volume_surface_kernel.
 __global__ void __launch_bounds__(kBlock) volume_medium_kernel(DeviceScene sc, PathBuffers pb, uint32_t depth) {
-    constexpr uint32_t kLists = 1u + kHitKinds;// list 0 = next wave, 1 + k = hit bucket k
-    __shared__ uint32_t s_warp[kLists][kBlock / 32];
-    __shared__ uint32_t s_base[kLists];
-    const uint32_t n = pb.counts[depth];
+    const uint32_t n = *path_count(pb.counts, depth);
     const int in = depth & 1u, out = in ^ 1;
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5u, lane_lt = (1u << lane) - 1u;
     const V3 sigma_a = v3(sc.sigma_a[0], sc.sigma_a[1], sc.sigma_a[2]), sigma_s = v3(sc.sigma_s[0], sc.sigma_s[1], sc.sigma_s[2]);
     for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {
         const uint32_t i = base + threadIdx.x;
@@ -312,34 +278,13 @@ __global__ void __launch_bounds__(kBlock) volume_medium_kernel(DeviceScene sc, P
                 if (nx.push) list = 0u;
             }
         }
-        uint32_t masks[kLists];
-#pragma unroll
-        for (uint32_t k = 0; k < kLists; k++) {
-            masks[k] = __ballot_sync(0xffffffffu, list == k);
-            if (lane == 0u) s_warp[k][warp] = __popc(masks[k]);
-        }
-        __syncthreads();
-        if (threadIdx.x < kLists) {
-            const uint32_t k = threadIdx.x;
-            uint32_t total = 0u;
-            for (int w = 0; w < kBlock / 32; w++) {
-                uint32_t c = s_warp[k][w];
-                s_warp[k][w] = total;
-                total += c;
-            }
-            uint32_t *counter = k == 0u ? pb.counts + depth + 1u : pb.counts + (4u + (k - 1u)) * kMaxDepthSlots + depth;
-            s_base[k] = total ? atomicAdd(counter, total) : 0u;
-        }
-        __syncthreads();
-        if (list != ~0u) {
-            uint32_t slot = s_base[list] + s_warp[list][warp];
-#pragma unroll
-            for (uint32_t k = 0; k < kLists; k++)
-                if (list == k) slot += __popc(masks[k] & lane_lt);
-            if (list == 0u) volume_store_next(pb, out, slot, nx);
-            else pb.hit_index[list - 1u][slot] = i;
-        }
-        __syncthreads();
+        // list 0: the next wave, list 1 + k: hit bucket k
+        block_append<kBlock, 1u + kHitKinds>(list != ~0u ? 1u << list : 0u,
+                                             [&](uint32_t l) { return l == 0u ? path_count(pb.counts, depth + 1u) : bucket_count(pb.counts, l - 1u, depth); },
+                                             [&](uint32_t l, uint32_t slot) {
+                                                 if (l == 0u) volume_store_next(pb, out, slot, nx);
+                                                 else pb.hit_index[l - 1u][slot] = i;
+                                             });
     }
 }
 
@@ -347,11 +292,8 @@ __global__ void __launch_bounds__(kBlock) volume_medium_kernel(DeviceScene sc, P
 // closure sample (mega_vpt_naive.cpp:300-437), then the common end of the iteration.
 template<uint32_t KIND, bool TEXTURED = false>
 __global__ void __launch_bounds__(kBlock, 2) volume_surface_kernel(DeviceScene sc, PathBuffers pb, uint32_t depth) {
-    __shared__ uint32_t s_warp_next[kBlock / 32], s_warp_shadow[kBlock / 32];
-    __shared__ uint32_t s_base_next, s_base_shadow;
-    const uint32_t n = pb.counts[(4u + KIND) * kMaxDepthSlots + depth];
+    const uint32_t n = *bucket_count(pb.counts, KIND, depth);
     const int in = depth & 1u, out = in ^ 1;
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5u;
     for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {
         const uint32_t j = base + threadIdx.x;
         bool push_shadow = false;
@@ -382,7 +324,7 @@ __global__ void __launch_bounds__(kBlock, 2) volume_surface_kernel(DeviceScene s
                 li.z += add.z;
                 pb.li[ir.x] = li;
             }
-            if (KIND != 0u) {
+            if (KIND != kHitEmitter) {
                 float u_sel = lcg(state);
                 float ul0 = lcg(state), ul1 = lcg(state);
                 float u_lobe = lcg(state);
@@ -393,15 +335,9 @@ __global__ void __launch_bounds__(kBlock, 2) volume_surface_kernel(DeviceScene s
                 V3 contrib = v3(0.f), wi, f;
                 float pdf;
                 // true_hit(medium_tag = 0) <=> 0 <= priority of the environment medium: always true (medium_tracker.cpp:19-21)
-                if (KIND == 1u) {
-                    MatteClosure cl;
-                    init_closure<TEXTURED>(sc, cl, surf, it);
-                    shade_surface<true>(cl, it, closure_frame<TEXTURED>(sc, surf, it, wo), wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
-                } else {
-                    DisneyClosure cl;
-                    init_closure<TEXTURED>(sc, cl, surf, it);
-                    shade_surface<true>(cl, it, closure_frame<TEXTURED>(sc, surf, it, wo), wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
-                }
+                with_hit_closure<KIND, TEXTURED>(sc, surf, it, wo, [&] { return closure_frame<TEXTURED>(sc, surf, it, wo); }, [&](auto &cl, const Frame &fr) {
+                    shade_surface<true>(cl, it, fr, wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
+                });
                 push_shadow = true;// traced even with a zero contribution: its occlusion advances the PCG stream of the next bounce
                 sro = ls.ray_o_tmin;
                 srd = ls.ray_d_tmax;
@@ -413,40 +349,21 @@ __global__ void __launch_bounds__(kBlock, 2) volume_surface_kernel(DeviceScene s
                 if (!nx.push && scon.x == 0.f && scon.y == 0.f && scon.z == 0.f) push_shadow = false;// nothing depends on it
             }
         }
-        uint32_t m_next = __ballot_sync(0xffffffffu, nx.push);
-        uint32_t m_shadow = __ballot_sync(0xffffffffu, push_shadow);
-        if (lane == 0u) {
-            s_warp_next[warp] = __popc(m_next);
-            s_warp_shadow[warp] = __popc(m_shadow);
-        }
-        __syncthreads();
-        if (threadIdx.x == 0u) {
-            uint32_t tn = 0u, ts = 0u;
-            for (int w = 0; w < kBlock / 32; w++) {
-                uint32_t a = s_warp_next[w], b = s_warp_shadow[w];
-                s_warp_next[w] = tn;
-                s_warp_shadow[w] = ts;
-                tn += a;
-                ts += b;
-            }
-            s_base_next = tn ? atomicAdd(pb.counts + depth + 1u, tn) : 0u;
-            s_base_shadow = ts ? atomicAdd(pb.counts + kMaxDepthSlots + depth, ts) : 0u;
-        }
-        __syncthreads();
-        const uint32_t lt = (1u << lane) - 1u;
+        // list 0: the next wave, list 1: the surface NEE shadow records (list 0's slot is stored first: the record points at it)
         uint32_t next_slot = ~0u;
-        if (nx.push) {
-            next_slot = s_base_next + s_warp_next[warp] + __popc(m_next & lt);
-            volume_store_next(pb, out, next_slot, nx);
-        }
-        if (push_shadow) {
-            uint32_t slot = s_base_shadow + s_warp_shadow[warp] + __popc(m_shadow & lt);
-            pb.sray_o[slot] = sro;
-            pb.sray_d[slot] = srd;
-            pb.scontrib[slot] = scon;
-            pb.s2_target[slot] = next_slot;
-        }
-        __syncthreads();
+        block_append<kBlock, 2u>((nx.push ? 1u : 0u) | (push_shadow ? 2u : 0u),
+                                 [&](uint32_t l) { return l == 0u ? path_count(pb.counts, depth + 1u) : shadow_count(pb.counts, depth); },
+                                 [&](uint32_t l, uint32_t slot) {
+                                     if (l == 0u) {
+                                         next_slot = slot;
+                                         volume_store_next(pb, out, slot, nx);
+                                     } else {
+                                         pb.sray_o[slot] = sro;
+                                         pb.sray_d[slot] = srd;
+                                         pb.scontrib[slot] = scon;
+                                         pb.s2_target[slot] = next_slot;
+                                     }
+                                 });
     }
 }
 

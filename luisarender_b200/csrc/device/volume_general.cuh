@@ -79,66 +79,15 @@ __device__ __forceinline__ uint32_t surface_event_of(const Frame &shading, V3 wo
     return wo_local.z * wi_local.z > 0.f ? LRK_EVENT_REFLECT : wi_local.z > 0.f ? LRK_EVENT_EXIT : LRK_EVENT_ENTER;
 }
 
-// Runs f(closure) with the closure of the hit's surface kind (the bucket key of the wavefront integrator's material sort).
+// Runs f(closure, shading) with the closure of the hit's kind (the bucket key of the wavefront integrator's material sort).  Nothing
+// for emitter-only hits and for Layered, which lrk_upload_scene refuses in the volume integrator.
 template<typename F>
-__device__ __forceinline__ void with_closure(const DeviceScene &sc, uint32_t kind, const lrk_surface *surf, const Interaction &it, F &&f) {
-    switch (kind) {
-        case 1u: {
-            MatteClosure cl;
-            init_closure<true>(sc, cl, surf, it);
-            f(cl);
-            break;
-        }
-        case 2u: {
-            DisneyClosure cl;
-            init_closure<true>(sc, cl, surf, it);
-            f(cl);
-            break;
-        }
-        case 8u: {
-            DisneyTransClosure cl;
-            init_closure<true>(sc, cl, surf, it);
-            f(cl);
-            break;
-        }
-        case 10u: {
-            DisneyThinClosure cl;
-            init_closure<true>(sc, cl, surf, it);
-            f(cl);
-            break;
-        }
-        case 7u: {
-            MixClosure cl;
-            cl.init(*surf, sc.surfaces);
-            f(cl);
-            break;
-        }
-        case 3u: {
-            MicrofacetFamilyClosure<2u> cl;
-            init_closure<true>(sc, cl, surf, it);
-            f(cl);
-            break;
-        }
-        case 4u: {
-            MicrofacetFamilyClosure<3u> cl;
-            init_closure<true>(sc, cl, surf, it);
-            f(cl);
-            break;
-        }
-        case 5u: {
-            MicrofacetFamilyClosure<4u> cl;
-            init_closure<true>(sc, cl, surf, it);
-            f(cl);
-            break;
-        }
-        case 6u: {
-            MicrofacetFamilyClosure<5u> cl;
-            init_closure<true>(sc, cl, surf, it);
-            f(cl);
-            break;
-        }
-        default: break;
-    }
+__device__ __forceinline__ void with_closure(const DeviceScene &sc, uint32_t kind, const lrk_surface *surf, const Interaction &it, const Frame &shading,
+                                             V3 wo, F &&f) {
+    with_hit_kind(kind, [&](auto k) {
+        constexpr uint32_t K = decltype(k)::value;
+        if constexpr (K != kHitLayered) with_hit_closure<K, true>(sc, surf, it, wo, [&] { return shading; }, f);
+    });
 }
 
 template<typename Closure, typename = void>
@@ -152,7 +101,7 @@ __device__ __noinline__ inline SurfEval general_surface_evaluate(const DeviceSce
     SurfEval e;
     e.f = v3(0.f);
     e.pdf = 0.f;
-    with_closure(sc, kind, surf, it, [&](auto &cl) {
+    with_closure(sc, kind, surf, it, shading, wo, [&](auto &cl, const Frame &) {
         const V3 wo_local = shading.world_to_local(wo), wi_local = shading.world_to_local(wi);
         cl.prepare(wo_local);
         e = cl.evaluate_local(wo_local, wi_local);
@@ -177,7 +126,7 @@ __device__ __noinline__ inline GeneralSurfaceSample general_surface_shade(const 
     out.light.pdf = out.pdf = 0.f;
     out.wi = v3(0.f, 0.f, 1.f);
     out.event = LRK_EVENT_REFLECT;
-    with_closure(sc, kind, surf, it, [&](auto &cl) {
+    with_closure(sc, kind, surf, it, shading, wo, [&](auto &cl, const Frame &) {
         shade_surface_eval(cl, it, shading, wo, ls, u_lobe, ub0, ub1, out.light, out.wi, out.f, out.pdf);
         if constexpr (has_event_member<std::remove_reference_t<decltype(cl)>>::value) out.event = cl.event;
     });

@@ -45,14 +45,7 @@ extern "C" int volume_general_host(const lrk_scene_desc *s, uint32_t spp_begin, 
         std::memcpy(&o2w[i * 3u], inst.object_to_world, 48);
         std::memcpy(&handles[i], inst.handle, 16);
         const uint32_t flags = inst.handle[0] & 1023u, surface_tag = (inst.handle[1] >> 12u) & 4095u;
-        uint32_t kind = 0u;
-        if (flags & LRK_SHAPE_HAS_SURFACE) {
-            const uint32_t type = s->surfaces[surface_tag].type;
-            kind = type + 1u;
-            if (type == LRK_SURFACE_DISNEY && (s->surfaces[surface_tag].flags & LRK_SURFACE_DISNEY_TRANSMISSIVE)) kind = 8u;
-            if (type == LRK_SURFACE_DISNEY && (s->surfaces[surface_tag].flags & LRK_SURFACE_DISNEY_THIN)) kind = 10u;
-        }
-        kinds[i] = kind;
+        kinds[i] = (flags & LRK_SHAPE_HAS_SURFACE) ? hit_kind_of(s->surfaces[surface_tag]) : kHitEmitter;
         if ((flags & LRK_SHAPE_MAYBE_NON_OPAQUE) && (flags & LRK_SHAPE_HAS_SURFACE)) alpha = true;
     }
     uint32_t overflow = 0u;
