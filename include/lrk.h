@@ -564,7 +564,14 @@ int lrk_reduce_film(lrk_ctx *ctx, uint32_t root);
  *                             nodes.  Read at lrk_upload_scene; the tree is built there from the scene description.  Another value
  *                             -> LRK_ERR_INVALID_ARGUMENT.  Surface integrator only: lrk_upload_scene returns LRK_ERR_UNSUPPORTED
  *                             for the volume integrator with the option on.  A scene with one emissive instance renders bit for bit
- *                             as without it.  LRK_ABI_VERSION stays 8: no layout or signature changed */
+ *                             as without it.  LRK_ABI_VERSION stays 8: no layout or signature changed
+ *   "light_solid_angle" (0/1) point sampling of next-event estimation: the point of the chosen emissive triangle is sampled
+ *                             uniformly in the solid angle the triangle subtends at the shading point (Arvo's spherical-triangle
+ *                             sampling) where that solid angle is in [3e-4, 6.22] sr, and uniformly by area, the reference's
+ *                             sampler, elsewhere.  Less noise where a light is large or close.  Read at lrk_upload_scene; another
+ *                             value -> LRK_ERR_INVALID_ARGUMENT.  Combines with "light_tree".  Surface integrator only:
+ *                             lrk_upload_scene returns LRK_ERR_UNSUPPORTED for the volume integrator with the option on.
+ *                             LRK_ABI_VERSION stays 8: no layout or signature changed */
 int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value);
 
 int lrk_film_clear(lrk_ctx *ctx);

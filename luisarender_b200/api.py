@@ -94,11 +94,15 @@ class Renderer:
     """One GPU context. Fails loudly when libb200pt.so or a CUDA device is missing (no CPU fallback).
 
     ``light_tree=True`` sets the option "light_tree" (include/lrk.h): from the next upload on, next-event estimation picks its
-    lights from a light tree by power, distance and orientation instead of uniformly (surface integrator only)."""
+    lights from a light tree by power, distance and orientation instead of uniformly (surface integrator only).
+    ``light_solid_angle=True`` sets the option "light_solid_angle": from the next upload on, next-event estimation samples the
+    point on the chosen emissive triangle uniformly in solid angle instead of by area (surface integrator only)."""
 
-    def __init__(self, device_index: int = -1, max_paths_per_pass: int = 0, light_tree: bool = False):
+    def __init__(self, device_index: int = -1, max_paths_per_pass: int = 0, light_tree: bool = False, light_solid_angle: bool = False):
         if light_tree not in (0, 1):
             raise ValueError(f"light_tree is False or True, not {light_tree!r}")
+        if light_solid_angle not in (0, 1):
+            raise ValueError(f"light_solid_angle is False or True, not {light_solid_angle!r}")
         self._lib = F.device_lib()
         cfg = F.DeviceCfg(device_index, 0, max_paths_per_pass)
         self._ctx = C.c_void_p()
@@ -108,6 +112,8 @@ class Renderer:
         self._res = None
         if light_tree:
             self.set_option("light_tree", 1)
+        if light_solid_angle:
+            self.set_option("light_solid_angle", 1)
 
     def _check(self, rc: int, what: str):
         if rc != 0:

@@ -144,6 +144,9 @@ struct lrk_ctx {
     // kernels' instantiations
     bool light_tree_option{false}, light_tree{false};
     DeviceLightTree light_tree_rec{};// the record after the scene's device copy (scene.cuh)
+    // solid-angle light sampling (option "light_solid_angle"): latched at lrk_upload_scene into light_solid_angle, which selects the
+    // shade kernels' instantiations
+    bool light_solid_angle_option{false}, light_solid_angle{false};
 
     ~lrk_ctx();
 };
@@ -399,8 +402,8 @@ int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset,
                 if (!(ctx->used_kinds & (1u << kind))) continue;
                 const bool strict = ctx->strict_math || hit_kind_always_strict(kind);
                 const int blocks = blocks_for(ctx, n, ctx->grid_shade[strict ? 1 : 0][kind]);
-                if (strict) strict::launch_shade(kind, ctx->textured, ctx->light_tree, blocks, ctx->stream, sc, pb, depth);
-                else fast::launch_shade(kind, ctx->textured, ctx->light_tree, blocks, ctx->stream, sc, pb, depth);
+                if (strict) strict::launch_shade(kind, ctx->textured, ctx->light_tree, ctx->light_solid_angle, blocks, ctx->stream, sc, pb, depth);
+                else fast::launch_shade(kind, ctx->textured, ctx->light_tree, ctx->light_solid_angle, blocks, ctx->stream, sc, pb, depth);
                 ctx->stats.kernel_launches++;
             }
         }
@@ -752,6 +755,9 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     if (ctx->light_tree_option && s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: the light tree (option light_tree) serves the surface integrator only; the volume "
                                               "integrator selects its lights uniformly");
+    if (ctx->light_solid_angle_option && s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
+        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: solid-angle light sampling (option light_solid_angle) serves the surface integrator "
+                                              "only; the volume integrator evaluates its light pdfs from the world origin");
     if (s->camera.resolution[0] > 65535u || s->camera.resolution[1] > 65535u)
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: film larger than 65535 pixels per side");
     if (s->light_count == 0u && !s->environment.present)// !pipeline().has_lighting(), wave_path.cpp:224-228
@@ -987,6 +993,7 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     sc.medium_count = s->medium_count;
     sc.env_medium_tag = s->environment_medium_tag;
     ctx->light_tree = ctx->light_tree_option;
+    ctx->light_solid_angle = ctx->light_solid_angle_option;
     {
         auto &lt = ctx->light_tree_rec;
         lt.nodes = ctx->light_tree && !tree.nodes.empty() ? a.lt_nodes.get<const LightTreeNode>() : nullptr;
@@ -1090,6 +1097,10 @@ int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value) {
     else if (n == "light_tree") {// takes effect at the next lrk_upload_scene
         if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_tree is 0 or 1");
         ctx->light_tree_option = value != 0;
+    }
+    else if (n == "light_solid_angle") {// takes effect at the next lrk_upload_scene
+        if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_solid_angle is 0 or 1");
+        ctx->light_solid_angle_option = value != 0;
     }
     else if (n == "pin_host_buffers") {
         ctx->pin_host = value != 0;

@@ -30,12 +30,12 @@ int grid_of(Kernel kernel, int block, int sm_count) {
     return (per_sm > 0 ? per_sm : 1) * sm_count;
 }
 
-// calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection)
-template<uint32_t SEL, typename F>
+// calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection, light point sampling)
+template<uint32_t SEL, uint32_t PT, typename F>
 void with_shade_kernel(uint32_t kind, bool textured, F &&f) {
     with_hit_kind(kind, [&](auto k) {
         constexpr uint32_t K = decltype(k)::value;
-        textured ? f(shade_kernel<K, true, SEL>) : f(shade_kernel<K, false, SEL>);
+        textured ? f(shade_kernel<K, true, SEL, PT>) : f(shade_kernel<K, false, SEL, PT>);
     });
 }
 
@@ -52,7 +52,7 @@ void with_volume_surface_kernel(uint32_t kind, bool textured, F &&f) {
 
 int shade_grid(uint32_t kind, int sm_count) {
     int g = 1;
-    with_shade_kernel<kLightSelectUniform>(kind, false, [&](auto kernel) { g = grid_of(kernel, kShadeBlock, sm_count); });
+    with_shade_kernel<kLightSelectUniform, kLightPointArea>(kind, false, [&](auto kernel) { g = grid_of(kernel, kShadeBlock, sm_count); });
     return g;
 }
 
@@ -64,11 +64,16 @@ int volume_surface_grid(uint32_t kind, int sm_count) {
     return g;
 }
 
-void launch_shade(uint32_t kind, bool textured, bool light_tree, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb,
-                  uint32_t depth) {
+void launch_shade(uint32_t kind, bool textured, bool light_tree, bool solid_angle, int blocks, cudaStream_t stream, const DeviceScene &sc,
+                  const PathBuffers &pb, uint32_t depth) {
     const auto launch = [&](auto kernel) { kernel<<<blocks, kShadeBlock, 0, stream>>>(sc, pb, depth); };
-    if (light_tree) with_shade_kernel<kLightSelectTree>(kind, textured, launch);
-    else with_shade_kernel<kLightSelectUniform>(kind, textured, launch);
+    if (solid_angle) {
+        if (light_tree) with_shade_kernel<kLightSelectTree, kLightPointSolidAngle>(kind, textured, launch);
+        else with_shade_kernel<kLightSelectUniform, kLightPointSolidAngle>(kind, textured, launch);
+    } else {
+        if (light_tree) with_shade_kernel<kLightSelectTree, kLightPointArea>(kind, textured, launch);
+        else with_shade_kernel<kLightSelectUniform, kLightPointArea>(kind, textured, launch);
+    }
 }
 
 void launch_volume_medium(int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth) {

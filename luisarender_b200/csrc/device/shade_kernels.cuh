@@ -40,8 +40,9 @@ __device__ __noinline__ inline BounceDraws draw_bounce_from_tables(SamplerRef sc
 }
 
 // Sorted-by-material dispatch, step 2: one shade kernel per closure kind, each over its own hit bucket.  SEL: the light selection
-// of next-event estimation (kLightSelectTree with the option "light_tree")
-template<uint32_t KIND, bool TEXTURED = false, uint32_t SEL = kLightSelectUniform>
+// of next-event estimation (kLightSelectTree with the option "light_tree"); PT: its point sampling (kLightPointSolidAngle with the
+// option "light_solid_angle")
+template<uint32_t KIND, bool TEXTURED = false, uint32_t SEL = kLightSelectUniform, uint32_t PT = kLightPointArea>
 __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kernel(DeviceScene sc, PathBuffers pb, uint32_t depth) {
     // the compaction is written out here rather than through block_append, which raises registers or spills of most instantiations
     __shared__ uint32_t s_warp_next[kShadeBlock / 32], s_warp_shadow[kShadeBlock / 32];
@@ -70,7 +71,7 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                 it.back_facing = dot(wo, it.ng) < 0.0f;
                 // emitter hit with MIS: mega_path.cpp:80-87, uniform.cpp:50-65
                 if (sc.light_count != 0u && it.shape.has_light()) {
-                    LightEval e = evaluate_hit<TEXTURED, SEL>(sc, it, v3(ro.x, ro.y, ro.z), hit.x);
+                    LightEval e = evaluate_hit<TEXTURED, SEL, PT>(sc, it, v3(ro.x, ro.y, ro.z), hit.x);
                     V3 add = beta * e.L * balance_heuristic(pdf_bsdf, e.pdf);
                     float4 li = pb.li[ir.x];
                     li.x += add.x;
@@ -100,7 +101,7 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                     ls.eval.pdf = 0.f;
                     ls.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
                     ls.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
-                    if (sc.light_count != 0u || sc.env_prob != 0.f) ls = sample_light<TEXTURED, SEL>(sc, it, u_sel, ul0, ul1);
+                    if (sc.light_count != 0u || sc.env_prob != 0.f) ls = sample_light<TEXTURED, SEL, PT>(sc, it, u_sel, ul0, ul1);
                     const lrk_surface *surf = sc.surfaces + it.shape.surface_tag;
                     V3 contrib, wi, f;
                     float pdf;

@@ -16,9 +16,10 @@ namespace lrk {
     int volume_medium_grid(int sm_count);                                                                                                    \
     int volume_surface_grid(uint32_t kind, int sm_count);                                                                                    \
     /* `textured`: the instantiation that evaluates image-textured parameters / normal maps; `light_tree`: the one whose next-event */      \
-    /* estimation selects lights with the light tree (option "light_tree") */                                                                \
-    void launch_shade(uint32_t kind, bool textured, bool light_tree, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, \
-                      uint32_t depth);                                                                                                       \
+    /* estimation selects lights with the light tree (option "light_tree"); `solid_angle`: the one that samples the light's point */        \
+    /* in solid angle (option "light_solid_angle") */                                                                                      \
+    void launch_shade(uint32_t kind, bool textured, bool light_tree, bool solid_angle, int blocks, cudaStream_t stream, const DeviceScene &sc,  \
+                      const PathBuffers &pb, uint32_t depth);                                                                                \
     void launch_volume_medium(int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth);                \
     void launch_volume_surface(uint32_t kind, bool textured, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb,  \
                                uint32_t depth);                                                                                              \

@@ -5,6 +5,7 @@
 // and this file evaluate the same fp32 expressions.
 #pragma once
 #include "scene.cuh"
+#include "spherical_triangle.h"
 
 namespace lrk {
 
@@ -256,10 +257,50 @@ __device__ __noinline__ inline float light_tree_pmf(const LightTreeNode *nodes, 
     return pmf;
 }
 
-// `inst`: the instance hit (used by the light tree only)
-template<bool TEX = true, uint32_t SEL = kLightSelectUniform>
+// Point sampling of next-event estimation: the reference's area sampling of the chosen triangle, or, with the option
+// "light_solid_angle", uniform sampling of the spherical triangle it subtends where use_spherical allows (spherical_triangle.h)
+enum LightPoint : uint32_t { kLightPointArea = 0u, kLightPointSolidAngle = 1u };
+
+// The solid-angle code, out of line like the tree's descents.  Both read the triangle's world-space vertices as make_interaction
+// transforms them; a sample and an emitter hit take omega from the one function, so their pdfs agree bit for bit for one point.
+__device__ __forceinline__ void light_triangle_world(const DeviceScene &sc, uint32_t inst, uint32_t prim, SphVec &v0, SphVec &v1, SphVec &v2) {
+    const ShapeHandle shape = decode_handle(__ldg(sc.inst_handles + inst));
+    const lrk_mesh mesh = sc.meshes[shape.mesh];
+    const lrk_triangle tri = sc.triangles[mesh.triangle_offset + prim];
+    const float4 *vb = reinterpret_cast<const float4 *>(sc.vertices + mesh.vertex_offset);
+    const float4 a0 = __ldg(vb + tri.i0 * 2u), b0 = __ldg(vb + tri.i1 * 2u), c0 = __ldg(vb + tri.i2 * 2u);
+    const Mat34 m = load_o2w(sc, inst);
+    const V3 t = m.col(3);
+    const V3 w0 = mul3(m, v3(a0.x, a0.y, a0.z)) + t, w1 = mul3(m, v3(b0.x, b0.y, b0.z)) + t, w2 = mul3(m, v3(c0.x, c0.y, c0.z)) + t;
+    v0 = {w0.x, w0.y, w0.z};
+    v1 = {w1.x, w1.y, w1.z};
+    v2 = {w2.x, w2.y, w2.z};
+}
+__device__ __noinline__ inline float light_triangle_solid_angle(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p) {
+    SphVec v0, v1, v2;
+    light_triangle_world(sc, inst, prim, v0, v1, v2);
+    return solid_angle({p.x, p.y, p.z}, v0, v1, v2);
+}
+__device__ __noinline__ inline V3 light_triangle_sample_spherical(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p, float omega, float u0,
+                                                                  float u1) {
+    SphVec v0, v1, v2;
+    light_triangle_world(sc, inst, prim, v0, v1, v2);
+    const SphVec b = sample_spherical_triangle({p.x, p.y, p.z}, v0, v1, v2, omega, u0, u1);
+    return v3(b.x, b.y, b.z);
+}
+// The pdf of a light point of triangle it_light.prim seen from a point where its solid angle is omega: pdf[tri] / omega where the
+// spherical sampler serves the triangle there, else area_pdf, the reference's area pdf in solid angle (diffuse_light_evaluate;
+// 0 for a point that emits nothing there, which stays 0)
+__device__ __forceinline__ float light_point_pdf(const DeviceScene &sc, const Interaction &it_light, float area_pdf, float omega) {
+    if (area_pdf == 0.f || !use_spherical(omega)) return area_pdf;
+    return __ldg(sc.pdf + sc.meshes[it_light.shape.mesh].triangle_offset + it_light.prim) / omega;
+}
+
+// `inst`: the instance hit (used by the light tree and the solid-angle sampler only)
+template<bool TEX = true, uint32_t SEL = kLightSelectUniform, uint32_t PT = kLightPointArea>
 __device__ __forceinline__ LightEval evaluate_hit(const DeviceScene &sc, const Interaction &it, V3 p_from, uint32_t inst = 0u) {
     LightEval e = diffuse_light_evaluate<TEX>(sc, it, p_from);
+    if (PT == kLightPointSolidAngle && e.pdf != 0.f) e.pdf = light_point_pdf(sc, it, e.pdf, light_triangle_solid_angle(*sc.self, inst, it.prim, p_from));
     if (SEL == kLightSelectTree) {
         const DeviceLightTree &lt = light_tree_of(sc);
         e.pdf *= (1.f - sc.env_prob) * light_tree_pmf(lt.nodes, lt.inst_light, lt.trail, p_from, inst);
@@ -282,7 +323,7 @@ struct LightSample {
 // `p_shading`: it_from.p_shading(), the point the light's emission and pdf are evaluated from (diffuse.cpp:62-86) - the hit point
 // for a surface interaction, but the WORLD ORIGIN for the volume integrator's Interaction{ray->origin()}, whose shading point is
 // never set (mega_vpt_naive.cpp:283-285; the reference's renders carry that, so this library does too)
-template<bool TEX = true, uint32_t SEL = kLightSelectUniform>
+template<bool TEX = true, uint32_t SEL = kLightSelectUniform, uint32_t PT = kLightPointArea>
 __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, const Interaction &it_from, V3 p_shading, float u_sel, float u0, float u1) {
     LightSample s;
     float n = static_cast<float>(sc.light_count);
@@ -345,10 +386,19 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
     bool keep = u_remapped < entry.prob;
     uint32_t triangle_id = keep ? i : entry.alias;
     float ux = keep ? u_remapped / entry.prob : (u_remapped - entry.prob) / (1.0f - entry.prob);
-    V3 uvw = sample_uniform_triangle(ux, u1);
+    V3 uvw;
+    float omega = 0.f;
+    if (PT == kLightPointSolidAngle) {// the same two numbers drive either sampler
+        omega = light_triangle_solid_angle(*sc.self, handle.instance_id, triangle_id, p_shading);
+        uvw = use_spherical(omega) ? light_triangle_sample_spherical(*sc.self, handle.instance_id, triangle_id, p_shading, omega, ux, u1)
+                                   : sample_uniform_triangle(ux, u1);
+    } else {
+        uvw = sample_uniform_triangle(ux, u1);
+    }
     Interaction it_light = make_interaction(sc, handle.instance_id, triangle_id, uvw);
     it_light.back_facing = dot(it_light.ng, it_from.pg - it_light.pg) < 0.f;
     s.eval = diffuse_light_evaluate<TEX>(sc, it_light, p_shading);
+    if (PT == kLightPointSolidAngle) s.eval.pdf = light_point_pdf(sc, it_light, s.eval.pdf, omega);
     s.eval.pdf *= sel_prob;
     // Interaction::spawn_ray_to, src/base/interaction.cpp:25-30
     V3 p_from = p_robust(it_from, it_light.pg - it_from.pg);
@@ -360,9 +410,9 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
     return s;
 }
 
-template<bool TEX = true, uint32_t SEL = kLightSelectUniform>
+template<bool TEX = true, uint32_t SEL = kLightSelectUniform, uint32_t PT = kLightPointArea>
 __device__ __forceinline__ LightSample sample_light(const DeviceScene &sc, const Interaction &it_from, float u_sel, float u0, float u1) {
-    return sample_light_from<TEX, SEL>(sc, it_from, it_from.pg, u_sel, u0, u1);
+    return sample_light_from<TEX, SEL, PT>(sc, it_from, it_from.pg, u_sel, u0, u1);
 }
 
 // ---- image textures: src/textures/image.cpp:132-166, sampled like the reference's software sampler

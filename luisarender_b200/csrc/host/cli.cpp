@@ -18,6 +18,9 @@
 //
 // Light tree (an extension): `--light-tree` sets lrk_set_option("light_tree", 1) before the upload, so that next-event estimation
 // picks its lights by power, distance and orientation.  Surface integrator only: a volume scene fails with the library's message.
+//
+// Solid-angle light sampling (an extension): `--light-solid-angle` sets lrk_set_option("light_solid_angle", 1) before the upload, so
+// that next-event estimation samples the point on an emissive triangle uniformly in solid angle.  Surface integrator only, as above.
 #include <sys/stat.h>
 #include <sys/wait.h>
 #include <unistd.h>
@@ -47,6 +50,7 @@ void usage() {
                 "      --adaptive-min-spp <n>   Samples per pixel of the first adaptive round (default 16, at most the camera's spp)\n"
                 "      --denoise                Also write the denoised image to <stem>.denoised<ext> (one GPU only)\n"
                 "      --light-tree             Pick next-event lights from a light tree (power, distance, orientation)\n"
+                "      --light-solid-angle      Sample next-event light points uniformly in solid angle, not by area\n"
                 "  -h, --help                   Display this help message\n");
 }
 
@@ -143,7 +147,7 @@ std::string denoised_path(const std::string &file) {
 int main(int argc, char *argv[]) {
     std::string backend, scene_path;
     int device = -1, gpus = 1;
-    bool denoise = false, light_tree = false;
+    bool denoise = false, light_tree = false, light_solid_angle = false;
     std::string adaptive_arg, min_spp_arg;
     std::vector<std::string> keys, values;
     auto add_macro = [&](const std::string &d) {
@@ -187,6 +191,7 @@ int main(int argc, char *argv[]) {
         else if (a.rfind("--adaptive-min-spp=", 0) == 0) min_spp_arg = a.substr(19);
         else if (a == "--denoise") denoise = true;
         else if (a == "--light-tree") light_tree = true;
+        else if (a == "--light-solid-angle") light_solid_angle = true;
         else if (a == "-D" || a == "--define") add_macro(need("definition"));
         else if (a.rfind("-D", 0) == 0) add_macro(a.substr(2));
         else if (!a.empty() && a[0] == '-') std::fprintf(stderr, "[warning] Unrecognized options: %s\n", a.c_str());
@@ -259,6 +264,7 @@ int main(int argc, char *argv[]) {
     if (int rc = lrk_create(&cfg, &ctx); rc != 0) die("Failed to create the CUDA device context (lrk_create = " + std::to_string(rc) + ").");
     if (denoise && lrk_set_option(ctx, "gbuffer", 1) != 0) die(lrk_last_error(ctx));
     if (light_tree && lrk_set_option(ctx, "light_tree", 1) != 0) die(lrk_last_error(ctx));
+    if (light_solid_angle && lrk_set_option(ctx, "light_solid_angle", 1) != 0) die(lrk_last_error(ctx));
     if (world > 1u) {
         uint8_t id[LRK_COMM_ID_BYTES];
         exchange_comm_id(rank, id);

@@ -221,6 +221,71 @@ def many_lights(resolution=(1920, 1080), spp=64, count=48, shared_node=False, sp
                              emission_spread=spread and not shared_node, output="many_lights.exr", **kw)
 
 
+def near_light(resolution=(512, 512), spp=16, depth=10, rr_depth=0, rr_threshold=0.95, seed=19980810, irradiance=False,
+               output="near_light.exr") -> str:
+    """The frame of solid-angle light sampling (option "light_solid_angle"): a Matte room with a desk under a one-sided 1.0 x 0.6
+    panel light 0.3 above the desk top, so that the panel is large and close seen from the desk and the walls next to it.
+
+    ``irradiance=True``: one one-sided triangle light of emission 4 facing down 0.5 above a Matte plane of albedo 0.5, seen from a
+    pinhole 0.3 above the plane looking straight down (the light is behind it), ``depth`` 2: every pixel is (0.5 / pi) * E, E the
+    light's irradiance at the plane point (Lambert's polygon formula), blurred only by the pixel's box filter."""
+    out = []
+    if irradiance:
+        out.append("Surface plane_surface : Matte { Kd : Constant { v { 0.5, 0.5, 0.5 } } }")
+        out.append("Light tri_light : Diffuse { emission : Constant { v { 4.0, 4.0, 4.0 } } two_sided { false } }")
+        g = 10.0
+        pos, idx = _mesh_props([[(-g, 0.0, g), (g, 0.0, g), (g, 0.0, -g), (-g, 0.0, -g)]])
+        out.append(f"Shape plane : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} surface {{ @plane_surface }} }}")
+        tri = [(-0.9, 0.5, 0.8), (-0.7, 0.5, -1.0), (1.1, 0.5, 0.1)]  # cross(p1 - p0, p2 - p0) points down: it lights the plane
+        pos = ", ".join(_fmt(c) for v in tri for c in v)
+        out.append(f"Shape light : InlineMesh {{ positions {{ {pos} }} indices {{ 0, 1, 2 }} light {{ @tri_light }} }}")
+        shapes = ["@plane", "@light"]
+        camera = "position { 0.0, 0.3, 0.0 }\n  front { 0.0, -1.0, 0.0 }\n  up { 0.0, 0.0, -1.0 }\n  fov { 60.0 }"
+        depth = 2
+    else:
+        colors = {"white": (0.725, 0.710, 0.680), "green": (0.140, 0.450, 0.091), "red": (0.630, 0.065, 0.050), "desk": (0.55, 0.45, 0.35)}
+        for name, rgb in colors.items():
+            out.append(f"Surface {name} : Matte {{ Kd : Constant {{ v {{ {_fmt(rgb[0])}, {_fmt(rgb[1])}, {_fmt(rgb[2])} }} }} }}")
+        out.append("Light panel_light : Diffuse { emission : Constant { v { 6.0, 5.5, 4.5 } } two_sided { false } }")
+        x0, x1, y0, y1, z0, z1 = -1.0, 1.0, 0.0, 2.0, -1.0, 1.0
+        quads = {  # (name, surface, [4 vertices])
+            "floor": ("white", [(x0, y0, z1), (x1, y0, z1), (x1, y0, z0), (x0, y0, z0)]),
+            "ceiling": ("white", [(x0, y1, z1), (x0, y1, z0), (x1, y1, z0), (x1, y1, z1)]),
+            "back_wall": ("white", [(x0, y0, z0), (x1, y0, z0), (x1, y1, z0), (x0, y1, z0)]),
+            "left_wall": ("red", [(x0, y0, z1), (x0, y0, z0), (x0, y1, z0), (x0, y1, z1)]),
+            "right_wall": ("green", [(x1, y0, z0), (x1, y0, z1), (x1, y1, z1), (x1, y1, z0)]),
+            "desk_top": ("desk", [(-0.7, 0.7, 0.1), (0.7, 0.7, 0.1), (0.7, 0.7, -0.9), (-0.7, 0.7, -0.9)]),
+            "desk_front": ("desk", [(-0.7, 0.0, 0.1), (0.7, 0.0, 0.1), (0.7, 0.7, 0.1), (-0.7, 0.7, 0.1)]),
+        }
+        shapes = []
+        for name, (surface, q) in quads.items():
+            pos, idx = _mesh_props([q])
+            out.append(f"Shape {name} : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} surface {{ @{surface} }} }}")
+            shapes.append(f"@{name}")
+        pos, idx = _mesh_props([[(-0.5, 1.0, -0.1), (-0.5, 1.0, -0.7), (0.5, 1.0, -0.7), (0.5, 1.0, -0.1)]])  # facing down
+        out.append(f"Shape panel : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} light {{ @panel_light }} }}")
+        shapes.append("@panel")
+        camera = "position { 0.0, 1.1, 3.4 }\n  front { 0.0, -0.08, -1.0 }\n  up { 0.0, 1.0, 0.0 }\n  fov { 38.0 }"
+    out.append(f"""Camera camera : Pinhole {{
+  {camera}
+  spp {{ {int(spp)} }}
+  film : Color {{ resolution {{ {int(resolution[0])}, {int(resolution[1])} }} }}
+  filter : Box {{ radius {{ 0.5 }} }}
+  file {{ "{output}" }}
+}}""")
+    out.append(f"""render {{
+  integrator : WavePath {{
+    depth {{ {int(depth)} }}
+    rr_depth {{ {int(rr_depth)} }}
+    rr_threshold {{ {_fmt(rr_threshold)} }}
+    sampler : Independent {{ seed {{ {int(seed)} }} }}
+  }}
+  cameras {{ @camera }}
+  shapes {{ {", ".join(shapes)} }}
+}}""")
+    return "\n".join(out) + "\n"
+
+
 def textured_materials(resolution=(64, 40), spp=4, depth=6, rr_depth=0, rr_threshold=0.95, seed=19980810, assets="tests/golden/assets",
                        output="texmat.exr", integrator="WavePath") -> str:
     """SURVEY.md §8 row f3 with image-textured parameters: four uv-mapped panels - Mirror (colour + roughness images), Glass (Kr, Kt
