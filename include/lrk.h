@@ -571,7 +571,14 @@ int lrk_reduce_film(lrk_ctx *ctx, uint32_t root);
  *                             sampler, elsewhere.  Less noise where a light is large or close.  Read at lrk_upload_scene; another
  *                             value -> LRK_ERR_INVALID_ARGUMENT.  Combines with "light_tree".  Surface integrator only:
  *                             lrk_upload_scene returns LRK_ERR_UNSUPPORTED for the volume integrator with the option on.
- *                             LRK_ABI_VERSION stays 8: no layout or signature changed */
+ *                             LRK_ABI_VERSION stays 8: no layout or signature changed
+ *   "light_tree_triangles" (0/1) the bottom level of "light_tree": the tree also picks the triangle of the chosen emitter, from a
+ *                             tree over the triangles of its mesh in object space (power = area, the triangle's normal as its
+ *                             cone), instead of by area.  Less noise from curved one-sided lights, whose far side emits nothing
+ *                             towards the point.  Read at lrk_upload_scene, which builds one such tree per emissive mesh and side
+ *                             (about 14 us per triangle on the host); another value -> LRK_ERR_INVALID_ARGUMENT; on without
+ *                             "light_tree" -> LRK_ERR_INVALID_ARGUMENT at lrk_upload_scene.  Combines with "light_solid_angle".
+ *                             Surface integrator only, as "light_tree".  LRK_ABI_VERSION stays 8: no layout or signature changed */
 int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value);
 
 int lrk_film_clear(lrk_ctx *ctx);

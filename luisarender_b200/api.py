@@ -96,13 +96,20 @@ class Renderer:
     ``light_tree=True`` sets the option "light_tree" (include/lrk.h): from the next upload on, next-event estimation picks its
     lights from a light tree by power, distance and orientation instead of uniformly (surface integrator only).
     ``light_solid_angle=True`` sets the option "light_solid_angle": from the next upload on, next-event estimation samples the
-    point on the chosen emissive triangle uniformly in solid angle instead of by area (surface integrator only)."""
+    point on the chosen emissive triangle uniformly in solid angle instead of by area (surface integrator only).
+    ``light_tree_triangles=True`` (with ``light_tree=True``) sets the option "light_tree_triangles": the light tree also picks the
+    triangle of the chosen emitter, from a tree over its mesh's triangles, instead of by area."""
 
-    def __init__(self, device_index: int = -1, max_paths_per_pass: int = 0, light_tree: bool = False, light_solid_angle: bool = False):
+    def __init__(self, device_index: int = -1, max_paths_per_pass: int = 0, light_tree: bool = False, light_solid_angle: bool = False,
+                 light_tree_triangles: bool = False):
         if light_tree not in (0, 1):
             raise ValueError(f"light_tree is False or True, not {light_tree!r}")
         if light_solid_angle not in (0, 1):
             raise ValueError(f"light_solid_angle is False or True, not {light_solid_angle!r}")
+        if light_tree_triangles not in (0, 1):
+            raise ValueError(f"light_tree_triangles is False or True, not {light_tree_triangles!r}")
+        if light_tree_triangles and not light_tree:
+            raise ValueError("light_tree_triangles is the bottom level of the light tree: it needs light_tree=True")
         self._lib = F.device_lib()
         cfg = F.DeviceCfg(device_index, 0, max_paths_per_pass)
         self._ctx = C.c_void_p()
@@ -114,6 +121,8 @@ class Renderer:
             self.set_option("light_tree", 1)
         if light_solid_angle:
             self.set_option("light_solid_angle", 1)
+        if light_tree_triangles:
+            self.set_option("light_tree_triangles", 1)
 
     def _check(self, rc: int, what: str):
         if rc != 0:

@@ -62,14 +62,19 @@ LRK_LIGHT_TREE_FN float light_tree_importance(const LightTreeNode &n, float px, 
 }
 
 // The descent from the root.  SAMPLE: chooses with u in [0, 1) and returns the light; otherwise follows `trail` (bit d = 1: the
-// second child at depth d) and returns the leaf's light.  pmf: the probability of that choice, 0 with kLightTreeNone.
+// second child at depth d) and returns the leaf's light.  pmf: the probability of that choice, 0 with kLightTreeNone.  u_left: where
+// not null, receives u as the sampling descent left it at the leaf, remapped to [0, 1) by every choice on the way.
 template<bool SAMPLE>
-LRK_LIGHT_TREE_FN uint32_t light_tree_walk(const LightTreeNode *nodes, float px, float py, float pz, float u, unsigned long long trail, float &pmf) {
+LRK_LIGHT_TREE_FN uint32_t light_tree_walk(const LightTreeNode *nodes, float px, float py, float pz, float u, unsigned long long trail, float &pmf,
+                                           float *u_left = nullptr) {
     pmf = 1.f;
     uint32_t i = 0u;
     for (;;) {
         const uint32_t index = nodes[i].index;
-        if (index & kLightTreeLeaf) return index & ~kLightTreeLeaf;
+        if (index & kLightTreeLeaf) {
+            if (u_left != nullptr) *u_left = u;
+            return index & ~kLightTreeLeaf;
+        }
         const float il = light_tree_importance(nodes[index], px, py, pz), ir = light_tree_importance(nodes[index + 1u], px, py, pz);
         const float total = il + ir;
         if (!(total > 0.f)) {
@@ -88,6 +93,22 @@ LRK_LIGHT_TREE_FN uint32_t light_tree_walk(const LightTreeNode *nodes, float px,
         pmf *= second ? pr : pl;
         i = index + (second ? 1u : 0u);
     }
+}
+
+// The bottom level of the option "light_tree_triangles": one tree per emissive mesh over its triangles, in the mesh's object space.
+// The shading point enters it mapped by the instance's world-to-object rows w2o (row-major 3x4) with the expressions traversal uses
+// (traverse.cuh); facing is invariant under that map, so the orientation cull stays conservative for any invertible transform.
+LRK_LIGHT_TREE_FN void light_tree_object_point(const float *w2o, float px, float py, float pz, float &qx, float &qy, float &qz) {
+    qx = fmaf(w2o[0], px, fmaf(w2o[1], py, fmaf(w2o[2], pz, w2o[3])));
+    qy = fmaf(w2o[4], px, fmaf(w2o[5], py, fmaf(w2o[6], pz, w2o[7])));
+    qz = fmaf(w2o[8], px, fmaf(w2o[9], py, fmaf(w2o[10], pz, w2o[11])));
+}
+
+// pmf of triangle `prim` of a bottom tree at object-space point q, following its trail.  A triangle the build left out (no area)
+// has trail 0, which leads to another triangle's leaf: pmf 0.
+LRK_LIGHT_TREE_FN float light_tree_triangle_pmf_at(const LightTreeNode *nodes, float qx, float qy, float qz, unsigned long long trail, uint32_t prim) {
+    float pmf;
+    return light_tree_walk<false>(nodes, qx, qy, qz, 0.f, trail, pmf) == prim ? pmf : 0.f;
 }
 
 }// namespace lrk
@@ -337,6 +358,28 @@ inline LightTreeBuild light_tree_build(const std::vector<LightTreeEmitter> &emit
     out.nodes.resize(1u);
     light_tree_detail::Builder{emitters, out}.build(lights, 0u, lights.size(), 0u, 0, 0ull);
     return out;
+}
+
+// The sides a bottom tree is built for: the triangles emit along cross(p1 - p0, p2 - p0) in object space; an instance whose
+// transform has a negative determinant emits along the negated normal (make_interaction takes ng from world-space edges); a
+// two-sided light emits along both.
+enum LightTreeSide : uint32_t { kLightTreeOneSided = 0u, kLightTreeMirrored = 1u, kLightTreeTwoSided = 2u };
+
+// The bottom tree of one emissive mesh: one emitter per object-space triangle (9 doubles each), phi = its area, its cone the
+// triangle's normal on the side it emits to (the whole sphere when two-sided).  Degenerate triangles get phi = 0 and stay out.
+inline LightTreeBuild light_tree_build_triangles(const std::vector<double> &tris, LightTreeSide side) {
+    std::vector<LightTreeEmitter> emitters;
+    emitters.reserve(tris.size() / 9u);
+    std::vector<double> one(9u);
+    for (size_t t = 0; t + 9u <= tris.size(); t += 9u) {
+        std::copy(tris.begin() + static_cast<std::ptrdiff_t>(t), tris.begin() + static_cast<std::ptrdiff_t>(t + 9u), one.begin());
+        LightTreeEmitter e = light_tree_emitter(one, 1.0, side == kLightTreeTwoSided);
+        if (side == kLightTreeTwoSided) e.phi *= 0.5;
+        if (side == kLightTreeMirrored)
+            for (double &a : e.axis) a = -a;
+        emitters.push_back(e);
+    }
+    return light_tree_build(emitters);
 }
 
 }// namespace lrk

@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstring>
 #include <limits>
+#include <map>
 #include <memory>
 #include <string>
 #include <type_traits>
@@ -61,7 +62,8 @@ private:
 
 struct DeviceArrays {
     DeviceBuffer vertices, triangles, alias, pdf, meshes, inst_handles, inst_kind, inst_o2w, inst_xform, bvh_nodes, traversal_overflow, sobol, vdc, vdc_inv, pmj, blue_noise, pmj_pixels, zsobol_hash, sampler, build_scratch, mesh_bounds, inst_mesh, visible_ids, scene_copy, media, textures, texels, env_alias, env_pdf,
-        tri_verts, surfaces, lights, light_handles, camera, lt_nodes, lt_light_inst, lt_trail, lt_inst_light;
+        tri_verts, surfaces, lights, light_handles, camera, lt_nodes, lt_light_inst, lt_trail, lt_inst_light, lt_bottom_nodes, lt_inst_bottom,
+        lt_bottom_trail;
 };
 
 enum KernelCategory { CAT_TRACE_CLOSEST = 0, CAT_TRACE_SHADOW = 1, CAT_SHADE = 2, CAT_OTHER = 3, CAT_COUNT = 4 };
@@ -144,6 +146,9 @@ struct lrk_ctx {
     // kernels' instantiations
     bool light_tree_option{false}, light_tree{false};
     DeviceLightTree light_tree_rec{};// the record after the scene's device copy (scene.cuh)
+    // triangle-level light trees (option "light_tree_triangles"): read at lrk_upload_scene, which then builds the bottom trees; the
+    // kernels find them through light_tree_rec.bottom_nodes
+    bool light_tree_triangles_option{false};
     // solid-angle light sampling (option "light_solid_angle"): latched at lrk_upload_scene into light_solid_angle, which selects the
     // shade kernels' instantiations
     bool light_solid_angle_option{false}, light_solid_angle{false};
@@ -638,6 +643,43 @@ int build_light_tree(lrk_ctx *ctx, const lrk_scene_desc *s, LightTreeBuild &tree
     return LRK_OK;
 }
 
+// The bottom trees of the option "light_tree_triangles" (light_tree_build_triangles): one per distinct (mesh, side) pair among the
+// instances of the top tree, shared by all of them.  nodes: the trees one after the other; inst_bottom: per instance {root, first
+// trail} (2 words), root kLightTreeNone for none; trail: per tree, one trail per triangle of its mesh.
+void build_bottom_light_trees(const lrk_scene_desc *s, const std::vector<uint32_t> &inst_light, std::vector<LightTreeNode> &nodes,
+                              std::vector<uint32_t> &inst_bottom, std::vector<unsigned long long> &trail) {
+    inst_bottom.assign(2u * s->instance_count, 0u);
+    std::map<std::pair<uint32_t, uint32_t>, std::pair<uint32_t, uint32_t>> built;// (mesh, side) -> (root, first trail)
+    std::vector<double> tris;
+    for (uint32_t i = 0; i < s->instance_count; i++) {
+        inst_bottom[2u * i] = kLightTreeNone;
+        if (inst_light[i] == kLightTreeNone) continue;
+        const auto &inst = s->instances[i];
+        const float *m = inst.object_to_world;// row-major 3x4
+        const double det = static_cast<double>(m[0]) * (static_cast<double>(m[5]) * m[10] - static_cast<double>(m[6]) * m[9]) -
+                           static_cast<double>(m[1]) * (static_cast<double>(m[4]) * m[10] - static_cast<double>(m[6]) * m[8]) +
+                           static_cast<double>(m[2]) * (static_cast<double>(m[4]) * m[9] - static_cast<double>(m[5]) * m[8]);
+        const LightTreeSide side = s->lights[inst.handle[1] & 4095u].two_sided ? kLightTreeTwoSided : det < 0.0 ? kLightTreeMirrored : kLightTreeOneSided;
+        auto it = built.find({inst.mesh, side});
+        if (it == built.end()) {
+            const lrk_mesh &mesh = s->meshes[inst.mesh];
+            tris.clear();
+            for (uint32_t t = 0; t < mesh.triangle_count; t++) {
+                const lrk_triangle &tri = s->triangles[mesh.triangle_offset + t];
+                for (uint32_t v : {tri.i0, tri.i1, tri.i2})
+                    for (int c = 0; c < 3; c++) tris.push_back(s->vertices[mesh.vertex_offset + v].p[c]);
+            }
+            const LightTreeBuild b = light_tree_build_triangles(tris, side);
+            const uint32_t root = b.nodes.empty() ? kLightTreeNone : static_cast<uint32_t>(nodes.size());
+            it = built.emplace(std::make_pair(inst.mesh, static_cast<uint32_t>(side)), std::make_pair(root, static_cast<uint32_t>(trail.size()))).first;
+            nodes.insert(nodes.end(), b.nodes.begin(), b.nodes.end());
+            trail.insert(trail.end(), b.trail.begin(), b.trail.end());
+        }
+        inst_bottom[2u * i] = it->second.first;
+        inst_bottom[2u * i + 1u] = it->second.second;
+    }
+}
+
 }// namespace
 
 // The one teardown of a context, run with its device current and its stream idle (lrk_destroy, or a failed lrk_create).  The device
@@ -755,6 +797,9 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     if (ctx->light_tree_option && s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: the light tree (option light_tree) serves the surface integrator only; the volume "
                                               "integrator selects its lights uniformly");
+    if (ctx->light_tree_triangles_option && !ctx->light_tree_option)
+        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: the triangle-level light trees (option light_tree_triangles) are the bottom "
+                                                   "level of the light tree: set the option light_tree too");
     if (ctx->light_solid_angle_option && s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: solid-angle light sampling (option light_solid_angle) serves the surface integrator "
                                               "only; the volume integrator evaluates its light pdfs from the world origin");
@@ -920,6 +965,15 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         if ((rc = upload(ctx, a.lt_trail, tree.trail.data(), tree.trail.size()))) return rc;
         if ((rc = upload(ctx, a.lt_inst_light, inst_light.data(), inst_light.size()))) return rc;
     }
+    std::vector<LightTreeNode> bottom_nodes;
+    std::vector<uint32_t> inst_bottom;
+    std::vector<unsigned long long> bottom_trail;
+    if (ctx->light_tree_triangles_option) {
+        build_bottom_light_trees(s, inst_light, bottom_nodes, inst_bottom, bottom_trail);
+        if ((rc = upload(ctx, a.lt_bottom_nodes, bottom_nodes.data(), bottom_nodes.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_inst_bottom, inst_bottom.data(), inst_bottom.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_bottom_trail, bottom_trail.data(), bottom_trail.size()))) return rc;
+    }
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
 
     auto &sc = ctx->scene;
@@ -1000,6 +1054,10 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         lt.light_inst = ctx->light_tree ? a.lt_light_inst.get<const uint32_t>() : nullptr;
         lt.trail = ctx->light_tree ? a.lt_trail.get<const unsigned long long>() : nullptr;
         lt.inst_light = ctx->light_tree ? a.lt_inst_light.get<const uint32_t>() : nullptr;
+        const bool bottom = ctx->light_tree_triangles_option && !bottom_nodes.empty();
+        lt.bottom_nodes = bottom ? a.lt_bottom_nodes.get<const LightTreeNode>() : nullptr;
+        lt.inst_bottom = bottom ? a.lt_inst_bottom.get<const uint2>() : nullptr;
+        lt.bottom_trail = bottom ? a.lt_bottom_trail.get<const unsigned long long>() : nullptr;
     }
 
     const size_t npix = static_cast<size_t>(sc.width) * sc.height;
@@ -1097,6 +1155,10 @@ int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value) {
     else if (n == "light_tree") {// takes effect at the next lrk_upload_scene
         if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_tree is 0 or 1");
         ctx->light_tree_option = value != 0;
+    }
+    else if (n == "light_tree_triangles") {// takes effect at the next lrk_upload_scene
+        if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_tree_triangles is 0 or 1");
+        ctx->light_tree_triangles_option = value != 0;
     }
     else if (n == "light_solid_angle") {// takes effect at the next lrk_upload_scene
         if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_solid_angle is 0 or 1");

@@ -77,6 +77,12 @@ struct DeviceLightTree {
     const uint32_t *light_inst;        // per tree light: its instance
     const unsigned long long *trail;   // per tree light: its root-to-leaf bit trail
     const uint32_t *inst_light;        // per instance: its tree light, kLightTreeNone for none
+    // The bottom level (option "light_tree_triangles"): a tree over the triangles of each emissive (mesh, side) pair, in object
+    // space.  All null unless the option was on at lrk_upload_scene; then the triangle's probability is part of the selection pmf.
+    const LightTreeNode *bottom_nodes;         // every bottom tree, each a slice whose child indices are relative to its root
+    const uint2 *inst_bottom;                  // per instance: {root of its bottom tree in bottom_nodes, first of its trails}, root
+                                               // kLightTreeNone for none
+    const unsigned long long *bottom_trail;    // per triangle of a bottom tree: its trail
 };
 __device__ __forceinline__ const DeviceLightTree &light_tree_of(const DeviceScene &sc) {
     return *reinterpret_cast<const DeviceLightTree *>(sc.self + 1);

@@ -221,11 +221,13 @@ struct LightEval {
 // image emission: max(texel.xyz, 0) at the interaction's uv (texture.cpp:47-57, srgb.cpp:48-54).  TEX: only the TEXTURED kernel
 // variants contain the lookup (lrk_upload_scene selects them when a light has an emission texture); the others keep the constant
 __device__ __noinline__ inline V3 light_emission_texel(const DeviceScene &sc, uint32_t emission_tex, float u, float v);
+// triangle_selected: the light selection chose the triangle itself (the bottom light trees), so its probability is in the selection
+// pmf and the point's pdf is 1 / area of the triangle
 template<bool TEX = true>
-__device__ __forceinline__ LightEval diffuse_light_evaluate(const DeviceScene &sc, const Interaction &it_light, V3 p_from) {
+__device__ __forceinline__ LightEval diffuse_light_evaluate(const DeviceScene &sc, const Interaction &it_light, V3 p_from, bool triangle_selected = false) {
     const lrk_light light = sc.lights[it_light.shape.light_tag];
     const lrk_mesh mesh = sc.meshes[it_light.shape.mesh];
-    float pdf_triangle = __ldg(sc.pdf + mesh.triangle_offset + it_light.prim);
+    float pdf_triangle = triangle_selected ? 1.f : __ldg(sc.pdf + mesh.triangle_offset + it_light.prim);
     float pdf_area = pdf_triangle / it_light.prim_area;
     float cos_wo = abs_dot(normalize(p_from - it_light.pg), it_light.ng);
     V3 L = v3(light.emission[0], light.emission[1], light.emission[2]);
@@ -245,8 +247,8 @@ __device__ __forceinline__ LightEval diffuse_light_evaluate(const DeviceScene &s
 enum LightSelect : uint32_t { kLightSelectUniform = 0u, kLightSelectTree = 1u };
 
 // The descents of the light tree, out of line so that the shade kernels' register allocation does not grow with them.
-__device__ __noinline__ inline uint32_t light_tree_sample(const LightTreeNode *nodes, V3 p, float u, float &pmf) {
-    return light_tree_walk<true>(nodes, p.x, p.y, p.z, u, 0ull, pmf);
+__device__ __noinline__ inline uint32_t light_tree_sample(const LightTreeNode *nodes, V3 p, float u, float &pmf, float &u_left) {
+    return light_tree_walk<true>(nodes, p.x, p.y, p.z, u, 0ull, pmf, &u_left);
 }
 __device__ __noinline__ inline float light_tree_pmf(const LightTreeNode *nodes, const uint32_t *inst_light, const unsigned long long *trail, V3 p,
                                                     uint32_t inst) {
@@ -255,6 +257,33 @@ __device__ __noinline__ inline float light_tree_pmf(const LightTreeNode *nodes, 
     float pmf;
     light_tree_walk<false>(nodes, p.x, p.y, p.z, 0.f, __ldg(trail + l), pmf);
     return pmf;
+}
+
+// The bottom level (option "light_tree_triangles", light_tree_of(sc).bottom_nodes not null): the walk of instance inst's tree over
+// its mesh's triangles at p mapped to object space.  Sampling continues with the u the top walk left; both return pmf 0 and the
+// sample kLightTreeNone for an instance without a tree or a point no triangle faces.
+__device__ __forceinline__ V3 light_tree_to_object(const DeviceScene &sc, uint32_t inst, V3 p) {
+    const float4 *x = sc.inst_xform + static_cast<size_t>(inst) * 4u;
+    const float4 m0 = __ldg(x + 0), m1 = __ldg(x + 1), m2 = __ldg(x + 2);
+    const float w2o[12] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w, m2.x, m2.y, m2.z, m2.w};
+    V3 q;
+    light_tree_object_point(w2o, p.x, p.y, p.z, q.x, q.y, q.z);
+    return q;
+}
+__device__ __noinline__ inline uint32_t light_tree_sample_triangle(const DeviceScene &sc, uint32_t inst, V3 p, float u, float &pmf) {
+    const DeviceLightTree &lt = light_tree_of(sc);
+    const uint32_t root = __ldg(lt.inst_bottom + inst).x;
+    pmf = 0.f;
+    if (root == kLightTreeNone) return kLightTreeNone;
+    const V3 q = light_tree_to_object(sc, inst, p);
+    return light_tree_walk<true>(lt.bottom_nodes + root, q.x, q.y, q.z, u, 0ull, pmf);
+}
+__device__ __noinline__ inline float light_tree_triangle_pmf(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p) {
+    const DeviceLightTree &lt = light_tree_of(sc);
+    const uint2 b = __ldg(lt.inst_bottom + inst);
+    if (b.x == kLightTreeNone) return 0.f;
+    const V3 q = light_tree_to_object(sc, inst, p);
+    return light_tree_triangle_pmf_at(lt.bottom_nodes + b.x, q.x, q.y, q.z, __ldg(lt.bottom_trail + b.y + prim), prim);
 }
 
 // Point sampling of next-event estimation: the reference's area sampling of the chosen triangle, or, with the option
@@ -290,20 +319,26 @@ __device__ __noinline__ inline V3 light_triangle_sample_spherical(const DeviceSc
 }
 // The pdf of a light point of triangle it_light.prim seen from a point where its solid angle is omega: pdf[tri] / omega where the
 // spherical sampler serves the triangle there, else area_pdf, the reference's area pdf in solid angle (diffuse_light_evaluate;
-// 0 for a point that emits nothing there, which stays 0)
-__device__ __forceinline__ float light_point_pdf(const DeviceScene &sc, const Interaction &it_light, float area_pdf, float omega) {
+// 0 for a point that emits nothing there, which stays 0; triangle_selected as in diffuse_light_evaluate: 1 / omega)
+__device__ __forceinline__ float light_point_pdf(const DeviceScene &sc, const Interaction &it_light, float area_pdf, float omega,
+                                                 bool triangle_selected = false) {
     if (area_pdf == 0.f || !use_spherical(omega)) return area_pdf;
-    return __ldg(sc.pdf + sc.meshes[it_light.shape.mesh].triangle_offset + it_light.prim) / omega;
+    return (triangle_selected ? 1.f : __ldg(sc.pdf + sc.meshes[it_light.shape.mesh].triangle_offset + it_light.prim)) / omega;
 }
 
 // `inst`: the instance hit (used by the light tree and the solid-angle sampler only)
 template<bool TEX = true, uint32_t SEL = kLightSelectUniform, uint32_t PT = kLightPointArea>
 __device__ __forceinline__ LightEval evaluate_hit(const DeviceScene &sc, const Interaction &it, V3 p_from, uint32_t inst = 0u) {
-    LightEval e = diffuse_light_evaluate<TEX>(sc, it, p_from);
-    if (PT == kLightPointSolidAngle && e.pdf != 0.f) e.pdf = light_point_pdf(sc, it, e.pdf, light_triangle_solid_angle(*sc.self, inst, it.prim, p_from));
+    // with the bottom light trees the selection pmf holds the triangle's probability (the top pmf times the bottom pmf)
+    const bool tri_sel = SEL == kLightSelectTree && light_tree_of(sc).bottom_nodes != nullptr;
+    LightEval e = diffuse_light_evaluate<TEX>(sc, it, p_from, tri_sel);
+    if (PT == kLightPointSolidAngle && e.pdf != 0.f)
+        e.pdf = light_point_pdf(sc, it, e.pdf, light_triangle_solid_angle(*sc.self, inst, it.prim, p_from), tri_sel);
     if (SEL == kLightSelectTree) {
         const DeviceLightTree &lt = light_tree_of(sc);
-        e.pdf *= (1.f - sc.env_prob) * light_tree_pmf(lt.nodes, lt.inst_light, lt.trail, p_from, inst);
+        float pmf = light_tree_pmf(lt.nodes, lt.inst_light, lt.trail, p_from, inst);
+        if (tri_sel && pmf != 0.f) pmf *= light_tree_triangle_pmf(*sc.self, inst, it.prim, p_from);
+        e.pdf *= (1.f - sc.env_prob) * pmf;
         return e;
     }
     float n = static_cast<float>(sc.light_count);
@@ -332,6 +367,8 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
     bool is_env = ep == 1.f;
     uint32_t tag = 0u;
     float sel_prob = 1.f;
+    bool tri_sel = false;// the bottom light trees chose the triangle: tree_tri
+    uint32_t tree_tri = 0u;
     if (SEL == kLightSelectTree) {// the environment keeps its probability; the tree divides the rest
         float uu = u_sel;
         if (ep != 0.f && ep != 1.f) {
@@ -343,8 +380,16 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
         } else {
             const DeviceLightTree &lt = light_tree_of(sc);
             const LightTreeNode *nodes = lt.nodes;
-            float pmf = 0.f;
-            const uint32_t l = nodes != nullptr ? light_tree_sample(nodes, it_from.pg, uu, pmf) : kLightTreeNone;
+            float pmf = 0.f, u_left = 0.f;
+            uint32_t l = nodes != nullptr ? light_tree_sample(nodes, it_from.pg, uu, pmf, u_left) : kLightTreeNone;
+            if (l != kLightTreeNone) tag = __ldg(lt.light_inst + l);// the instance itself
+            tri_sel = lt.bottom_nodes != nullptr;
+            if (tri_sel && l != kLightTreeNone) {// one selection number for the whole descent: the top walk's u continues
+                float tri_pmf;
+                tree_tri = light_tree_sample_triangle(*sc.self, tag, it_from.pg, u_left, tri_pmf);
+                if (tree_tri == kLightTreeNone) l = kLightTreeNone;
+                pmf *= tri_pmf;
+            }
             if (l == kLightTreeNone) {// no emitter can reach the point: nothing to trace
                 s.eval.L = v3(0.f);
                 s.eval.pdf = 0.f;
@@ -352,7 +397,6 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
                 s.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
                 return s;
             }
-            tag = __ldg(lt.light_inst + l);// the instance itself
             sel_prob = ep == 0.f ? pmf : (1.f - ep) * pmf;
         }
     } else if (ep == 0.f) {
@@ -378,14 +422,20 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
     else handle = sc.light_handles[tag];
     ShapeHandle light_inst = decode_handle(__ldg(sc.inst_handles + handle.instance_id));
     const lrk_mesh mesh = sc.meshes[light_inst.mesh];
-    // sample_alias_table: src/util/sampling.h:38-50
-    float u = u0 * static_cast<float>(light_inst.tri_count);
-    uint32_t i = min(max(static_cast<uint32_t>(u), 0u), light_inst.tri_count - 1u);
-    float u_remapped = u - floorf(u);
-    lrk_alias_entry entry = sc.alias[mesh.triangle_offset + i];
-    bool keep = u_remapped < entry.prob;
-    uint32_t triangle_id = keep ? i : entry.alias;
-    float ux = keep ? u_remapped / entry.prob : (u_remapped - entry.prob) / (1.0f - entry.prob);
+    uint32_t triangle_id;
+    float ux;
+    if (SEL == kLightSelectTree && tri_sel) {
+        triangle_id = tree_tri;
+        ux = u0;
+    } else {// sample_alias_table: src/util/sampling.h:38-50
+        float u = u0 * static_cast<float>(light_inst.tri_count);
+        uint32_t i = min(max(static_cast<uint32_t>(u), 0u), light_inst.tri_count - 1u);
+        float u_remapped = u - floorf(u);
+        lrk_alias_entry entry = sc.alias[mesh.triangle_offset + i];
+        bool keep = u_remapped < entry.prob;
+        triangle_id = keep ? i : entry.alias;
+        ux = keep ? u_remapped / entry.prob : (u_remapped - entry.prob) / (1.0f - entry.prob);
+    }
     V3 uvw;
     float omega = 0.f;
     if (PT == kLightPointSolidAngle) {// the same two numbers drive either sampler
@@ -397,8 +447,8 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
     }
     Interaction it_light = make_interaction(sc, handle.instance_id, triangle_id, uvw);
     it_light.back_facing = dot(it_light.ng, it_from.pg - it_light.pg) < 0.f;
-    s.eval = diffuse_light_evaluate<TEX>(sc, it_light, p_shading);
-    if (PT == kLightPointSolidAngle) s.eval.pdf = light_point_pdf(sc, it_light, s.eval.pdf, omega);
+    s.eval = diffuse_light_evaluate<TEX>(sc, it_light, p_shading, tri_sel);
+    if (PT == kLightPointSolidAngle) s.eval.pdf = light_point_pdf(sc, it_light, s.eval.pdf, omega, tri_sel);
     s.eval.pdf *= sel_prob;
     // Interaction::spawn_ray_to, src/base/interaction.cpp:25-30
     V3 p_from = p_robust(it_from, it_light.pg - it_from.pg);

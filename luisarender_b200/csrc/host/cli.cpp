@@ -21,6 +21,9 @@
 //
 // Solid-angle light sampling (an extension): `--light-solid-angle` sets lrk_set_option("light_solid_angle", 1) before the upload, so
 // that next-event estimation samples the point on an emissive triangle uniformly in solid angle.  Surface integrator only, as above.
+//
+// Triangle-level light trees (an extension): `--light-tree-triangles` sets the options "light_tree" and "light_tree_triangles", so
+// that the light tree also picks the emissive triangle by power, distance and orientation.  Surface integrator only, as above.
 #include <sys/stat.h>
 #include <sys/wait.h>
 #include <unistd.h>
@@ -51,6 +54,7 @@ void usage() {
                 "      --denoise                Also write the denoised image to <stem>.denoised<ext> (one GPU only)\n"
                 "      --light-tree             Pick next-event lights from a light tree (power, distance, orientation)\n"
                 "      --light-solid-angle      Sample next-event light points uniformly in solid angle, not by area\n"
+                "      --light-tree-triangles   Also pick the emissive triangle from the light tree (implies --light-tree)\n"
                 "  -h, --help                   Display this help message\n");
 }
 
@@ -147,7 +151,7 @@ std::string denoised_path(const std::string &file) {
 int main(int argc, char *argv[]) {
     std::string backend, scene_path;
     int device = -1, gpus = 1;
-    bool denoise = false, light_tree = false, light_solid_angle = false;
+    bool denoise = false, light_tree = false, light_solid_angle = false, light_tree_triangles = false;
     std::string adaptive_arg, min_spp_arg;
     std::vector<std::string> keys, values;
     auto add_macro = [&](const std::string &d) {
@@ -192,6 +196,7 @@ int main(int argc, char *argv[]) {
         else if (a == "--denoise") denoise = true;
         else if (a == "--light-tree") light_tree = true;
         else if (a == "--light-solid-angle") light_solid_angle = true;
+        else if (a == "--light-tree-triangles") light_tree = light_tree_triangles = true;
         else if (a == "-D" || a == "--define") add_macro(need("definition"));
         else if (a.rfind("-D", 0) == 0) add_macro(a.substr(2));
         else if (!a.empty() && a[0] == '-') std::fprintf(stderr, "[warning] Unrecognized options: %s\n", a.c_str());
@@ -265,6 +270,7 @@ int main(int argc, char *argv[]) {
     if (denoise && lrk_set_option(ctx, "gbuffer", 1) != 0) die(lrk_last_error(ctx));
     if (light_tree && lrk_set_option(ctx, "light_tree", 1) != 0) die(lrk_last_error(ctx));
     if (light_solid_angle && lrk_set_option(ctx, "light_solid_angle", 1) != 0) die(lrk_last_error(ctx));
+    if (light_tree_triangles && lrk_set_option(ctx, "light_tree_triangles", 1) != 0) die(lrk_last_error(ctx));
     if (world > 1u) {
         uint8_t id[LRK_COMM_ID_BYTES];
         exchange_comm_id(rank, id);

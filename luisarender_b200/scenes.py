@@ -243,29 +243,43 @@ def near_light(resolution=(512, 512), spp=16, depth=10, rr_depth=0, rr_threshold
         camera = "position { 0.0, 0.3, 0.0 }\n  front { 0.0, -1.0, 0.0 }\n  up { 0.0, 0.0, -1.0 }\n  fov { 60.0 }"
         depth = 2
     else:
-        colors = {"white": (0.725, 0.710, 0.680), "green": (0.140, 0.450, 0.091), "red": (0.630, 0.065, 0.050), "desk": (0.55, 0.45, 0.35)}
-        for name, rgb in colors.items():
-            out.append(f"Surface {name} : Matte {{ Kd : Constant {{ v {{ {_fmt(rgb[0])}, {_fmt(rgb[1])}, {_fmt(rgb[2])} }} }} }}")
-        out.append("Light panel_light : Diffuse { emission : Constant { v { 6.0, 5.5, 4.5 } } two_sided { false } }")
-        x0, x1, y0, y1, z0, z1 = -1.0, 1.0, 0.0, 2.0, -1.0, 1.0
-        quads = {  # (name, surface, [4 vertices])
-            "floor": ("white", [(x0, y0, z1), (x1, y0, z1), (x1, y0, z0), (x0, y0, z0)]),
-            "ceiling": ("white", [(x0, y1, z1), (x0, y1, z0), (x1, y1, z0), (x1, y1, z1)]),
-            "back_wall": ("white", [(x0, y0, z0), (x1, y0, z0), (x1, y1, z0), (x0, y1, z0)]),
-            "left_wall": ("red", [(x0, y0, z1), (x0, y0, z0), (x0, y1, z0), (x0, y1, z1)]),
-            "right_wall": ("green", [(x1, y0, z0), (x1, y0, z1), (x1, y1, z1), (x1, y1, z0)]),
-            "desk_top": ("desk", [(-0.7, 0.7, 0.1), (0.7, 0.7, 0.1), (0.7, 0.7, -0.9), (-0.7, 0.7, -0.9)]),
-            "desk_front": ("desk", [(-0.7, 0.0, 0.1), (0.7, 0.0, 0.1), (0.7, 0.7, 0.1), (-0.7, 0.7, 0.1)]),
-        }
-        shapes = []
-        for name, (surface, q) in quads.items():
-            pos, idx = _mesh_props([q])
-            out.append(f"Shape {name} : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} surface {{ @{surface} }} }}")
-            shapes.append(f"@{name}")
+        shapes = _matte_room(out, "Light panel_light : Diffuse { emission : Constant { v { 6.0, 5.5, 4.5 } } two_sided { false } }")
         pos, idx = _mesh_props([[(-0.5, 1.0, -0.1), (-0.5, 1.0, -0.7), (0.5, 1.0, -0.7), (0.5, 1.0, -0.1)]])  # facing down
         out.append(f"Shape panel : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} light {{ @panel_light }} }}")
         shapes.append("@panel")
-        camera = "position { 0.0, 1.1, 3.4 }\n  front { 0.0, -0.08, -1.0 }\n  up { 0.0, 1.0, 0.0 }\n  fov { 38.0 }"
+        camera = _MATTE_ROOM_CAMERA
+    return _matte_room_render(out, shapes, camera, resolution, spp, depth, rr_depth, rr_threshold, seed, output)
+
+
+_MATTE_ROOM_CAMERA = "position { 0.0, 1.1, 3.4 }\n  front { 0.0, -0.08, -1.0 }\n  up { 0.0, 1.0, 0.0 }\n  fov { 38.0 }"
+
+
+def _matte_room(out, light_line):
+    """The Matte room of ``near_light`` and ``emissive_globe``: its surfaces, the Light node ``light_line``, then its walls and desk.
+    Returns the shape references."""
+    colors = {"white": (0.725, 0.710, 0.680), "green": (0.140, 0.450, 0.091), "red": (0.630, 0.065, 0.050), "desk": (0.55, 0.45, 0.35)}
+    for name, rgb in colors.items():
+        out.append(f"Surface {name} : Matte {{ Kd : Constant {{ v {{ {_fmt(rgb[0])}, {_fmt(rgb[1])}, {_fmt(rgb[2])} }} }} }}")
+    out.append(light_line)
+    x0, x1, y0, y1, z0, z1 = -1.0, 1.0, 0.0, 2.0, -1.0, 1.0
+    quads = {  # (name, surface, [4 vertices])
+        "floor": ("white", [(x0, y0, z1), (x1, y0, z1), (x1, y0, z0), (x0, y0, z0)]),
+        "ceiling": ("white", [(x0, y1, z1), (x0, y1, z0), (x1, y1, z0), (x1, y1, z1)]),
+        "back_wall": ("white", [(x0, y0, z0), (x1, y0, z0), (x1, y1, z0), (x0, y1, z0)]),
+        "left_wall": ("red", [(x0, y0, z1), (x0, y0, z0), (x0, y1, z0), (x0, y1, z1)]),
+        "right_wall": ("green", [(x1, y0, z0), (x1, y0, z1), (x1, y1, z1), (x1, y1, z0)]),
+        "desk_top": ("desk", [(-0.7, 0.7, 0.1), (0.7, 0.7, 0.1), (0.7, 0.7, -0.9), (-0.7, 0.7, -0.9)]),
+        "desk_front": ("desk", [(-0.7, 0.0, 0.1), (0.7, 0.0, 0.1), (0.7, 0.7, 0.1), (-0.7, 0.7, 0.1)]),
+    }
+    shapes = []
+    for name, (surface, q) in quads.items():
+        pos, idx = _mesh_props([q])
+        out.append(f"Shape {name} : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} surface {{ @{surface} }} }}")
+        shapes.append(f"@{name}")
+    return shapes
+
+
+def _matte_room_render(out, shapes, camera, resolution, spp, depth, rr_depth, rr_threshold, seed, output) -> str:
     out.append(f"""Camera camera : Pinhole {{
   {camera}
   spp {{ {int(spp)} }}
@@ -284,6 +298,74 @@ def near_light(resolution=(512, 512), spp=16, depth=10, rr_depth=0, rr_threshold
   shapes {{ {", ".join(shapes)} }}
 }}""")
     return "\n".join(out) + "\n"
+
+
+def _icosphere(subdivision: int):
+    """The unit icosphere of ``subdivision`` levels as (positions [n, 3], triangles [m, 3]), wound so that cross(p1 - p0, p2 - p0)
+    points outwards: each level splits every triangle into four at its edges' midpoints, pushed onto the sphere."""
+    t = (1.0 + 5.0 ** 0.5) / 2.0
+    verts = [(-1, t, 0), (1, t, 0), (-1, -t, 0), (1, -t, 0), (0, -1, t), (0, 1, t), (0, -1, -t), (0, 1, -t),
+             (t, 0, -1), (t, 0, 1), (-t, 0, -1), (-t, 0, 1)]
+    verts = [tuple(np.array(v, np.float64) / np.linalg.norm(v)) for v in verts]
+    tris = [(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2), (10, 7, 6), (7, 1, 8),
+            (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11), (6, 2, 10), (8, 6, 7), (9, 8, 1)]
+    for _ in range(int(subdivision)):
+        mid = {}
+
+        def midpoint(a, b):
+            key = (min(a, b), max(a, b))
+            if key not in mid:
+                m = np.add(verts[a], verts[b])
+                verts.append(tuple(m / np.linalg.norm(m)))
+                mid[key] = len(verts) - 1
+            return mid[key]
+
+        new = []
+        for a, b, c in tris:
+            ab, bc, ca = midpoint(a, b), midpoint(b, c), midpoint(c, a)
+            new += [(a, ab, ca), (b, bc, ab), (c, ca, bc), (ab, bc, ca)]
+        tris = new
+    return np.array(verts, np.float64), np.array(tris, np.int64)
+
+
+def emissive_globe(resolution=(512, 512), spp=16, subdivision=5, transform="uniform", depth=10, rr_depth=0, rr_threshold=0.95,
+                   seed=19980810, output="emissive_globe.exr") -> str:
+    """The frame of the triangle-level light trees (option "light_tree_triangles"): ``near_light``'s Matte room lit only by a
+    one-sided emissive icosphere of radius 0.25 (``subdivision`` levels) whose lowest point hangs 0.15 above the desk top.  Seen
+    from the desk, most of the globe faces away: an emitter whose triangles are picked by area wastes most of its shadow rays.
+
+    ``transform`` places the globe: "uniform" (an SRT of uniform scale), "stretched" (a Matrix of non-uniform scale 0.3 / 0.2 /
+    0.25 under a rotation) or "mirrored" (a Matrix of negative determinant that mirrors x, applied to an icosphere wound inwards,
+    so that its world-space triangles face outwards as the others do)."""
+    out = []
+    shapes = _matte_room(out, "Light globe_light : Diffuse { emission : Constant { v { 9.0, 8.0, 6.5 } } two_sided { false } }")
+    desk_top, gap = 0.7, 0.15
+    if transform == "uniform":
+        r = 0.25
+        out.append(f"Shape globe_mesh : Sphere {{ subdivision {{ {int(subdivision)} }} }}")
+        place = f"transform : SRT {{ scale {{ {_fmt(r)} }} translate {{ 0.0, {_fmt(desk_top + gap + r)}, -0.4 }} }}"
+    elif transform in ("stretched", "mirrored"):
+        if transform == "stretched":
+            out.append(f"Shape globe_mesh : Sphere {{ subdivision {{ {int(subdivision)} }} }}")
+            a, b = np.radians(35.0), np.radians(20.0)
+            rz = np.array([[np.cos(a), -np.sin(a), 0.0], [np.sin(a), np.cos(a), 0.0], [0.0, 0.0, 1.0]])
+            ry = np.array([[np.cos(b), 0.0, np.sin(b)], [0.0, 1.0, 0.0], [-np.sin(b), 0.0, np.cos(b)]])
+            m = ry @ rz @ np.diag([0.3, 0.2, 0.25])
+        else:
+            v, f = _icosphere(subdivision)
+            pos = ", ".join(_fmt(c) for c in v.reshape(-1))
+            idx = ", ".join(str(int(i)) for i in f[:, ::-1].reshape(-1))  # wound inwards: the mirror turns them outwards
+            out.append(f"Shape globe_mesh : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} }}")
+            m = np.diag([-0.25, 0.25, 0.25])
+        low = np.linalg.norm(m[1])  # the lowest point of the ellipsoid lies |row y| below its centre
+        t = (0.0, desk_top + gap + low, -0.4)
+        rows = [list(m[i]) + [t[i]] for i in range(3)] + [[0.0, 0.0, 0.0, 1.0]]
+        place = "transform : Matrix { m { " + ", ".join(_fmt(x) for row in rows for x in row) + " } }"
+    else:
+        raise ValueError(f"transform is 'uniform', 'stretched' or 'mirrored', not {transform!r}")
+    out.append(f"Shape globe : Instance {{ shape {{ @globe_mesh }} light {{ @globe_light }} {place} }}")
+    shapes.append("@globe")
+    return _matte_room_render(out, shapes, _MATTE_ROOM_CAMERA, resolution, spp, depth, rr_depth, rr_threshold, seed, output)
 
 
 def textured_materials(resolution=(64, 40), spp=4, depth=6, rr_depth=0, rr_threshold=0.95, seed=19980810, assets="tests/golden/assets",
