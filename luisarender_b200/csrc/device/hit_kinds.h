@@ -39,8 +39,8 @@ LRK_HIT_KINDS_FN uint32_t hit_kind_of(const lrk_surface &s) {
 
 // Kinds whose shade kernel runs in IEEE arithmetic even without the option strict_math: the near-specular closures (Mirror, Glass,
 // Plastic, Metal and Mix of them), whose lobes amplify a 1e-6 error in the half vector into percents of the lobe value, and Layered
-// and thin Disney.
-LRK_HIT_KINDS_FN bool hit_kind_always_strict(uint32_t kind) { return (kind >= kHitMirror && kind <= kHitMix) || kind >= kHitLayered; }
+// and thin Disney.  constexpr: the fast variant of shade.cu does not compile these kinds' kernels.
+LRK_HIT_KINDS_FN constexpr bool hit_kind_always_strict(uint32_t kind) { return (kind >= kHitMirror && kind <= kHitMix) || kind >= kHitLayered; }
 
 // Calls f(std::integral_constant<uint32_t, kind>{}): the run-time kind as a compile-time one.  Host and device code call it with
 // their own kind of f.

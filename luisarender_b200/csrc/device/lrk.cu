@@ -733,7 +733,7 @@ int lrk_create(const lrk_device_cfg *cfg, lrk_ctx **out) {
     ctx->grid_trace = grid_for(reinterpret_cast<const void *>(trace_closest_kernel<false, false>), kTraceBlock);
     ctx->grid_shadow = grid_for(reinterpret_cast<const void *>(trace_shadow_kernel<false, false>), kTraceBlock);
     for (uint32_t kind = 0; kind < kHitKinds; kind++) {
-        ctx->grid_shade[0][kind] = fast::shade_grid(kind, ctx->sm_count);
+        if (!hit_kind_always_strict(kind)) ctx->grid_shade[0][kind] = fast::shade_grid(kind, ctx->sm_count);
         ctx->grid_shade[1][kind] = strict::shade_grid(kind, ctx->sm_count);
     }
     ctx->grid_classify = grid_for(reinterpret_cast<const void *>(classify_hits_kernel));

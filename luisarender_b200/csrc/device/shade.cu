@@ -23,6 +23,13 @@ namespace LRK_SHADE_VARIANT {
 
 namespace {
 
+// LRK_SHADE_VARIANT as a compile-time value
+#define LRK_SHADE_IS_FAST_fast true
+#define LRK_SHADE_IS_FAST_strict false
+#define LRK_SHADE_IS_FAST_OF(v) LRK_SHADE_IS_FAST_##v
+#define LRK_SHADE_IS_FAST(v) LRK_SHADE_IS_FAST_OF(v)
+constexpr bool kFastVariant = LRK_SHADE_IS_FAST(LRK_SHADE_VARIANT);
+
 template<typename Kernel>
 int grid_of(Kernel kernel, int block, int sm_count) {
     int per_sm = 0;
@@ -30,12 +37,15 @@ int grid_of(Kernel kernel, int block, int sm_count) {
     return (per_sm > 0 ? per_sm : 1) * sm_count;
 }
 
-// calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection, light point sampling)
+// calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection, light point sampling).  The fast
+// variant has none for the kinds that always run in strict arithmetic (hit_kind_always_strict): render_pass never launches them
+// there.
 template<uint32_t SEL, uint32_t PT, typename F>
 void with_shade_kernel(uint32_t kind, bool textured, F &&f) {
     with_hit_kind(kind, [&](auto k) {
         constexpr uint32_t K = decltype(k)::value;
-        textured ? f(shade_kernel<K, true, SEL, PT>) : f(shade_kernel<K, false, SEL, PT>);
+        if constexpr (!(kFastVariant && hit_kind_always_strict(K)))
+            textured ? f(shade_kernel<K, true, SEL, PT>) : f(shade_kernel<K, false, SEL, PT>);
     });
 }
 
