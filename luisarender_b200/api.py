@@ -102,12 +102,10 @@ class Renderer:
 
     def __init__(self, device_index: int = -1, max_paths_per_pass: int = 0, light_tree: bool = False, light_solid_angle: bool = False,
                  light_tree_triangles: bool = False):
-        if light_tree not in (0, 1):
-            raise ValueError(f"light_tree is False or True, not {light_tree!r}")
-        if light_solid_angle not in (0, 1):
-            raise ValueError(f"light_solid_angle is False or True, not {light_solid_angle!r}")
-        if light_tree_triangles not in (0, 1):
-            raise ValueError(f"light_tree_triangles is False or True, not {light_tree_triangles!r}")
+        light_options = {"light_tree": light_tree, "light_solid_angle": light_solid_angle, "light_tree_triangles": light_tree_triangles}
+        for name, value in light_options.items():
+            if value not in (0, 1):
+                raise ValueError(f"{name} is False or True, not {value!r}")
         if light_tree_triangles and not light_tree:
             raise ValueError("light_tree_triangles is the bottom level of the light tree: it needs light_tree=True")
         self._lib = F.device_lib()
@@ -117,12 +115,9 @@ class Renderer:
         if rc != 0:
             raise RuntimeError(f"lrk_create failed ({rc}): no usable CUDA device")
         self._res = None
-        if light_tree:
-            self.set_option("light_tree", 1)
-        if light_solid_angle:
-            self.set_option("light_solid_angle", 1)
-        if light_tree_triangles:
-            self.set_option("light_tree_triangles", 1)
+        for name, value in light_options.items():
+            if value:
+                self.set_option(name, 1)
 
     def _check(self, rc: int, what: str):
         if rc != 0:

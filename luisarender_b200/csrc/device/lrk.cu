@@ -142,16 +142,9 @@ struct lrk_ctx {
     bool gbuffer_option{false}, gbuffer_film{false};
     DeviceBuffer d_gb_albedo, d_gb_normal, d_gb_hits;// per pixel (sum albedo, S), (sum n, sum t), H
     DeviceBuffer d_dn_albedo_cov, d_dn_normal_depth, d_dn_variance, d_dn_ping[2];// lrk_denoise / lrk_download_gbuffer scratch
-    // light tree (option "light_tree"): the option's value at lrk_upload_scene is latched into light_tree, which selects the shade
-    // kernels' instantiations
-    bool light_tree_option{false}, light_tree{false};
-    DeviceLightTree light_tree_rec{};// the record after the scene's device copy (scene.cuh)
-    // triangle-level light trees (option "light_tree_triangles"): read at lrk_upload_scene, which then builds the bottom trees; the
-    // kernels find them through light_tree_rec.bottom_nodes
-    bool light_tree_triangles_option{false};
-    // solid-angle light sampling (option "light_solid_angle"): latched at lrk_upload_scene into light_solid_angle, which selects the
-    // shade kernels' instantiations
-    bool light_solid_angle_option{false}, light_solid_angle{false};
+    // next-event light sampling: light_requested holds the options "light_tree", "light_tree_triangles" and "light_solid_angle";
+    // lrk_upload_scene latches it into light_active, which selects the shade kernels' instantiations (upload_light_sampling)
+    LightSampling light_requested, light_active;
 
     ~lrk_ctx();
 };
@@ -407,8 +400,8 @@ int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset,
                 if (!(ctx->used_kinds & (1u << kind))) continue;
                 const bool strict = ctx->strict_math || hit_kind_always_strict(kind);
                 const int blocks = blocks_for(ctx, n, ctx->grid_shade[strict ? 1 : 0][kind]);
-                if (strict) strict::launch_shade(kind, ctx->textured, ctx->light_tree, ctx->light_solid_angle, blocks, ctx->stream, sc, pb, depth);
-                else fast::launch_shade(kind, ctx->textured, ctx->light_tree, ctx->light_solid_angle, blocks, ctx->stream, sc, pb, depth);
+                if (strict) strict::launch_shade(kind, ctx->textured, ctx->light_active, blocks, ctx->stream, sc, pb, depth);
+                else fast::launch_shade(kind, ctx->textured, ctx->light_active, blocks, ctx->stream, sc, pb, depth);
                 ctx->stats.kernel_launches++;
             }
         }
@@ -596,6 +589,22 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
     return LRK_OK;
 }
 
+// The triangles of `mesh`, 9 doubles each: in world space through the row-major 3x4 object-to-world matrix m, or in object space
+// when m is null.
+void gather_triangles(const lrk_scene_desc *s, const lrk_mesh &mesh, const float *m, std::vector<double> &tris) {
+    tris.clear();
+    for (uint32_t t = 0; t < mesh.triangle_count; t++) {
+        const lrk_triangle &tri = s->triangles[mesh.triangle_offset + t];
+        for (uint32_t v : {tri.i0, tri.i1, tri.i2}) {
+            const float *p = s->vertices[mesh.vertex_offset + v].p;
+            for (int r = 0; r < 3; r++)
+                tris.push_back(m == nullptr ? static_cast<double>(p[r])
+                                            : static_cast<double>(m[4 * r]) * p[0] + static_cast<double>(m[4 * r + 1]) * p[1] +
+                                                  static_cast<double>(m[4 * r + 2]) * p[2] + m[4 * r + 3]);
+        }
+    }
+}
+
 // The light tree of the option "light_tree" (light_tree.h) over every instance that carries a light - not only the first light_count
 // handles - from the scene's own arrays: world-space triangles, the emission (the mean of max(texel, 0) of an image emission) and the
 // sidedness.  tree_inst: per tree light its instance; inst_light: per instance its tree light, kLightTreeNone for instances without
@@ -621,18 +630,7 @@ int build_light_tree(lrk_ctx *ctx, const lrk_scene_desc *s, LightTreeBuild &tree
         }
         for (double &c : rgb) c = std::max(c, 0.0);
         const double lum = 0.2126 * rgb[0] + 0.7152 * rgb[1] + 0.0722 * rgb[2];
-        const lrk_mesh &mesh = s->meshes[inst.mesh];
-        const float *m = inst.object_to_world;// row-major 3x4
-        tris.clear();
-        for (uint32_t t = 0; t < mesh.triangle_count; t++) {
-            const lrk_triangle &tri = s->triangles[mesh.triangle_offset + t];
-            for (uint32_t v : {tri.i0, tri.i1, tri.i2}) {
-                const lrk_vertex &vx = s->vertices[mesh.vertex_offset + v];
-                for (int r = 0; r < 3; r++)
-                    tris.push_back(static_cast<double>(m[4 * r]) * vx.p[0] + static_cast<double>(m[4 * r + 1]) * vx.p[1] +
-                                   static_cast<double>(m[4 * r + 2]) * vx.p[2] + m[4 * r + 3]);
-            }
-        }
+        gather_triangles(s, s->meshes[inst.mesh], inst.object_to_world, tris);
         inst_light[i] = static_cast<uint32_t>(emitters.size());
         tree_inst.push_back(i);
         emitters.push_back(light_tree_emitter(tris, lum * light.scale, light.two_sided != 0u));
@@ -662,13 +660,7 @@ void build_bottom_light_trees(const lrk_scene_desc *s, const std::vector<uint32_
         const LightTreeSide side = s->lights[inst.handle[1] & 4095u].two_sided ? kLightTreeTwoSided : det < 0.0 ? kLightTreeMirrored : kLightTreeOneSided;
         auto it = built.find({inst.mesh, side});
         if (it == built.end()) {
-            const lrk_mesh &mesh = s->meshes[inst.mesh];
-            tris.clear();
-            for (uint32_t t = 0; t < mesh.triangle_count; t++) {
-                const lrk_triangle &tri = s->triangles[mesh.triangle_offset + t];
-                for (uint32_t v : {tri.i0, tri.i1, tri.i2})
-                    for (int c = 0; c < 3; c++) tris.push_back(s->vertices[mesh.vertex_offset + v].p[c]);
-            }
+            gather_triangles(s, s->meshes[inst.mesh], nullptr, tris);
             const LightTreeBuild b = light_tree_build_triangles(tris, side);
             const uint32_t root = b.nodes.empty() ? kLightTreeNone : static_cast<uint32_t>(nodes.size());
             it = built.emplace(std::make_pair(inst.mesh, static_cast<uint32_t>(side)), std::make_pair(root, static_cast<uint32_t>(trail.size()))).first;
@@ -678,6 +670,71 @@ void build_bottom_light_trees(const lrk_scene_desc *s, const std::vector<uint32_
         inst_bottom[2u * i] = it->second.first;
         inst_bottom[2u * i + 1u] = it->second.second;
     }
+}
+
+// The field of LightSampling the option `name` sets, or null for another option
+bool LightSampling::*light_sampling_option(const std::string &name) {
+    if (name == "light_tree") return &LightSampling::tree;
+    if (name == "light_tree_triangles") return &LightSampling::triangles;
+    if (name == "light_solid_angle") return &LightSampling::solid_angle;
+    return nullptr;
+}
+
+// lrk_upload_scene's refusals of the requested light sampling
+int check_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
+    const LightSampling &want = ctx->light_requested;
+    const bool volume = s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH;
+    if (want.tree && volume)
+        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: the light tree (option light_tree) serves the surface integrator only; the volume "
+                                              "integrator selects its lights uniformly");
+    if (want.triangles && !want.tree)
+        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: the triangle-level light trees (option light_tree_triangles) are the bottom "
+                                                   "level of the light tree: set the option light_tree too");
+    if (want.solid_angle && volume)
+        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: solid-angle light sampling (option light_solid_angle) serves the surface integrator "
+                                              "only; the volume integrator evaluates its light pdfs from the world origin");
+    return LRK_OK;
+}
+
+// lrk_upload_scene's part for the requested light sampling, once the scene record is in a.scene_copy: builds and uploads the light
+// tree and its bottom trees where requested, writes the record the kernels find them through (scene.cuh: null arrays for what is
+// off) after the scene record, and latches the request into ctx->light_active.
+int upload_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
+    const LightSampling want = ctx->light_requested;
+    auto &a = ctx->arrays;
+    int rc;
+    DeviceLightTree rec{};
+    LightTreeBuild tree;
+    std::vector<uint32_t> tree_inst, inst_light;
+    if (want.tree) {
+        if ((rc = build_light_tree(ctx, s, tree, tree_inst, inst_light))) return rc;
+        if ((rc = upload(ctx, a.lt_nodes, tree.nodes.data(), tree.nodes.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_light_inst, tree_inst.data(), tree_inst.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_trail, tree.trail.data(), tree.trail.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_inst_light, inst_light.data(), inst_light.size()))) return rc;
+        rec.nodes = tree.nodes.empty() ? nullptr : a.lt_nodes.get<const LightTreeNode>();
+        rec.light_inst = a.lt_light_inst.get<const uint32_t>();
+        rec.trail = a.lt_trail.get<const unsigned long long>();
+        rec.inst_light = a.lt_inst_light.get<const uint32_t>();
+    }
+    std::vector<LightTreeNode> bottom_nodes;
+    std::vector<uint32_t> inst_bottom;
+    std::vector<unsigned long long> bottom_trail;
+    if (want.triangles) {
+        build_bottom_light_trees(s, inst_light, bottom_nodes, inst_bottom, bottom_trail);
+        if ((rc = upload(ctx, a.lt_bottom_nodes, bottom_nodes.data(), bottom_nodes.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_inst_bottom, inst_bottom.data(), inst_bottom.size()))) return rc;
+        if ((rc = upload(ctx, a.lt_bottom_trail, bottom_trail.data(), bottom_trail.size()))) return rc;
+        if (!bottom_nodes.empty()) {
+            rec.bottom_nodes = a.lt_bottom_nodes.get<const LightTreeNode>();
+            rec.inst_bottom = a.lt_inst_bottom.get<const uint2>();
+            rec.bottom_trail = a.lt_bottom_trail.get<const unsigned long long>();
+        }
+    }
+    LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get<char>() + sizeof(DeviceScene), &rec, sizeof(DeviceLightTree), cudaMemcpyHostToDevice, ctx->stream));
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));// the host arrays and `rec` are locals
+    ctx->light_active = want;
+    return LRK_OK;
 }
 
 }// namespace
@@ -794,15 +851,7 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: an environment medium needs the volume path integrator (MegaVPTNaive)");
     }
     if (s->integrator.max_depth > kMaxDepthSlots - 1u) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: max depth > 63");
-    if (ctx->light_tree_option && s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: the light tree (option light_tree) serves the surface integrator only; the volume "
-                                              "integrator selects its lights uniformly");
-    if (ctx->light_tree_triangles_option && !ctx->light_tree_option)
-        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: the triangle-level light trees (option light_tree_triangles) are the bottom "
-                                                   "level of the light tree: set the option light_tree too");
-    if (ctx->light_solid_angle_option && s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: solid-angle light sampling (option light_solid_angle) serves the surface integrator "
-                                              "only; the volume integrator evaluates its light pdfs from the world origin");
+    if (const int rc = check_light_sampling(ctx, s)) return rc;
     if (s->camera.resolution[0] > 65535u || s->camera.resolution[1] > 65535u)
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: film larger than 65535 pixels per side");
     if (s->light_count == 0u && !s->environment.present)// !pipeline().has_lighting(), wave_path.cpp:224-228
@@ -956,24 +1005,6 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     }
     for (uint32_t i = 0; i < s->instance_count; i++) std::memcpy(&xform[i * 16u + 12u], &mesh_root[s->instances[i].mesh], 4);
     if ((rc = upload(ctx, a.inst_xform, xform.data(), xform.size()))) return rc;
-    LightTreeBuild tree;
-    std::vector<uint32_t> tree_inst, inst_light;
-    if (ctx->light_tree_option) {
-        if ((rc = build_light_tree(ctx, s, tree, tree_inst, inst_light))) return rc;
-        if ((rc = upload(ctx, a.lt_nodes, tree.nodes.data(), tree.nodes.size()))) return rc;
-        if ((rc = upload(ctx, a.lt_light_inst, tree_inst.data(), tree_inst.size()))) return rc;
-        if ((rc = upload(ctx, a.lt_trail, tree.trail.data(), tree.trail.size()))) return rc;
-        if ((rc = upload(ctx, a.lt_inst_light, inst_light.data(), inst_light.size()))) return rc;
-    }
-    std::vector<LightTreeNode> bottom_nodes;
-    std::vector<uint32_t> inst_bottom;
-    std::vector<unsigned long long> bottom_trail;
-    if (ctx->light_tree_triangles_option) {
-        build_bottom_light_trees(s, inst_light, bottom_nodes, inst_bottom, bottom_trail);
-        if ((rc = upload(ctx, a.lt_bottom_nodes, bottom_nodes.data(), bottom_nodes.size()))) return rc;
-        if ((rc = upload(ctx, a.lt_inst_bottom, inst_bottom.data(), inst_bottom.size()))) return rc;
-        if ((rc = upload(ctx, a.lt_bottom_trail, bottom_trail.data(), bottom_trail.size()))) return rc;
-    }
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
 
     auto &sc = ctx->scene;
@@ -1046,19 +1077,6 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     sc.media = a.media.get<const lrk_medium>();
     sc.medium_count = s->medium_count;
     sc.env_medium_tag = s->environment_medium_tag;
-    ctx->light_tree = ctx->light_tree_option;
-    ctx->light_solid_angle = ctx->light_solid_angle_option;
-    {
-        auto &lt = ctx->light_tree_rec;
-        lt.nodes = ctx->light_tree && !tree.nodes.empty() ? a.lt_nodes.get<const LightTreeNode>() : nullptr;
-        lt.light_inst = ctx->light_tree ? a.lt_light_inst.get<const uint32_t>() : nullptr;
-        lt.trail = ctx->light_tree ? a.lt_trail.get<const unsigned long long>() : nullptr;
-        lt.inst_light = ctx->light_tree ? a.lt_inst_light.get<const uint32_t>() : nullptr;
-        const bool bottom = ctx->light_tree_triangles_option && !bottom_nodes.empty();
-        lt.bottom_nodes = bottom ? a.lt_bottom_nodes.get<const LightTreeNode>() : nullptr;
-        lt.inst_bottom = bottom ? a.lt_inst_bottom.get<const uint2>() : nullptr;
-        lt.bottom_trail = bottom ? a.lt_bottom_trail.get<const unsigned long long>() : nullptr;
-    }
 
     const size_t npix = static_cast<size_t>(sc.width) * sc.height;
     ctx->film_pixels = 0;
@@ -1069,9 +1087,7 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         LRK_CUDA(a.scene_copy.reserve(sizeof(DeviceScene) + sizeof(DeviceLightTree)));
         sc.self = a.scene_copy.get<const DeviceScene>();
         LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get(), &sc, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
-        LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get<char>() + sizeof(DeviceScene), &ctx->light_tree_rec, sizeof(DeviceLightTree), cudaMemcpyHostToDevice,
-                                 ctx->stream));
-        LRK_CUDA(cudaStreamSynchronize(ctx->stream));
+        if ((rc = upload_light_sampling(ctx, s))) return rc;
     }
     ctx->has_scene = true;
     // a balanced assignment stays a valid partition for any scene of the same film size (a frame loop re-uploads per frame and
@@ -1152,17 +1168,9 @@ int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value) {
     else if (n == "device_bvh") ctx->device_bvh = value != 0;
     else if (n == "strict_math") ctx->strict_math = value != 0;
     else if (n == "gbuffer") ctx->gbuffer_option = value != 0;// takes effect at the next film clear
-    else if (n == "light_tree") {// takes effect at the next lrk_upload_scene
-        if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_tree is 0 or 1");
-        ctx->light_tree_option = value != 0;
-    }
-    else if (n == "light_tree_triangles") {// takes effect at the next lrk_upload_scene
-        if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_tree_triangles is 0 or 1");
-        ctx->light_tree_triangles_option = value != 0;
-    }
-    else if (n == "light_solid_angle") {// takes effect at the next lrk_upload_scene
-        if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_solid_angle is 0 or 1");
-        ctx->light_solid_angle_option = value != 0;
+    else if (bool LightSampling::*field = light_sampling_option(n)) {// takes effect at the next lrk_upload_scene
+        if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: " + n + " is 0 or 1");
+        ctx->light_requested.*field = value != 0;
     }
     else if (n == "pin_host_buffers") {
         ctx->pin_host = value != 0;

@@ -74,14 +74,16 @@ int volume_surface_grid(uint32_t kind, int sm_count) {
     return g;
 }
 
-void launch_shade(uint32_t kind, bool textured, bool light_tree, bool solid_angle, int blocks, cudaStream_t stream, const DeviceScene &sc,
+// the light sampling as the kernels' <SEL, PT>; the triangle-level trees need no instantiation of their own: the kernels find them
+// through light_tree_of(sc).bottom_nodes
+void launch_shade(uint32_t kind, bool textured, const LightSampling &light, int blocks, cudaStream_t stream, const DeviceScene &sc,
                   const PathBuffers &pb, uint32_t depth) {
     const auto launch = [&](auto kernel) { kernel<<<blocks, kShadeBlock, 0, stream>>>(sc, pb, depth); };
-    if (solid_angle) {
-        if (light_tree) with_shade_kernel<kLightSelectTree, kLightPointSolidAngle>(kind, textured, launch);
+    if (light.solid_angle) {
+        if (light.tree) with_shade_kernel<kLightSelectTree, kLightPointSolidAngle>(kind, textured, launch);
         else with_shade_kernel<kLightSelectUniform, kLightPointSolidAngle>(kind, textured, launch);
     } else {
-        if (light_tree) with_shade_kernel<kLightSelectTree, kLightPointArea>(kind, textured, launch);
+        if (light.tree) with_shade_kernel<kLightSelectTree, kLightPointArea>(kind, textured, launch);
         else with_shade_kernel<kLightSelectUniform, kLightPointArea>(kind, textured, launch);
     }
 }

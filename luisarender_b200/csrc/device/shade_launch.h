@@ -8,6 +8,12 @@
 
 namespace lrk {
 
+// How next-event estimation picks a light and a point on it: the options "light_tree", "light_tree_triangles" (the light tree's
+// bottom level: set with tree only) and "light_solid_angle".  Not part of the ABI.
+struct LightSampling {
+    bool tree{false}, triangles{false}, solid_angle{false};
+};
+
 #define LRK_DECLARE_SHADE_VARIANT(NS)                                                                                                        \
     namespace NS {                                                                                                                           \
     /* blocks of one persistent grid (occupancy x SM count): surface shade kernel of hit bucket `kind` (0 .. kHitKinds - 1), the     */      \
@@ -15,10 +21,8 @@ namespace lrk {
     int shade_grid(uint32_t kind, int sm_count);                                                                                             \
     int volume_medium_grid(int sm_count);                                                                                                    \
     int volume_surface_grid(uint32_t kind, int sm_count);                                                                                    \
-    /* `textured`: the instantiation that evaluates image-textured parameters / normal maps; `light_tree`: the one whose next-event */      \
-    /* estimation selects lights with the light tree (option "light_tree"); `solid_angle`: the one that samples the light's point */        \
-    /* in solid angle (option "light_solid_angle") */                                                                                      \
-    void launch_shade(uint32_t kind, bool textured, bool light_tree, bool solid_angle, int blocks, cudaStream_t stream, const DeviceScene &sc,  \
+    /* `textured`: the instantiation that evaluates image-textured parameters / normal maps; `light`: the one of that light sampling */   \
+    void launch_shade(uint32_t kind, bool textured, const LightSampling &light, int blocks, cudaStream_t stream, const DeviceScene &sc,       \
                       const PathBuffers &pb, uint32_t depth);                                                                                \
     void launch_volume_medium(int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth);                \
     void launch_volume_surface(uint32_t kind, bool textured, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb,  \

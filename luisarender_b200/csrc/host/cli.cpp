@@ -42,6 +42,17 @@
 
 namespace {
 
+// the light-sampling flags: the options each sets to 1 before the upload
+struct LightFlag {
+    const char *flag, *help;
+    std::vector<const char *> options;
+};
+const LightFlag kLightFlags[] = {
+    {"--light-tree", "Pick next-event lights from a light tree (power, distance, orientation)", {"light_tree"}},
+    {"--light-solid-angle", "Sample next-event light points uniformly in solid angle, not by area", {"light_solid_angle"}},
+    {"--light-tree-triangles", "Also pick the emissive triangle from the light tree (implies --light-tree)", {"light_tree", "light_tree_triangles"}},
+};
+
 void usage() {
     std::printf("Usage:\n  luisa-render-cli [OPTION...] <file>\n\n"
                 "  -b, --backend <backend>      Compute backend name (cuda)\n"
@@ -51,11 +62,9 @@ void usage() {
                 "      --gpus <n>               Render on n GPUs, one process each (tiles sharded, films summed on GPU 0)\n"
                 "      --adaptive <threshold>   Adaptive sampling: stop 8x4 pixel blocks whose relative error is below threshold\n"
                 "      --adaptive-min-spp <n>   Samples per pixel of the first adaptive round (default 16, at most the camera's spp)\n"
-                "      --denoise                Also write the denoised image to <stem>.denoised<ext> (one GPU only)\n"
-                "      --light-tree             Pick next-event lights from a light tree (power, distance, orientation)\n"
-                "      --light-solid-angle      Sample next-event light points uniformly in solid angle, not by area\n"
-                "      --light-tree-triangles   Also pick the emissive triangle from the light tree (implies --light-tree)\n"
-                "  -h, --help                   Display this help message\n");
+                "      --denoise                Also write the denoised image to <stem>.denoised<ext> (one GPU only)\n");
+    for (const LightFlag &l : kLightFlags) std::printf("      %-25s%s\n", l.flag, l.help);
+    std::printf("  -h, --help                   Display this help message\n");
 }
 
 [[noreturn]] void die(const std::string &msg) {
@@ -151,7 +160,8 @@ std::string denoised_path(const std::string &file) {
 int main(int argc, char *argv[]) {
     std::string backend, scene_path;
     int device = -1, gpus = 1;
-    bool denoise = false, light_tree = false, light_solid_angle = false, light_tree_triangles = false;
+    bool denoise = false;
+    std::vector<const char *> light_options;
     std::string adaptive_arg, min_spp_arg;
     std::vector<std::string> keys, values;
     auto add_macro = [&](const std::string &d) {
@@ -194,9 +204,9 @@ int main(int argc, char *argv[]) {
         else if (a == "--adaptive-min-spp") min_spp_arg = need("count");
         else if (a.rfind("--adaptive-min-spp=", 0) == 0) min_spp_arg = a.substr(19);
         else if (a == "--denoise") denoise = true;
-        else if (a == "--light-tree") light_tree = true;
-        else if (a == "--light-solid-angle") light_solid_angle = true;
-        else if (a == "--light-tree-triangles") light_tree = light_tree_triangles = true;
+        else if (auto l = std::find_if(std::begin(kLightFlags), std::end(kLightFlags), [&](const LightFlag &f) { return a == f.flag; });
+                 l != std::end(kLightFlags))
+            light_options.insert(light_options.end(), l->options.begin(), l->options.end());
         else if (a == "-D" || a == "--define") add_macro(need("definition"));
         else if (a.rfind("-D", 0) == 0) add_macro(a.substr(2));
         else if (!a.empty() && a[0] == '-') std::fprintf(stderr, "[warning] Unrecognized options: %s\n", a.c_str());
@@ -268,9 +278,8 @@ int main(int argc, char *argv[]) {
     lrk_ctx *ctx = nullptr;
     if (int rc = lrk_create(&cfg, &ctx); rc != 0) die("Failed to create the CUDA device context (lrk_create = " + std::to_string(rc) + ").");
     if (denoise && lrk_set_option(ctx, "gbuffer", 1) != 0) die(lrk_last_error(ctx));
-    if (light_tree && lrk_set_option(ctx, "light_tree", 1) != 0) die(lrk_last_error(ctx));
-    if (light_solid_angle && lrk_set_option(ctx, "light_solid_angle", 1) != 0) die(lrk_last_error(ctx));
-    if (light_tree_triangles && lrk_set_option(ctx, "light_tree_triangles", 1) != 0) die(lrk_last_error(ctx));
+    for (const char *option : light_options)
+        if (lrk_set_option(ctx, option, 1) != 0) die(lrk_last_error(ctx));
     if (world > 1u) {
         uint8_t id[LRK_COMM_ID_BYTES];
         exchange_comm_id(rank, id);

@@ -9,20 +9,15 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+import host_harness
 from luisarender_b200 import _ffi as F
 
 REPO = Path(__file__).resolve().parents[1]
-SRC = REPO / "tests" / "host_device" / "adaptive_host.cpp"
-OUT = REPO / "tests" / "host_device" / "_build" / "libadaptive_host.so"
-HEADER = REPO / "luisarender_b200" / "csrc" / "device" / "adaptive.h"
 
 
 @pytest.fixture(scope="module")
 def lib():
-    if not OUT.exists() or OUT.stat().st_mtime < max(SRC.stat().st_mtime, HEADER.stat().st_mtime):
-        OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-ffp-contract=off", "-shared", str(SRC), "-o", str(OUT)], check=True)
-    handle = C.CDLL(str(OUT))
+    handle = host_harness.load("adaptive_host", [host_harness.DEVICE / "adaptive.h"], ["-O2", "-ffp-contract=off"])
     handle.adaptive_error_host.argtypes = [C.c_void_p] * 5 + [C.c_int64]
     return handle
 

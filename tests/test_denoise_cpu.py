@@ -10,22 +10,17 @@ import numpy as np
 import pytest
 
 import denoise_ref as R
+import host_harness
 from luisarender_b200 import _ffi as F
 
 REPO = Path(__file__).resolve().parents[1]
-SRC = REPO / "tests" / "host_device" / "denoise_host.cpp"
-OUT = REPO / "tests" / "host_device" / "_build" / "libdenoise_host.so"
-HEADERS = [REPO / "luisarender_b200" / "csrc" / "device" / h for h in ("denoise.h", "adaptive.h")]
 f32 = np.float32
 W, H = 64, 48
 
 
 @pytest.fixture(scope="module")
 def lib():
-    if not OUT.exists() or OUT.stat().st_mtime < max(p.stat().st_mtime for p in [SRC, *HEADERS]):
-        OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-ffp-contract=off", "-shared", str(SRC), "-o", str(OUT)], check=True)
-    handle = C.CDLL(str(OUT))
+    handle = host_harness.load("denoise_host", [host_harness.DEVICE / h for h in ("denoise.h", "adaptive.h")], ["-O2", "-ffp-contract=off"])
     handle.denoise_guides_host.argtypes = [C.c_int64] + [C.c_void_p] * 5
     handle.denoise_normal_weight_host.argtypes = [C.c_int64] + [C.c_void_p] * 5
     handle.denoise_host.argtypes = [C.c_int, C.c_int] + [C.c_void_p] * 5

@@ -10,33 +10,25 @@ is CUDA's libm and code generation.  No GPU, no /root/reference needed.
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 import sys
 from pathlib import Path
 
 import numpy as np
 import pytest
 
+import host_harness
+
 REPO = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(REPO / "tools"))
 import gen_ref_pins as G  # noqa: E402
 
-SRC = REPO / "tests" / "host_device" / "closures_host.cpp"
-OUT = REPO / "tests" / "host_device" / "_build" / "libclosures_host.so"
 CLOSURE_PINS = sorted(n for n in G.PINS if n.split("_")[0] in ("matte", "disney", "disneytrans", "disneythin", "mirror", "glass", "plastic", "metal"))
 
 
 @pytest.fixture(scope="module")
 def lib():
-    cuda_include = Path("/usr/local/cuda/include")
-    if not (cuda_include / "cuda_runtime.h").exists():
-        pytest.skip("CUDA headers not found")
-    deps = [SRC, REPO / "luisarender_b200" / "csrc" / "device" / "shading.cuh", REPO / "luisarender_b200" / "csrc" / "device" / "vecmath.cuh"]
-    if not OUT.exists() or OUT.stat().st_mtime < max(d.stat().st_mtime for d in deps):
-        OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O1", "-fPIC", "-w", "-ffp-contract=off", f"-I{cuda_include}", "-shared", "-Wl,-Bsymbolic", str(SRC), "-o", str(OUT)],
-                       check=True)
-    handle = C.CDLL(str(OUT))
+    handle = host_harness.load("closures_host", [host_harness.DEVICE / "shading.cuh", host_harness.DEVICE / "vecmath.cuh"],
+                               ["-O1", "-w", "-ffp-contract=off", host_harness.cuda_include_flag(), "-Wl,-Bsymbolic"])
     handle.device_closure_unit.argtypes = [C.c_char_p, C.c_void_p, C.c_void_p, C.c_int]
     return handle
 

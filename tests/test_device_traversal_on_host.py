@@ -10,33 +10,24 @@ same number of nodes; what is left for the GPU tests is the warp scheduling arou
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
 import pytest
 
+import host_harness
 from luisarender_b200 import scenes
 from luisarender_b200.api import Scene
 from oracle import binding as O
 
 REPO = Path(__file__).resolve().parent.parent
-SRC = REPO / "tests" / "host_device" / "traverse_host.cpp"
-OUT = REPO / "tests" / "host_device" / "_build" / "libtraverse_host.so"
-DEV = REPO / "luisarender_b200" / "csrc" / "device"
+DEV = host_harness.DEVICE
 
 
 @pytest.fixture(scope="module")
 def lib():
-    cuda_include = Path("/usr/local/cuda/include")
-    if not (cuda_include / "cuda_runtime.h").exists():
-        pytest.skip("CUDA headers not found")
-    deps = [SRC, DEV / "traverse.cuh", DEV / "scene.cuh", DEV / "vecmath.cuh", DEV / "shading.cuh", REPO / "include" / "lrk.h"]
-    if not OUT.exists() or OUT.stat().st_mtime < max(d.stat().st_mtime for d in deps):
-        OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off", f"-I{cuda_include}", "-shared", "-Wl,-Bsymbolic", str(SRC), "-o", str(OUT)],
-                       check=True)
-    handle = C.CDLL(str(OUT))
+    deps = [DEV / "traverse.cuh", DEV / "scene.cuh", DEV / "vecmath.cuh", DEV / "shading.cuh", REPO / "include" / "lrk.h"]
+    handle = host_harness.load("traverse_host", deps, ["-O2", "-w", "-ffp-contract=off", host_harness.cuda_include_flag(), "-Wl,-Bsymbolic"])
     handle.wide_trace_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p]
     return handle
 

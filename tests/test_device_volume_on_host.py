@@ -10,32 +10,23 @@ to the unmodified reference renderer on these scenes (tests/test_ref_render.py: 
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
 import pytest
 
+import host_harness
 from luisarender_b200 import scenes
 from luisarender_b200.api import Scene
 from oracle import binding as O
 
 REPO = Path(__file__).resolve().parent.parent
-SRC = REPO / "tests" / "host_device" / "volume_host.cpp"
-OUT = REPO / "tests" / "host_device" / "_build" / "libvolume_host.so"
 
 
 @pytest.fixture(scope="module")
 def lib():
-    cuda_include = Path("/usr/local/cuda/include")
-    if not (cuda_include / "cuda_runtime.h").exists():
-        pytest.skip("CUDA headers not found")
-    deps = [SRC] + sorted((REPO / "luisarender_b200" / "csrc" / "device").glob("*.cuh")) + [REPO / "include" / "lrk.h"]
-    if not OUT.exists() or OUT.stat().st_mtime < max(d.stat().st_mtime for d in deps):
-        OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O1", "-fPIC", "-w", "-ffp-contract=off", f"-I{cuda_include}", "-shared", "-Wl,-Bsymbolic",
-                        str(SRC), "-o", str(OUT)], check=True)
-    handle = C.CDLL(str(OUT))
+    deps = sorted(host_harness.DEVICE.glob("*.cuh")) + [REPO / "include" / "lrk.h"]
+    handle = host_harness.load("volume_host", deps, ["-O1", "-w", "-ffp-contract=off", host_harness.cuda_include_flag(), "-Wl,-Bsymbolic"])
     handle.volume_general_host.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]
     return handle
 

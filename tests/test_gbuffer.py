@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 import denoise_ref as R
+from light_sampling_checks import bits
 
 REPO = Path(__file__).resolve().parents[1]
 pytestmark = pytest.mark.gpu
@@ -76,10 +77,6 @@ def render_gbuffer(r, desc, spp_end, spp_begin=0):
     r.upload(desc)  # the upload clears the film: the option decides that it is a G-buffer film
     r.render(spp_begin, spp_end)
     return r.gbuffer()
-
-
-def bits(a):
-    return np.ascontiguousarray(a).view(np.uint32)
 
 
 # ---- 1. the mode changes no film bit ---------------------------------------------------------------------------------------------

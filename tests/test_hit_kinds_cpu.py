@@ -4,31 +4,24 @@ the reference-render scenes, and the set of kinds that always run in IEEE arithm
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
 import pytest
 
+import host_harness
 from luisarender_b200 import _ffi as F
 from luisarender_b200 import scenes
 from luisarender_b200.api import Scene
 
 REPO = Path(__file__).resolve().parents[1]
-SRC = REPO / "tests" / "host_device" / "hit_kinds_host.cpp"
-OUT = REPO / "tests" / "host_device" / "_build" / "libhit_kinds_host.so"
-DEPS = [SRC, REPO / "luisarender_b200" / "csrc" / "device" / "hit_kinds.h", REPO / "include" / "lrk.h"]
-
 SURFACE_DISNEY, SURFACE_LAYERED = 1, 7
 SURFACE_DISNEY_TRANSMISSIVE, SURFACE_DISNEY_THIN = 16, 64
 
 
 @pytest.fixture(scope="module")
 def lib():
-    if not OUT.exists() or OUT.stat().st_mtime < max(p.stat().st_mtime for p in DEPS):
-        OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-shared", str(SRC), "-o", str(OUT)], check=True)
-    h = C.CDLL(str(OUT))
+    h = host_harness.load("hit_kinds_host", [host_harness.DEVICE / "hit_kinds.h", REPO / "include" / "lrk.h"], ["-O2"])
     h.hit_kinds_of_surfaces.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
     h.hit_kinds_always_strict_mask.restype = C.c_uint32
     h.hit_kinds_count.restype = C.c_uint32

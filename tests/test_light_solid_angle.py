@@ -11,9 +11,12 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from light_sampling_checks import (SUB_SPP, SUBRENDERS, Z_MAX, bits, block_means, r, reference, rel_mse, render,  # noqa: F401
+                                   sub_renders, z_scores)
+
 REPO = Path(__file__).resolve().parents[1]
 pytestmark = pytest.mark.gpu
-BLOCK = 16
+AREA, SOLID_ANGLE = {"light_solid_angle": 0}, {"light_solid_angle": 1}
 
 
 def _scene(src):
@@ -79,54 +82,6 @@ def medium_small():
                                            small_count=12))
 
 
-@pytest.fixture
-def r(gpu_renderer):
-    """gpu_renderer, with the options this file touches back at their defaults afterwards (the renderer is shared by the session)."""
-    yield gpu_renderer
-    for name, value in (("light_solid_angle", 0), ("light_tree", 0), ("gbuffer", 0), ("max_paths_per_pass", 136 << 20)):
-        gpu_renderer.set_option(name, value)
-    gpu_renderer.set_shard(0, 1, 32)
-
-
-def render(r, desc, spp_begin, spp_end, solid_angle, raw=True):
-    r.set_option("light_solid_angle", int(solid_angle))
-    r.upload(desc)
-    r.render(spp_begin, spp_end)
-    return r.film(raw=raw).copy()
-
-
-def bits(a):
-    return np.ascontiguousarray(a).view(np.uint32)
-
-
-def sub_renders(r, desc, solid_angle, first, count, spp):
-    """`count` independent renders of `spp` samples each from sample index `first` on, as normalised films [count, H, W, 3]."""
-    return np.stack([render(r, desc, first + k * spp, first + (k + 1) * spp, solid_angle, raw=False)[..., :3]
-                     for k in range(count)]).astype(np.float64)
-
-
-def block_means(films):
-    n, h, w, _ = films.shape
-    hb, wb = h // BLOCK, w // BLOCK
-    b = films[:, :hb * BLOCK, :wb * BLOCK].reshape(n, hb, BLOCK, wb, BLOCK, 3).mean(axis=(2, 4, 5)).reshape(n, -1)
-    return np.concatenate([films.mean(axis=(1, 2, 3))[:, None], b], axis=1)  # column 0: the whole image
-
-
-def z_scores(a, b):
-    """(mean a - mean b) / its standard error, per block, from the spread of the independent sub-renders.  A block without noise in
-    either (the black background) gives 0 if the means agree, else inf."""
-    ma, mb = block_means(a), block_means(b)
-    se = np.sqrt(ma.var(axis=0, ddof=1) / len(ma) + mb.var(axis=0, ddof=1) / len(mb))
-    diff = ma.mean(axis=0) - mb.mean(axis=0)
-    return np.where(se > 0, diff / np.where(se > 0, se, 1.0), np.where(diff == 0, 0.0, np.inf))
-
-
-# As in test_light_tree.py: 1 + (16 x 16 blocks) means of 32 + 32 sub-renders compared at 4 sigma; with sigma estimated from the
-# sub-renders (t, 62 dof) each comparison fails by chance with probability 1.7e-4.  The renders are seeded: a frame passes or fails
-# for good.
-SUBRENDERS, SUB_SPP, Z_MAX = 32, 16, 4.0
-
-
 # ---- 1. off changes nothing -------------------------------------------------------------------------------------------------------
 def test_option_off_equals_a_context_that_never_set_it(cornell, r):
     from luisarender_b200.api import Renderer
@@ -139,8 +94,8 @@ def test_option_off_equals_a_context_that_never_set_it(cornell, r):
         want, want_launches = fresh.film(raw=True), fresh.stats()["kernel_launches"]
     finally:
         fresh.close()
-    render(r, cornell.desc(), 0, 4, solid_angle=True)  # leaves the option's kernels behind in this context
-    got = render(r, cornell.desc(), 0, 4, solid_angle=False)
+    render(r, cornell.desc(), 0, 4, SOLID_ANGLE)  # leaves the option's kernels behind in this context
+    got = render(r, cornell.desc(), 0, 4, AREA)
     assert np.array_equal(bits(got), bits(want))
     assert r.stats()["kernel_launches"] == want_launches
 
@@ -151,8 +106,8 @@ def test_solid_angle_agrees_with_area_sampling(request, name, r):
     d = request.getfixturevalue(name).desc()
     if name == "many":
         r.set_option("light_tree", 1)  # both choices of next-event estimation at once
-    area = sub_renders(r, d, False, 0, SUBRENDERS, SUB_SPP)
-    solid = sub_renders(r, d, True, SUBRENDERS * SUB_SPP, SUBRENDERS, SUB_SPP)  # disjoint sample indices
+    area = sub_renders(r, d, AREA, 0, SUBRENDERS, SUB_SPP)
+    solid = sub_renders(r, d, SOLID_ANGLE, SUBRENDERS * SUB_SPP, SUBRENDERS, SUB_SPP)  # disjoint sample indices
     assert not np.array_equal(area.mean(axis=0), solid.mean(axis=0))
     z = z_scores(solid, area)
     assert np.abs(z).max() < Z_MAX, z
@@ -200,7 +155,7 @@ def analytic_irradiance_film(desc, sub=4):
 @pytest.mark.parametrize("solid_angle", [False, True])
 def test_irradiance_frame_matches_lambert(irradiance, r, solid_angle):
     d = irradiance.desc()
-    films = sub_renders(r, d, solid_angle, 0, SUBRENDERS, SUB_SPP)
+    films = sub_renders(r, d, {"light_solid_angle": solid_angle}, 0, SUBRENDERS, SUB_SPP)
     want = analytic_irradiance_film(d)
     m = block_means(films)
     w = block_means(np.repeat(want[None, :, :, None], 3, axis=3))[0]
@@ -219,14 +174,8 @@ NEAR_LIGHT_ERROR_RATIO = 0.8
 
 def test_near_light_error_is_lower(near, r):
     d = near.desc()
-    ref = render(r, d, 1 << 20, (1 << 20) + 1024, True, raw=False)[..., :3].astype(np.float64)
-
-    def rel_mse(solid_angle, first):
-        errs = [((render(r, d, first + 16 * k, first + 16 * (k + 1), solid_angle, raw=False)[..., :3] - ref) ** 2 / (ref ** 2 + 1e-2)).mean()
-                for k in range(8)]
-        return float(np.mean(errs))
-
-    area, solid = rel_mse(False, 0), rel_mse(True, 4096)
+    ref = reference(r, d, SOLID_ANGLE)
+    area, solid = rel_mse(r, d, AREA, ref, 0), rel_mse(r, d, SOLID_ANGLE, ref, 4096)
     print(f"near_light 16 spp rel. MSE: area {area:.4e}, solid angle {solid:.4e}, ratio {solid / area:.4f} (fast={r.fast})")
     assert solid <= NEAR_LIGHT_ERROR_RATIO * area, (solid, area, solid / area)
 
@@ -234,7 +183,7 @@ def test_near_light_error_is_lower(near, r):
 # ---- 5. scheduling and the other modes --------------------------------------------------------------------------------------------
 def test_scheduling_and_sharding_change_no_bit(near, r):
     d = near.desc()
-    whole = render(r, d, 0, 8, solid_angle=True)
+    whole = render(r, d, 0, 8, SOLID_ANGLE)
     r.clear()
     r.render(0, 3)
     r.render(3, 8)
@@ -258,15 +207,15 @@ def test_scheduling_and_sharding_change_no_bit(near, r):
 def test_gbuffer_and_adaptive_compose(near, r):
     d = near.desc()
     r.set_option("gbuffer", 1)
-    off = render(r, d, 0, 4, solid_angle=False)
+    off = render(r, d, 0, 4, AREA)
     gb_off = r.gbuffer()
-    on = render(r, d, 0, 4, solid_angle=True)
+    on = render(r, d, 0, 4, SOLID_ANGLE)
     gb_on = r.gbuffer()
     assert not np.array_equal(bits(on), bits(off))  # the option changes the film ...
     for a, b in zip(gb_on[:2], gb_off[:2]):  # ... not the first-hit guides (the third, the luminance variance, follows the film)
         assert np.array_equal(bits(a), bits(b))
     r.set_option("gbuffer", 0)
-    uniform = render(r, d, 0, 8, solid_angle=True)
+    uniform = render(r, d, 0, 8, SOLID_ANGLE)
     r.render_adaptive(0.0, 4, 8)
     assert np.array_equal(bits(r.film(raw=True)), bits(uniform))
 
@@ -274,10 +223,10 @@ def test_gbuffer_and_adaptive_compose(near, r):
 # ---- 6. errors --------------------------------------------------------------------------------------------------------------------
 def test_volume_integrator_and_bad_values_are_refused(medium_small, r):
     d = medium_small.desc()
-    before = render(r, d, 0, 2, solid_angle=False)
+    before = render(r, d, 0, 2, AREA)
     r.set_option("light_solid_angle", 1)
     with pytest.raises(RuntimeError, match=r"lrk_upload_scene failed \(-5\): .*solid-angle"):
         r.upload(d)
     with pytest.raises(RuntimeError, match=r"failed \(-1\)"):
         r.set_option("light_solid_angle", 2)
-    assert np.array_equal(bits(render(r, d, 0, 2, solid_angle=False)), bits(before))
+    assert np.array_equal(bits(render(r, d, 0, 2, AREA)), bits(before))

@@ -5,29 +5,21 @@ command line."""
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 from scipy import stats
 
-from luisarender_b200 import _ffi as F
+import host_harness
+from light_sampling_checks import check_cli_lists_and_parses_flag, check_python_option_rejects_bad_values
 
-REPO = Path(__file__).resolve().parents[1]
-SRC = REPO / "tests" / "host_device" / "spherical_triangle_host.cpp"
-OUT = REPO / "tests" / "host_device" / "_build" / "libspherical_triangle_host.so"
-HEADER = REPO / "luisarender_b200" / "csrc" / "device" / "spherical_triangle.h"
 f32 = np.float32
 EPS = float(np.finfo(f32).eps)
 
 
 @pytest.fixture(scope="module")
 def lib():
-    if not OUT.exists() or OUT.stat().st_mtime < max(p.stat().st_mtime for p in [SRC, HEADER]):
-        OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-ffp-contract=off", "-shared", str(SRC), "-o", str(OUT)], check=True)
-    h = C.CDLL(str(OUT))
+    h = host_harness.load("spherical_triangle_host", [host_harness.DEVICE / "spherical_triangle.h"], ["-O2", "-ffp-contract=off"])
     h.st_solid_angle.argtypes = [C.c_int64] + [C.c_void_p] * 3
     h.st_use_spherical.argtypes = [C.c_int64] + [C.c_void_p] * 2
     h.st_sample.argtypes = [C.c_int64] + [C.c_void_p] * 8
@@ -291,20 +283,11 @@ def test_spherical_sampling_is_quieter_close_to_a_large_light(lib):
 
 # ---- the option's surface ---------------------------------------------------------------------------------------------------------
 def test_python_option_rejects_unknown_values():
-    from luisarender_b200.api import Renderer
-
-    for bad in (2, -1, "yes", 0.5):
-        with pytest.raises(ValueError):
-            Renderer(light_solid_angle=bad)  # checked before a device is looked for
+    check_python_option_rejects_bad_values("light_solid_angle")
 
 
 def test_cli_lists_and_parses_light_solid_angle(tmp_path):
-    cli = F.LIB_DIR / "luisa-render-cli"
-    r = subprocess.run([str(cli), "--help"], capture_output=True, text=True, timeout=60)
-    assert r.returncode == 0 and "--light-solid-angle" in r.stdout
-    # the flag parses: the run gets as far as reading the scene, which does not exist
-    r = subprocess.run([str(cli), "-b", "cuda", "--light-solid-angle", str(tmp_path / "missing.luisa")], capture_output=True, text=True, timeout=60)
-    assert r.returncode != 0 and "Unrecognized options" not in r.stderr and "[error]" in r.stderr
+    check_cli_lists_and_parses_flag("--light-solid-angle", tmp_path)
 
 
 def test_near_light_scene_generators():

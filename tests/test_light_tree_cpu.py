@@ -5,29 +5,22 @@ command line."""
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 from scipy import stats
 
-from luisarender_b200 import _ffi as F
+import host_harness
+from light_sampling_checks import check_cli_lists_and_parses_flag, check_python_option_rejects_bad_values
 
-REPO = Path(__file__).resolve().parents[1]
-SRC = REPO / "tests" / "host_device" / "light_tree_host.cpp"
-OUT = REPO / "tests" / "host_device" / "_build" / "liblight_tree_host.so"
-HEADER = REPO / "luisarender_b200" / "csrc" / "device" / "light_tree.h"
 NONE = 0xFFFFFFFF
 f32 = np.float32
 
 
 @pytest.fixture(scope="module")
 def lib():
-    if not OUT.exists() or OUT.stat().st_mtime < max(p.stat().st_mtime for p in [SRC, HEADER]):
-        OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-ffp-contract=off", "-shared", str(SRC), "-o", str(OUT)], check=True)
-    h = C.CDLL(str(OUT))
+    """The harness of light_tree.h: the instance-level trees (lt_*) and the triangle-level ones (ltt_*, test_light_tree_triangles_cpu.py)."""
+    h = host_harness.load("light_tree_host", [host_harness.DEVICE / "light_tree.h"], ["-O2", "-ffp-contract=off"])
     h.lt_build.restype = C.c_void_p
     h.lt_build.argtypes = [C.c_int] + [C.c_void_p] * 4
     h.lt_free.argtypes = [C.c_void_p]
@@ -37,6 +30,16 @@ def lib():
     h.lt_pmf.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]
     h.lt_sample.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 4
     h.lt_dead_mass.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    h.ltt_build.restype = C.c_void_p
+    h.ltt_build.argtypes = [C.c_int64, C.c_void_p, C.c_int]
+    h.ltt_free.argtypes = [C.c_void_p]
+    h.ltt_node_count.restype = C.c_int64
+    h.ltt_node_count.argtypes = [C.c_void_p]
+    h.ltt_copy.argtypes = [C.c_void_p] * 3
+    h.ltt_pmf.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    h.ltt_sample.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 5
+    h.ltt_sample_u_left.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 4
+    h.ltt_dead_mass.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 3
     return h
 
 
@@ -239,20 +242,11 @@ def test_single_light_pmf_is_exactly_one(lib):
 
 
 def test_python_option_rejects_unknown_values():
-    from luisarender_b200.api import Renderer
-
-    for bad in (2, -1, "yes", 0.5):
-        with pytest.raises(ValueError):
-            Renderer(light_tree=bad)  # checked before a device is looked for
+    check_python_option_rejects_bad_values("light_tree")
 
 
 def test_cli_lists_and_parses_light_tree(tmp_path):
-    cli = F.LIB_DIR / "luisa-render-cli"
-    r = subprocess.run([str(cli), "--help"], capture_output=True, text=True, timeout=60)
-    assert r.returncode == 0 and "--light-tree" in r.stdout
-    # the flag parses: the run gets as far as reading the scene, which does not exist
-    r = subprocess.run([str(cli), "-b", "cuda", "--light-tree", str(tmp_path / "missing.luisa")], capture_output=True, text=True, timeout=60)
-    assert r.returncode != 0 and "Unrecognized options" not in r.stderr and "[error]" in r.stderr
+    check_cli_lists_and_parses_flag("--light-tree", tmp_path)
 
 
 def test_many_light_scene_generator():

@@ -12,9 +12,10 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from light_sampling_checks import SUB_SPP, SUBRENDERS, Z_MAX, bits, r, reference, rel_mse, render, sub_renders, z_scores  # noqa: F401
+
 REPO = Path(__file__).resolve().parents[1]
 pytestmark = pytest.mark.gpu
-BLOCK = 16
 
 
 def _scene(src):
@@ -51,68 +52,8 @@ def frames():
     return get
 
 
-@pytest.fixture
-def r(gpu_renderer):
-    """gpu_renderer, with the options this file touches back at their defaults afterwards (the renderer is shared by the session)."""
-    yield gpu_renderer
-    for name, value in (("light_tree_triangles", 0), ("light_tree", 0), ("light_solid_angle", 0), ("gbuffer", 0),
-                        ("max_paths_per_pass", 136 << 20)):
-        gpu_renderer.set_option(name, value)
-    gpu_renderer.set_shard(0, 1, 32)
-
-
-MODES = {"uniform": (0, 0), "tree": (1, 0), "triangles": (1, 1)}
-
-
-def upload(r, desc, mode):
-    tree, tris = MODES[mode]
-    r.set_option("light_tree", tree)
-    r.set_option("light_tree_triangles", tris)
-    r.upload(desc)
-
-
-def render(r, desc, spp_begin, spp_end, mode, raw=True):
-    upload(r, desc, mode)
-    r.render(spp_begin, spp_end)
-    return r.film(raw=raw).copy()
-
-
-def bits(a):
-    return np.ascontiguousarray(a).view(np.uint32)
-
-
-def sub_renders(r, desc, mode, first, count, spp):
-    """`count` independent renders of `spp` samples each from sample index `first` on, as normalised films [count, H, W, 3]: one
-    upload (the bottom trees are built there), then a cleared film per render."""
-    upload(r, desc, mode)
-    films = []
-    for k in range(count):
-        r.clear()
-        r.render(first + k * spp, first + (k + 1) * spp)
-        films.append(r.film(raw=False)[..., :3].copy())
-    return np.stack(films).astype(np.float64)
-
-
-def block_means(films):
-    n, h, w, _ = films.shape
-    hb, wb = h // BLOCK, w // BLOCK
-    b = films[:, :hb * BLOCK, :wb * BLOCK].reshape(n, hb, BLOCK, wb, BLOCK, 3).mean(axis=(2, 4, 5)).reshape(n, -1)
-    return np.concatenate([films.mean(axis=(1, 2, 3))[:, None], b], axis=1)  # column 0: the whole image
-
-
-def z_scores(a, b):
-    """(mean a - mean b) / its standard error, per block, from the spread of the independent sub-renders.  A block without noise in
-    either (the black background) gives 0 if the means agree, else inf."""
-    ma, mb = block_means(a), block_means(b)
-    se = np.sqrt(ma.var(axis=0, ddof=1) / len(ma) + mb.var(axis=0, ddof=1) / len(mb))
-    diff = ma.mean(axis=0) - mb.mean(axis=0)
-    return np.where(se > 0, diff / np.where(se > 0, se, 1.0), np.where(diff == 0, 0.0, np.inf))
-
-
-# As in test_light_tree.py: 1 + (16 x 16 blocks) means of 32 + 32 sub-renders compared at 4 sigma; with sigma estimated from the
-# sub-renders (t, 62 dof) each comparison fails by chance with probability 1.7e-4.  The renders are seeded: a frame passes or fails
-# for good.
-SUBRENDERS, SUB_SPP, Z_MAX = 32, 16, 4.0
+MODES = {"uniform": {"light_tree": 0, "light_tree_triangles": 0}, "tree": {"light_tree": 1, "light_tree_triangles": 0},
+         "triangles": {"light_tree": 1, "light_tree_triangles": 1}}
 
 
 # ---- 1. off changes nothing; single-triangle emitters render bit for bit ----------------------------------------------------------
@@ -128,8 +69,8 @@ def test_option_off_equals_a_context_that_never_set_it(frames, r):
         want, want_launches = fresh.film(raw=True), fresh.stats()["kernel_launches"]
     finally:
         fresh.close()
-    render(r, d, 0, 4, "triangles")  # leaves the bottom trees behind in this context
-    got = render(r, d, 0, 4, "tree")
+    render(r, d, 0, 4, MODES["triangles"])  # leaves the bottom trees behind in this context
+    got = render(r, d, 0, 4, MODES["tree"])
     assert np.array_equal(bits(got), bits(want))
     assert r.stats()["kernel_launches"] == want_launches
 
@@ -138,8 +79,8 @@ def test_option_off_equals_a_context_that_never_set_it(frames, r):
 def test_single_triangle_emitters_render_bit_identically(frames, r, solid_angle):
     d = frames("irradiance").desc()
     r.set_option("light_solid_angle", solid_angle)
-    off = render(r, d, 0, 8, "tree")
-    on = render(r, d, 0, 8, "triangles")
+    off = render(r, d, 0, 8, MODES["tree"])
+    on = render(r, d, 0, 8, MODES["triangles"])
     assert np.array_equal(bits(on), bits(off))
 
 
@@ -150,8 +91,8 @@ def test_single_triangle_emitters_render_bit_identically(frames, r, solid_angle)
 def test_triangle_tree_agrees_with_uniform(frames, r, name, solid_angle):
     d = frames(name).desc()
     r.set_option("light_solid_angle", solid_angle)
-    uniform = sub_renders(r, d, "uniform", 0, SUBRENDERS, SUB_SPP)
-    tris = sub_renders(r, d, "triangles", SUBRENDERS * SUB_SPP, SUBRENDERS, SUB_SPP)  # disjoint sample indices
+    uniform = sub_renders(r, d, MODES["uniform"], 0, SUBRENDERS, SUB_SPP)
+    tris = sub_renders(r, d, MODES["triangles"], SUBRENDERS * SUB_SPP, SUBRENDERS, SUB_SPP)  # disjoint sample indices
     assert uniform.mean() > 0
     z = z_scores(tris, uniform)
     assert np.abs(z).max() < Z_MAX, z
@@ -160,8 +101,8 @@ def test_triangle_tree_agrees_with_uniform(frames, r, name, solid_angle):
 def test_globe_transforms_light_the_room_alike(frames, r):
     """The mirrored globe is the uniform one's sphere (wound inwards, then mirrored in x, so that it faces outwards): it lights the
     room alike.  The mirror swaps which side of the globe faces the red and the green wall, so only the image means are compared."""
-    a = sub_renders(r, frames("globe_uniform").desc(), "triangles", 0, 16, SUB_SPP).mean(axis=(1, 2, 3))
-    b = sub_renders(r, frames("globe_mirrored").desc(), "triangles", 16 * SUB_SPP, 16, SUB_SPP).mean(axis=(1, 2, 3))
+    a = sub_renders(r, frames("globe_uniform").desc(), MODES["triangles"], 0, 16, SUB_SPP).mean(axis=(1, 2, 3))
+    b = sub_renders(r, frames("globe_mirrored").desc(), MODES["triangles"], 16 * SUB_SPP, 16, SUB_SPP).mean(axis=(1, 2, 3))
     se = np.sqrt(a.var(ddof=1) / len(a) + b.var(ddof=1) / len(b))
     assert a.mean() > 0 and abs(a.mean() - b.mean()) < 0.05 * a.mean() + Z_MAX * se
 
@@ -177,15 +118,8 @@ ERROR_RATIO_BOUND = {"globe_uniform": 0.7, "many": 0.95}
 @pytest.mark.parametrize("name", sorted(ERROR_RATIO_BOUND))
 def test_error_is_lower_than_the_instance_tree(frames, r, name):
     d = frames(name).desc()
-    upload(r, d, "triangles")
-    r.render(1 << 20, (1 << 20) + 1024)
-    ref = r.film(raw=False)[..., :3].astype(np.float64)
-
-    def rel_mse(mode, first):
-        films = sub_renders(r, d, mode, first, 8, 16)
-        return float(np.mean([((f - ref) ** 2 / (ref ** 2 + 1e-2)).mean() for f in films]))
-
-    tree, tris = rel_mse("tree", 0), rel_mse("triangles", 4096)
+    ref = reference(r, d, MODES["triangles"])
+    tree, tris = rel_mse(r, d, MODES["tree"], ref, 0), rel_mse(r, d, MODES["triangles"], ref, 4096)
     print(f"{name} 16 spp rel. MSE: instance tree {tree:.4e}, triangle trees {tris:.4e}, ratio {tris / tree:.4f} (fast={r.fast})")
     assert tris <= ERROR_RATIO_BOUND[name] * tree, (tris, tree, tris / tree)
 
@@ -193,7 +127,7 @@ def test_error_is_lower_than_the_instance_tree(frames, r, name):
 # ---- 4. scheduling and the other modes --------------------------------------------------------------------------------------------
 def test_scheduling_and_sharding_change_no_bit(frames, r):
     d = frames("many").desc()
-    whole = render(r, d, 0, 8, "triangles")
+    whole = render(r, d, 0, 8, MODES["triangles"])
     r.clear()
     r.render(0, 3)
     r.render(3, 8)
@@ -217,15 +151,15 @@ def test_scheduling_and_sharding_change_no_bit(frames, r):
 def test_gbuffer_and_adaptive_compose(frames, r):
     d = frames("globe_stretched").desc()
     r.set_option("gbuffer", 1)
-    off = render(r, d, 0, 4, "tree")
+    off = render(r, d, 0, 4, MODES["tree"])
     gb_off = r.gbuffer()
-    on = render(r, d, 0, 4, "triangles")
+    on = render(r, d, 0, 4, MODES["triangles"])
     gb_on = r.gbuffer()
     assert not np.array_equal(bits(on), bits(off))  # the option changes the film ...
     for a, b in zip(gb_on[:2], gb_off[:2]):  # ... not the first-hit guides
         assert np.array_equal(bits(a), bits(b))
     r.set_option("gbuffer", 0)
-    want = render(r, d, 0, 8, "triangles")
+    want = render(r, d, 0, 8, MODES["triangles"])
     r.render_adaptive(0.0, 4, 8)
     assert np.array_equal(bits(r.film(raw=True)), bits(want))
 
@@ -233,7 +167,7 @@ def test_gbuffer_and_adaptive_compose(frames, r):
 # ---- 5. errors --------------------------------------------------------------------------------------------------------------------
 def test_refusals(frames, r):
     d = frames("medium").desc()
-    before = render(r, d, 0, 2, "uniform")
+    before = render(r, d, 0, 2, MODES["uniform"])
     r.set_option("light_tree", 1)
     r.set_option("light_tree_triangles", 1)
     with pytest.raises(RuntimeError, match=r"lrk_upload_scene failed \(-5\)"):
@@ -243,4 +177,4 @@ def test_refusals(frames, r):
         r.upload(frames("cornell").desc())
     with pytest.raises(RuntimeError, match=r"failed \(-1\)"):
         r.set_option("light_tree_triangles", 2)
-    assert np.array_equal(bits(render(r, d, 0, 2, "uniform")), bits(before))
+    assert np.array_equal(bits(render(r, d, 0, 2, MODES["uniform"])), bits(before))

@@ -5,44 +5,19 @@ transforms with the expressions the shade kernels use.  Also the top-level trees
 surface in Python and on the command line."""
 from __future__ import annotations
 
-import ctypes as C
 import hashlib
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 from scipy import stats
 
-from luisarender_b200 import _ffi as F
+from light_sampling_checks import check_cli_lists_and_parses_flag, check_python_option_rejects_bad_values
 from luisarender_b200.scenes import _icosphere
+from test_light_tree_cpu import LightSet, lib  # noqa: F401 (lib: the fixture of light_tree.h's harness)
 
-REPO = Path(__file__).resolve().parents[1]
-SRC = REPO / "tests" / "host_device" / "light_tree_triangles_host.cpp"
-OUT = REPO / "tests" / "host_device" / "_build" / "liblight_tree_triangles_host.so"
-HEADER = REPO / "luisarender_b200" / "csrc" / "device" / "light_tree.h"
 NONE = 0xFFFFFFFF
 ONE_SIDED, MIRRORED, TWO_SIDED = 0, 1, 2
 f32 = np.float32
-
-
-@pytest.fixture(scope="module")
-def lib():
-    if not OUT.exists() or OUT.stat().st_mtime < max(p.stat().st_mtime for p in [SRC, HEADER]):
-        OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-ffp-contract=off", "-shared", str(SRC), "-o", str(OUT)], check=True)
-    h = C.CDLL(str(OUT))
-    h.ltt_build.restype = C.c_void_p
-    h.ltt_build.argtypes = [C.c_int64, C.c_void_p, C.c_int]
-    h.ltt_free.argtypes = [C.c_void_p]
-    h.ltt_node_count.restype = C.c_int64
-    h.ltt_node_count.argtypes = [C.c_void_p]
-    h.ltt_copy.argtypes = [C.c_void_p] * 3
-    h.ltt_pmf.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    h.ltt_sample.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 5
-    h.ltt_sample_u_left.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 4
-    h.ltt_dead_mass.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 3
-    return h
 
 
 # ---- meshes (object space, [n, 3, 3]) and transforms (object-to-world 3x4) -------------------------------------------------------
@@ -338,40 +313,21 @@ PARENT_TOP_TREE_SHA256 = {
 
 
 @pytest.mark.parametrize("n", sorted(PARENT_TOP_TREE_SHA256))
-def test_instance_level_trees_keep_their_bytes(n):
-    import test_light_tree_cpu as T  # the instance-level harness, built as that module's fixture builds it
-
-    if not T.OUT.exists() or T.OUT.stat().st_mtime < max(q.stat().st_mtime for q in [T.SRC, T.HEADER]):
-        T.OUT.parent.mkdir(parents=True, exist_ok=True)
-        subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-ffp-contract=off", "-shared", str(T.SRC), "-o", str(T.OUT)], check=True)
-    top = C.CDLL(str(T.OUT))
-    top.lt_build.restype = C.c_void_p
-    top.lt_build.argtypes = [C.c_int] + [C.c_void_p] * 4
-    top.lt_free.argtypes = [C.c_void_p]
-    top.lt_node_count.restype = C.c_int64
-    top.lt_node_count.argtypes = [C.c_void_p]
-    top.lt_copy.argtypes = [C.c_void_p] * 3
-    assert hashlib.sha256(T.LightSet(n, seed=n).build(top).bytes()).hexdigest() == PARENT_TOP_TREE_SHA256[n]
+def test_instance_level_trees_keep_their_bytes(lib, n):
+    assert hashlib.sha256(LightSet(n, seed=n).build(lib).bytes()).hexdigest() == PARENT_TOP_TREE_SHA256[n]
 
 
 # ---- 6. the option's surface ----------------------------------------------------------------------------------------------------
 def test_python_option_rejects_bad_values():
     from luisarender_b200.api import Renderer
 
-    for bad in (2, -1, "yes", 0.5):
-        with pytest.raises(ValueError):
-            Renderer(light_tree=True, light_tree_triangles=bad)  # checked before a device is looked for
+    check_python_option_rejects_bad_values("light_tree_triangles", light_tree=True)
     with pytest.raises(ValueError, match="light_tree=True"):
         Renderer(light_tree_triangles=True)
 
 
 def test_cli_lists_and_parses_light_tree_triangles(tmp_path):
-    cli = F.LIB_DIR / "luisa-render-cli"
-    r = subprocess.run([str(cli), "--help"], capture_output=True, text=True, timeout=60)
-    assert r.returncode == 0 and "--light-tree-triangles" in r.stdout
-    r = subprocess.run([str(cli), "-b", "cuda", "--light-tree-triangles", str(tmp_path / "missing.luisa")], capture_output=True, text=True,
-                       timeout=60)
-    assert r.returncode != 0 and "Unrecognized options" not in r.stderr and "[error]" in r.stderr
+    check_cli_lists_and_parses_flag("--light-tree-triangles", tmp_path)
 
 
 def test_emissive_globe_generator():
