@@ -578,7 +578,16 @@ int lrk_reduce_film(lrk_ctx *ctx, uint32_t root);
  *                             towards the point.  Read at lrk_upload_scene, which builds one such tree per emissive mesh and side
  *                             (about 14 us per triangle on the host); another value -> LRK_ERR_INVALID_ARGUMENT; on without
  *                             "light_tree" -> LRK_ERR_INVALID_ARGUMENT at lrk_upload_scene.  Combines with "light_solid_angle".
- *                             Surface integrator only, as "light_tree".  LRK_ABI_VERSION stays 8: no layout or signature changed */
+ *                             Surface integrator only, as "light_tree".  LRK_ABI_VERSION stays 8: no layout or signature changed
+ *   "light_candidates" (0..32) resampled next-event estimation: for M = 2 .. 32, each surface vertex draws M candidates from the
+ *                             light sampling the three options above configure, weights each by the luminance of its unshadowed
+ *                             contribution (closure value x cosine x emission x MIS weight) over its pdf, and traces the shadow
+ *                             ray of one, chosen in proportion to its weight (resampled importance sampling without reuse across
+ *                             pixels).  Unbiased for every M; less noise where the closure or the receiver's orientation matters,
+ *                             at the cost of M light samples and M closure evaluations per vertex.  0 (the default) and 1: one
+ *                             light sample, as without the option.  Read at lrk_upload_scene; another value ->
+ *                             LRK_ERR_INVALID_ARGUMENT.  Surface integrator only: lrk_upload_scene returns LRK_ERR_UNSUPPORTED for
+ *                             the volume integrator with M >= 2.  LRK_ABI_VERSION stays 8: no layout or signature changed */
 int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value);
 
 int lrk_film_clear(lrk_ctx *ctx);

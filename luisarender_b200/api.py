@@ -98,16 +98,21 @@ class Renderer:
     ``light_solid_angle=True`` sets the option "light_solid_angle": from the next upload on, next-event estimation samples the
     point on the chosen emissive triangle uniformly in solid angle instead of by area (surface integrator only).
     ``light_tree_triangles=True`` (with ``light_tree=True``) sets the option "light_tree_triangles": the light tree also picks the
-    triangle of the chosen emitter, from a tree over its mesh's triangles, instead of by area."""
+    triangle of the chosen emitter, from a tree over its mesh's triangles, instead of by area.
+    ``light_candidates=M`` (an int from 0 to 32) sets the option "light_candidates": for M >= 2, from the next upload on,
+    next-event estimation draws M candidates from the light sampling above and traces the shadow ray of one, chosen by its
+    unshadowed contribution (resampled importance sampling; surface integrator only).  0 and 1 keep one light sample per vertex."""
 
     def __init__(self, device_index: int = -1, max_paths_per_pass: int = 0, light_tree: bool = False, light_solid_angle: bool = False,
-                 light_tree_triangles: bool = False):
+                 light_tree_triangles: bool = False, light_candidates: int = 1):
         light_options = {"light_tree": light_tree, "light_solid_angle": light_solid_angle, "light_tree_triangles": light_tree_triangles}
         for name, value in light_options.items():
             if value not in (0, 1):
                 raise ValueError(f"{name} is False or True, not {value!r}")
         if light_tree_triangles and not light_tree:
             raise ValueError("light_tree_triangles is the bottom level of the light tree: it needs light_tree=True")
+        if type(light_candidates) is not int or not 0 <= light_candidates <= 32:
+            raise ValueError(f"light_candidates is an int from 0 to 32, not {light_candidates!r}")
         self._lib = F.device_lib()
         cfg = F.DeviceCfg(device_index, 0, max_paths_per_pass)
         self._ctx = C.c_void_p()
@@ -118,6 +123,8 @@ class Renderer:
         for name, value in light_options.items():
             if value:
                 self.set_option(name, 1)
+        if light_candidates >= 2:
+            self.set_option("light_candidates", light_candidates)
 
     def _check(self, rc: int, what: str):
         if rc != 0:

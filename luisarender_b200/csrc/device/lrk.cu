@@ -693,6 +693,10 @@ int check_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
     if (want.solid_angle && volume)
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: solid-angle light sampling (option light_solid_angle) serves the surface integrator "
                                               "only; the volume integrator evaluates its light pdfs from the world origin");
+    if (want.candidates >= 2u && volume)
+        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: resampled next-event estimation (option light_candidates >= 2) serves the surface "
+                                              "integrator only; the volume integrator traces every light sample it draws, since the "
+                                              "occlusion of each advances its random stream");
     return LRK_OK;
 }
 
@@ -731,6 +735,9 @@ int upload_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
             rec.bottom_trail = a.lt_bottom_trail.get<const unsigned long long>();
         }
     }
+    rec.select = want.tree ? kLightSelectTree : kLightSelectUniform;
+    rec.point = want.solid_angle ? kLightPointSolidAngle : kLightPointArea;
+    rec.candidates = want.candidates;
     LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get<char>() + sizeof(DeviceScene), &rec, sizeof(DeviceLightTree), cudaMemcpyHostToDevice, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));// the host arrays and `rec` are locals
     ctx->light_active = want;
@@ -1171,6 +1178,10 @@ int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value) {
     else if (bool LightSampling::*field = light_sampling_option(n)) {// takes effect at the next lrk_upload_scene
         if (value != 0 && value != 1) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: " + n + " is 0 or 1");
         ctx->light_requested.*field = value != 0;
+    } else if (n == "light_candidates") {// takes effect at the next lrk_upload_scene
+        if (value < 0 || value > static_cast<int64_t>(kLightCandidatesMax))
+            return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_set_option: light_candidates is 0 to 32 (0 and 1: one light sample, no resampling)");
+        ctx->light_requested.candidates = static_cast<uint32_t>(value);
     }
     else if (n == "pin_host_buffers") {
         ctx->pin_host = value != 0;

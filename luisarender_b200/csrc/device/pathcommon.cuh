@@ -6,6 +6,7 @@
 #include <utility>
 
 #include "hit_kinds.h"
+#include "light_resampling.h"
 #include "shading.cuh"
 
 namespace lrk {
@@ -198,6 +199,92 @@ __device__ __forceinline__ void shade_surface(Closure &cl, const Interaction &it
             contrib = w * beta * e_light.f * ls.eval.L;
         }
     }
+}
+
+// shade_surface of the surface integrator with resampled next-event estimation (option "light_candidates" = m >= 2,
+// light_resampling.h): draw_light(u_sel, u0, u1) returns the LightSample of the configured light sampling; candidate 0 takes the
+// bounce's (u_sel, ul0, ul1).  The m candidates and the closure's own sample are evaluated through ONE copy of the closure code, as
+// in shade_surface_eval (a loop that is deliberately not unrolled; sample_world runs before any evaluate_world).  Returns the kept
+// candidate's contribution beta * c_y * W / (m * p_hat_y) and its shadow ray; a zero contribution when every weight was 0.
+template<typename Closure, typename DrawLight>
+__device__ __forceinline__ void shade_surface_resampled(Closure &cl, const Interaction &it, const Frame &shading, V3 wo, DrawLight &&draw_light,
+                                                        uint32_t m, uint32_t depth, float u_sel, float ul0, float ul1, V3 beta, float u_lobe,
+                                                        float ub0, float ub1, V3 &contrib, float4 &ray_o, float4 &ray_d, V3 &wi_world,
+                                                        V3 &f_over, float &pdf_bsdf) {
+    V3 wo_local = shading.world_to_local(wo);
+    cl.prepare(wo_local);
+    V3 wi_sampled_local;
+    bool run_sampled;
+    if constexpr (has_world_api<Closure>::value) {
+        run_sampled = cl.sample_world(u_lobe, ub0, ub1);
+        wi_world = cl.sampled_wi;
+        wi_sampled_local = shading.world_to_local(wi_world);
+    } else {
+        run_sampled = cl.sample_direction(wo_local, u_lobe, ub0, ub1, wi_sampled_local);
+        wi_world = shading.local_to_world(wi_sampled_local);
+    }
+    uint32_t state = light_candidates_seed(u_sel, ul0, ul1, depth);
+    LightReservoir res = light_reservoir_empty();
+    V3 c_kept = v3(0.f);
+    float p_hat_kept = 0.f;
+    ray_o = make_float4(0.f, 0.f, 0.f, 0.f);
+    ray_d = make_float4(0.f, 0.f, 1.f, 0.f);
+    f_over = v3(0.f);
+    pdf_bsdf = 0.f;
+#pragma unroll 1
+    for (uint32_t k = 0; k <= m; k++) {// k < m: candidate k; k = m: the closure's own sample
+        const bool light = k < m;
+        LightSample ls;
+        float u_res = 0.f;
+        V3 wi_w = wi_world, wi_l = wi_sampled_local;
+        bool run = run_sampled;
+        if (light) {
+            float us = u_sel, u0 = ul0, u1 = ul1;
+            if (k != 0u) light_candidate_numbers(state, us, u0, u1, u_res);
+            ls = draw_light(us, u0, u1);
+            wi_w = v3(ls.ray_d_tmax.x, ls.ray_d_tmax.y, ls.ray_d_tmax.z);
+            wi_l = shading.world_to_local(wi_w);
+            run = ls.eval.pdf > 0.0f;
+        }
+        SurfEval e;
+        e.f = v3(0.f);
+        e.pdf = 0.f;
+        if (run) {
+            if constexpr (has_world_api<Closure>::value) {
+                if (light) {
+                    e = cl.evaluate_world(wi_w);
+                } else {
+                    e.f = cl.sampled.f;
+                    e.pdf = cl.sampled.pdf;
+                }
+            } else if constexpr (has_evaluate_sampled<Closure>::value) {
+                e = light ? cl.evaluate_local(wo_local, wi_l) : cl.evaluate_sampled(wo_local, wi_l);
+            } else {
+                e = cl.evaluate_local(wo_local, wi_l);
+            }
+            if (!validate_surface_sides(it.ng, shading.n, wo, wi_w)) {
+                e.f = v3(0.f);
+                e.pdf = 0.f;
+            }
+        }
+        if (light) {
+            if (run) {
+                const V3 c = e.f * ls.eval.L * balance_heuristic(ls.eval.pdf, e.pdf);
+                const float p_hat = resampling_target(c.x, c.y, c.z);
+                if (light_reservoir_add(res, k, resampling_weight(p_hat, ls.eval.pdf), u_res)) {
+                    c_kept = c;
+                    p_hat_kept = p_hat;
+                    ray_o = ls.ray_o_tmin;
+                    ray_d = ls.ray_d_tmax;
+                }
+            }
+        } else {
+            f_over = e.f;
+            pdf_bsdf = e.pdf;
+        }
+    }
+    const float w = light_reservoir_weight(res, m, p_hat_kept);
+    contrib = w > 0.f ? beta * c_kept * w : v3(0.f);
 }
 
 struct PCG32 {// src/util/rng.cpp:142-174

@@ -83,6 +83,9 @@ struct DeviceLightTree {
     const uint2 *inst_bottom;                  // per instance: {root of its bottom tree in bottom_nodes, first of its trails}, root
                                                // kLightTreeNone for none
     const unsigned long long *bottom_trail;    // per triangle of a bottom tree: its trail
+    // The light sampling as the resampling shade kernels read it at run time (option "light_candidates" >= 2; the other kernels
+    // have it as template values): LightSelect, LightPoint (shading.cuh) and the candidate count M.
+    uint32_t select, point, candidates;
 };
 __device__ __forceinline__ const DeviceLightTree &light_tree_of(const DeviceScene &sc) {
     return *reinterpret_cast<const DeviceLightTree *>(sc.self + 1);

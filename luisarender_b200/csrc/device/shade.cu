@@ -37,15 +37,15 @@ int grid_of(Kernel kernel, int block, int sm_count) {
     return (per_sm > 0 ? per_sm : 1) * sm_count;
 }
 
-// calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection, light point sampling).  The fast
-// variant has none for the kinds that always run in strict arithmetic (hit_kind_always_strict): render_pass never launches them
-// there.
-template<uint32_t SEL, uint32_t PT, typename F>
+// calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection, light point sampling), or with the
+// kind's resampling instantiation (RESAMPLE; none for emitter-only hits).  The fast variant has none for the kinds that always run
+// in strict arithmetic (hit_kind_always_strict): render_pass never launches them there.
+template<uint32_t SEL, uint32_t PT, bool RESAMPLE = false, typename F>
 void with_shade_kernel(uint32_t kind, bool textured, F &&f) {
     with_hit_kind(kind, [&](auto k) {
         constexpr uint32_t K = decltype(k)::value;
-        if constexpr (!(kFastVariant && hit_kind_always_strict(K)))
-            textured ? f(shade_kernel<K, true, SEL, PT>) : f(shade_kernel<K, false, SEL, PT>);
+        if constexpr (!(kFastVariant && hit_kind_always_strict(K)) && !(RESAMPLE && K == kHitEmitter))
+            textured ? f(shade_kernel<K, true, SEL, PT, RESAMPLE>) : f(shade_kernel<K, false, SEL, PT, RESAMPLE>);
     });
 }
 
@@ -75,11 +75,14 @@ int volume_surface_grid(uint32_t kind, int sm_count) {
 }
 
 // the light sampling as the kernels' <SEL, PT>; the triangle-level trees need no instantiation of their own: the kernels find them
-// through light_tree_of(sc).bottom_nodes
+// through light_tree_of(sc).bottom_nodes.  Resampling (candidates >= 2) has one instantiation per kind, which reads the selection,
+// the point sampling and the candidate count from light_tree_of(sc); emitter-only hits sample no light and keep theirs.
 void launch_shade(uint32_t kind, bool textured, const LightSampling &light, int blocks, cudaStream_t stream, const DeviceScene &sc,
                   const PathBuffers &pb, uint32_t depth) {
     const auto launch = [&](auto kernel) { kernel<<<blocks, kShadeBlock, 0, stream>>>(sc, pb, depth); };
-    if (light.solid_angle) {
+    if (light.candidates >= 2u && kind != kHitEmitter) {
+        with_shade_kernel<kLightSelectUniform, kLightPointArea, true>(kind, textured, launch);
+    } else if (light.solid_angle) {
         if (light.tree) with_shade_kernel<kLightSelectTree, kLightPointSolidAngle>(kind, textured, launch);
         else with_shade_kernel<kLightSelectUniform, kLightPointSolidAngle>(kind, textured, launch);
     } else {

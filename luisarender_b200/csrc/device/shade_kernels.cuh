@@ -39,11 +39,42 @@ __device__ __noinline__ inline BounceDraws draw_bounce_from_tables(SamplerRef sc
     return d;
 }
 
+// The light sampling of the resampling shade kernels, chosen at run time from light_tree_of(sc): one instantiation per TEXTURED
+// serves every (selection, point) pair, out of line so that the kernels hold one call site each.  `sc`: *DeviceScene::self.
+template<bool TEXTURED>
+__device__ __noinline__ LightSample sample_light_configured(const DeviceScene &sc, const Interaction &it, float u_sel, float u0, float u1) {
+    if (sc.light_count == 0u && sc.env_prob == 0.f) {
+        LightSample ls;
+        ls.eval.L = v3(0.f);
+        ls.eval.pdf = 0.f;
+        ls.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
+        ls.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
+        return ls;
+    }
+    const DeviceLightTree &lt = light_tree_of(sc);
+    if (lt.select == kLightSelectTree)
+        return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectTree, kLightPointSolidAngle>(sc, it, u_sel, u0, u1)
+                                                 : sample_light<TEXTURED, kLightSelectTree, kLightPointArea>(sc, it, u_sel, u0, u1);
+    return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectUniform, kLightPointSolidAngle>(sc, it, u_sel, u0, u1)
+                                             : sample_light<TEXTURED, kLightSelectUniform, kLightPointArea>(sc, it, u_sel, u0, u1);
+}
+template<bool TEXTURED>
+__device__ __noinline__ LightEval evaluate_hit_configured(const DeviceScene &sc, const Interaction &it, V3 p_from, uint32_t inst) {
+    const DeviceLightTree &lt = light_tree_of(sc);
+    if (lt.select == kLightSelectTree)
+        return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectTree, kLightPointSolidAngle>(sc, it, p_from, inst)
+                                                 : evaluate_hit<TEXTURED, kLightSelectTree, kLightPointArea>(sc, it, p_from, inst);
+    return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointSolidAngle>(sc, it, p_from, inst)
+                                             : evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointArea>(sc, it, p_from, inst);
+}
+
 // Sorted-by-material dispatch, step 2: one shade kernel per closure kind, each over its own hit bucket.  SEL: the light selection
 // of next-event estimation (kLightSelectTree with the option "light_tree"); PT: its point sampling (kLightPointSolidAngle with the
-// option "light_solid_angle")
-template<uint32_t KIND, bool TEXTURED = false, uint32_t SEL = kLightSelectUniform, uint32_t PT = kLightPointArea>
+// option "light_solid_angle").  RESAMPLE: resampled next-event estimation (option "light_candidates" >= 2, every kind but
+// emitter-only): the light sampling and the candidate count come from light_tree_of(sc) at run time instead of SEL and PT.
+template<uint32_t KIND, bool TEXTURED = false, uint32_t SEL = kLightSelectUniform, uint32_t PT = kLightPointArea, bool RESAMPLE = false>
 __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kernel(DeviceScene sc, PathBuffers pb, uint32_t depth) {
+    static_assert(!RESAMPLE || (KIND != kHitEmitter && SEL == kLightSelectUniform && PT == kLightPointArea), "one resampling kernel per kind");
     // the compaction is written out here rather than through block_append, which raises registers or spills of most instantiations
     __shared__ uint32_t s_warp_next[kShadeBlock / 32], s_warp_shadow[kShadeBlock / 32];
     __shared__ uint32_t s_base_next, s_base_shadow;
@@ -71,7 +102,9 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                 it.back_facing = dot(wo, it.ng) < 0.0f;
                 // emitter hit with MIS: mega_path.cpp:80-87, uniform.cpp:50-65
                 if (sc.light_count != 0u && it.shape.has_light()) {
-                    LightEval e = evaluate_hit<TEXTURED, SEL, PT>(sc, it, v3(ro.x, ro.y, ro.z), hit.x);
+                    LightEval e;
+                    if constexpr (RESAMPLE) e = evaluate_hit_configured<TEXTURED>(*sc.self, it, v3(ro.x, ro.y, ro.z), hit.x);
+                    else e = evaluate_hit<TEXTURED, SEL, PT>(sc, it, v3(ro.x, ro.y, ro.z), hit.x);
                     V3 add = beta * e.L * balance_heuristic(pdf_bsdf, e.pdf);
                     float4 li = pb.li[ir.x];
                     li.x += add.x;
@@ -96,18 +129,25 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                         u_sel = dr.u_sel; ul0 = dr.ul0; ul1 = dr.ul1; u_lobe = dr.u_lobe; ub0 = dr.ub0; ub1 = dr.ub1; u_rr = dr.u_rr;
                         state = dr.state;
                     }
-                    LightSample ls;
+                    LightSample ls;// with RESAMPLE: the kept candidate's shadow ray only
                     ls.eval.L = v3(0.f);
                     ls.eval.pdf = 0.f;
                     ls.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
                     ls.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
-                    if (sc.light_count != 0u || sc.env_prob != 0.f) ls = sample_light<TEXTURED, SEL, PT>(sc, it, u_sel, ul0, ul1);
+                    if constexpr (!RESAMPLE)
+                        if (sc.light_count != 0u || sc.env_prob != 0.f) ls = sample_light<TEXTURED, SEL, PT>(sc, it, u_sel, ul0, ul1);
                     const lrk_surface *surf = sc.surfaces + it.shape.surface_tag;
                     V3 contrib, wi, f;
                     float pdf;
                     const float eta_scale = with_hit_closure<KIND, TEXTURED>(sc, surf, it, wo, [&] { return closure_frame<TEXTURED>(sc, surf, it, wo); },
                                                                            [&](auto &cl, const Frame &fr) {
-                        shade_surface<false>(cl, it, fr, wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
+                        if constexpr (RESAMPLE) {
+                            const auto draw_light = [&](float us, float u0, float u1) { return sample_light_configured<TEXTURED>(*sc.self, it, us, u0, u1); };
+                            shade_surface_resampled(cl, it, fr, wo, draw_light, light_tree_of(sc).candidates, depth, u_sel, ul0, ul1, beta, u_lobe, ub0, ub1,
+                                                    contrib, ls.ray_o_tmin, ls.ray_d_tmax, wi, f, pdf);
+                        } else {
+                            shade_surface<false>(cl, it, fr, wo, ls, beta, u_lobe, ub0, ub1, contrib, wi, f, pdf);
+                        }
                     });
                     if (contrib.x != 0.f || contrib.y != 0.f || contrib.z != 0.f) {
                         // a zero (or NaN-free zero) contribution needs no shadow ray; NaNs must reach the film filter

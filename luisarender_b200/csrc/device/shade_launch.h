@@ -9,9 +9,11 @@
 namespace lrk {
 
 // How next-event estimation picks a light and a point on it: the options "light_tree", "light_tree_triangles" (the light tree's
-// bottom level: set with tree only) and "light_solid_angle".  Not part of the ABI.
+// bottom level: set with tree only), "light_solid_angle" and "light_candidates" (M: 0 .. 32, resampling from M candidates for
+// M >= 2).  Not part of the ABI.
 struct LightSampling {
     bool tree{false}, triangles{false}, solid_angle{false};
+    uint32_t candidates{0u};
 };
 
 #define LRK_DECLARE_SHADE_VARIANT(NS)                                                                                                        \

@@ -24,6 +24,10 @@
 //
 // Triangle-level light trees (an extension): `--light-tree-triangles` sets the options "light_tree" and "light_tree_triangles", so
 // that the light tree also picks the emissive triangle by power, distance and orientation.  Surface integrator only, as above.
+//
+// Resampled light sampling (an extension): `--light-candidates <n>` sets lrk_set_option("light_candidates", n) before the upload;
+// for n from 2 to 32, next-event estimation draws n candidates with the light sampling the flags above choose and traces the shadow
+// ray of one, picked by its unshadowed contribution.  0 and 1 keep one light sample.  Surface integrator only, as above.
 #include <sys/stat.h>
 #include <sys/wait.h>
 #include <unistd.h>
@@ -64,6 +68,7 @@ void usage() {
                 "      --adaptive-min-spp <n>   Samples per pixel of the first adaptive round (default 16, at most the camera's spp)\n"
                 "      --denoise                Also write the denoised image to <stem>.denoised<ext> (one GPU only)\n");
     for (const LightFlag &l : kLightFlags) std::printf("      %-25s%s\n", l.flag, l.help);
+    std::printf("      --light-candidates <n>   Resample next-event lights from n candidates (2 to 32; 0 or 1: one light sample)\n");
     std::printf("  -h, --help                   Display this help message\n");
 }
 
@@ -162,7 +167,7 @@ int main(int argc, char *argv[]) {
     int device = -1, gpus = 1;
     bool denoise = false;
     std::vector<const char *> light_options;
-    std::string adaptive_arg, min_spp_arg;
+    std::string adaptive_arg, min_spp_arg, candidates_arg;
     std::vector<std::string> keys, values;
     auto add_macro = [&](const std::string &d) {
         auto p = d.find('=');
@@ -207,6 +212,8 @@ int main(int argc, char *argv[]) {
         else if (auto l = std::find_if(std::begin(kLightFlags), std::end(kLightFlags), [&](const LightFlag &f) { return a == f.flag; });
                  l != std::end(kLightFlags))
             light_options.insert(light_options.end(), l->options.begin(), l->options.end());
+        else if (a == "--light-candidates") candidates_arg = need("count");
+        else if (a.rfind("--light-candidates=", 0) == 0) candidates_arg = a.substr(19);
         else if (a == "-D" || a == "--define") add_macro(need("definition"));
         else if (a.rfind("-D", 0) == 0) add_macro(a.substr(2));
         else if (!a.empty() && a[0] == '-') std::fprintf(stderr, "[warning] Unrecognized options: %s\n", a.c_str());
@@ -242,6 +249,15 @@ int main(int argc, char *argv[]) {
             return -1;
         }
         min_spp = static_cast<uint32_t>(v);
+    }
+    long candidates = -1;// -1: the option is left at its default
+    if (!candidates_arg.empty()) {
+        char *end = nullptr;
+        candidates = std::strtol(candidates_arg.c_str(), &end, 10);
+        if (end == candidates_arg.c_str() || *end != '\0' || candidates < 0 || candidates > 32) {
+            std::fprintf(stderr, "[error] --light-candidates takes a count from 0 to 32, not '%s'.\n", candidates_arg.c_str());
+            return -1;
+        }
     }
     if (denoise && (gpus > 1 || env_u32("WORLD_SIZE", 1u) > 1u)) {
         std::fprintf(stderr, "[error] --denoise renders on one GPU: the G-buffer of sharded renders is not reduced.\n");
@@ -280,6 +296,7 @@ int main(int argc, char *argv[]) {
     if (denoise && lrk_set_option(ctx, "gbuffer", 1) != 0) die(lrk_last_error(ctx));
     for (const char *option : light_options)
         if (lrk_set_option(ctx, option, 1) != 0) die(lrk_last_error(ctx));
+    if (candidates >= 0 && lrk_set_option(ctx, "light_candidates", candidates) != 0) die(lrk_last_error(ctx));
     if (world > 1u) {
         uint8_t id[LRK_COMM_ID_BYTES];
         exchange_comm_id(rank, id);

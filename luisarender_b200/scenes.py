@@ -222,9 +222,12 @@ def many_lights(resolution=(1920, 1080), spp=64, count=48, shared_node=False, sp
 
 
 def near_light(resolution=(512, 512), spp=16, depth=10, rr_depth=0, rr_threshold=0.95, seed=19980810, irradiance=False,
-               output="near_light.exr") -> str:
+               output="near_light.exr", glossy_desk=False) -> str:
     """The frame of solid-angle light sampling (option "light_solid_angle"): a Matte room with a desk under a one-sided 1.0 x 0.6
     panel light 0.3 above the desk top, so that the panel is large and close seen from the desk and the walls next to it.
+
+    ``glossy_desk=True``: the frame of resampled light sampling (option "light_candidates"): the same room with a glossy Disney desk
+    (roughness 0.15, metallic 0.6), whose lobe under the panel decides which light samples matter.
 
     ``irradiance=True``: one one-sided triangle light of emission 4 facing down 0.5 above a Matte plane of albedo 0.5, seen from a
     pinhole 0.3 above the plane looking straight down (the light is behind it), ``depth`` 2: every pixel is (0.5 / pi) * E, E the
@@ -243,7 +246,8 @@ def near_light(resolution=(512, 512), spp=16, depth=10, rr_depth=0, rr_threshold
         camera = "position { 0.0, 0.3, 0.0 }\n  front { 0.0, -1.0, 0.0 }\n  up { 0.0, 0.0, -1.0 }\n  fov { 60.0 }"
         depth = 2
     else:
-        shapes = _matte_room(out, "Light panel_light : Diffuse { emission : Constant { v { 6.0, 5.5, 4.5 } } two_sided { false } }")
+        shapes = _matte_room(out, "Light panel_light : Diffuse { emission : Constant { v { 6.0, 5.5, 4.5 } } two_sided { false } }",
+                             glossy_desk)
         pos, idx = _mesh_props([[(-0.5, 1.0, -0.1), (-0.5, 1.0, -0.7), (0.5, 1.0, -0.7), (0.5, 1.0, -0.1)]])  # facing down
         out.append(f"Shape panel : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} light {{ @panel_light }} }}")
         shapes.append("@panel")
@@ -254,12 +258,17 @@ def near_light(resolution=(512, 512), spp=16, depth=10, rr_depth=0, rr_threshold
 _MATTE_ROOM_CAMERA = "position { 0.0, 1.1, 3.4 }\n  front { 0.0, -0.08, -1.0 }\n  up { 0.0, 1.0, 0.0 }\n  fov { 38.0 }"
 
 
-def _matte_room(out, light_line):
+def _matte_room(out, light_line, glossy_desk=False):
     """The Matte room of ``near_light`` and ``emissive_globe``: its surfaces, the Light node ``light_line``, then its walls and desk.
-    Returns the shape references."""
+    ``glossy_desk``: the desk is a glossy Disney surface of the same colour.  Returns the shape references."""
     colors = {"white": (0.725, 0.710, 0.680), "green": (0.140, 0.450, 0.091), "red": (0.630, 0.065, 0.050), "desk": (0.55, 0.45, 0.35)}
     for name, rgb in colors.items():
-        out.append(f"Surface {name} : Matte {{ Kd : Constant {{ v {{ {_fmt(rgb[0])}, {_fmt(rgb[1])}, {_fmt(rgb[2])} }} }} }}")
+        color = f"{_fmt(rgb[0])}, {_fmt(rgb[1])}, {_fmt(rgb[2])}"
+        if name == "desk" and glossy_desk:
+            out.append(f"Surface desk : Disney {{ color : Constant {{ v {{ {color} }} }} metallic : Constant {{ v {{ 0.6 }} }} "
+                       f"roughness : Constant {{ v {{ 0.15 }} }} }}")
+        else:
+            out.append(f"Surface {name} : Matte {{ Kd : Constant {{ v {{ {color} }} }} }}")
     out.append(light_line)
     x0, x1, y0, y1, z0, z1 = -1.0, 1.0, 0.0, 2.0, -1.0, 1.0
     quads = {  # (name, surface, [4 vertices])

@@ -1,6 +1,6 @@
 """Next-event light sampling options against what they replace, on cuda:0.  Prints one JSON line.
 
-    python tools/bench_light_sampling.py --compare {tree,solid_angle,triangles} [--spp 64] [--reference-spp 4096]
+    python tools/bench_light_sampling.py --compare {tree,solid_angle,triangles,candidates} [--spp 64] [--reference-spp 4096]
 
 A frame's comparison: a reference of `--reference-spp` samples of the indices [SPP, SPP + reference) rendered with the setting under
 test, then alternately, twice each, the renders of [0, SPP) under every setting of the comparison.  Device time (lrk_stats::
@@ -18,6 +18,10 @@ one over that of the other, since the error of an unbiased render falls as 1 / s
     frame, the emissive globe (scenes.emissive_globe, 1024x1024, one level-5 sphere), C3 (1920x1080 @1024 by its own count) and
     near_light (1024x1024, one quad).  Also the host time of lrk_upload_scene with the option off and on (light_tree on in both),
     for the many-light frame and for the globe at subdivision 7 (327 680 emissive triangles): the bottom trees are built there.
+  * candidates (option "light_candidates" M = 2, 4, 8 against M = 1, one light sample; the reference at M = 8): C3 (1920x1080: Disney
+    spheres, two quads), C2's Cornell box (1024x1024), near_light (1024x1024), near_light with its glossy Disney desk (1024x1024:
+    the frame where the closure decides which light samples matter) and the many-light frame (1920x1080) with the light tree on
+    in every setting.
 The card's name and power limit are read in the same run.
 """
 from __future__ import annotations
@@ -121,7 +125,21 @@ def compare_triangles(r, desc, spp: int, ref_spp: int) -> dict:
                           "globe_subdivision_7": upload_ms(r, desc(scenes.emissive_globe(resolution=(64, 64), spp=1, subdivision=7)))}}
 
 
-COMPARE = {"tree": compare_tree, "solid_angle": compare_solid_angle, "triangles": compare_triangles}
+def compare_candidates(r, desc, spp: int, ref_spp: int) -> dict:
+    from luisarender_b200 import scenes
+
+    def candidates_frame(src, light_tree=False):
+        settings = {f"m{m}": {"light_tree": int(light_tree), "light_candidates": m} for m in (1, 2, 4, 8)}
+        return frame(r, desc(src), settings, "m1", spp, ref_spp, light_tree=light_tree)
+
+    return {"c3": candidates_frame(scenes.instanced_spheres(resolution=(1920, 1080), spp=spp, seed=1)),
+            "c2_cornell": candidates_frame(scenes.cornell_box(resolution=(1024, 1024), spp=spp)),
+            "near_light": candidates_frame(scenes.near_light(resolution=(1024, 1024), spp=spp)),
+            "glossy_desk": candidates_frame(scenes.near_light(resolution=(1024, 1024), spp=spp, glossy_desk=True)),
+            "many_lights_tree": candidates_frame(scenes.many_lights(resolution=(1920, 1080), spp=spp), light_tree=True)}
+
+
+COMPARE = {"tree": compare_tree, "solid_angle": compare_solid_angle, "triangles": compare_triangles, "candidates": compare_candidates}
 
 
 def main():
