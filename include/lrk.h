@@ -587,7 +587,15 @@ int lrk_reduce_film(lrk_ctx *ctx, uint32_t root);
  *                             at the cost of M light samples and M closure evaluations per vertex.  0 (the default) and 1: one
  *                             light sample, as without the option.  Read at lrk_upload_scene; another value ->
  *                             LRK_ERR_INVALID_ARGUMENT.  Surface integrator only: lrk_upload_scene returns LRK_ERR_UNSUPPORTED for
- *                             the volume integrator with M >= 2.  LRK_ABI_VERSION stays 8: no layout or signature changed */
+ *                             the volume integrator with M >= 2.  LRK_ABI_VERSION stays 8: no layout or signature changed
+ *   "light_receiver" (0/1)    receiver-aware light sampling: the geometric normal of the shading point (on the side the path
+ *                             leaves from) enters the light tree's importance (pbrt-v4's cos theta'_i term; lights wholly behind a
+ *                             reflect-only surface get probability 0) and warps the solid-angle sampler's points towards its
+ *                             cosine (pbrt-v4's bilinear warp).  Each path carries the normal as a 32-bit word, so that emitter hits
+ *                             weigh with the pdf the light sample had.  Read at lrk_upload_scene; another value ->
+ *                             LRK_ERR_INVALID_ARGUMENT; on without "light_tree" or "light_solid_angle" -> LRK_ERR_INVALID_ARGUMENT
+ *                             at lrk_upload_scene.  Combines with "light_tree_triangles" and "light_candidates".  Surface
+ *                             integrator only, as "light_tree".  LRK_ABI_VERSION stays 8: no layout or signature changed */
 int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value);
 
 int lrk_film_clear(lrk_ctx *ctx);

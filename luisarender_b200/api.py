@@ -101,16 +101,21 @@ class Renderer:
     triangle of the chosen emitter, from a tree over its mesh's triangles, instead of by area.
     ``light_candidates=M`` (an int from 0 to 32) sets the option "light_candidates": for M >= 2, from the next upload on,
     next-event estimation draws M candidates from the light sampling above and traces the shadow ray of one, chosen by its
-    unshadowed contribution (resampled importance sampling; surface integrator only).  0 and 1 keep one light sample per vertex."""
+    unshadowed contribution (resampled importance sampling; surface integrator only).  0 and 1 keep one light sample per vertex.
+    ``light_receiver=True`` (with ``light_tree=True`` or ``light_solid_angle=True``) sets the option "light_receiver": the light tree
+    and the solid-angle sampler also weigh lights and points by the shading point's normal."""
 
     def __init__(self, device_index: int = -1, max_paths_per_pass: int = 0, light_tree: bool = False, light_solid_angle: bool = False,
-                 light_tree_triangles: bool = False, light_candidates: int = 1):
-        light_options = {"light_tree": light_tree, "light_solid_angle": light_solid_angle, "light_tree_triangles": light_tree_triangles}
+                 light_tree_triangles: bool = False, light_candidates: int = 1, light_receiver: bool = False):
+        light_options = {"light_tree": light_tree, "light_solid_angle": light_solid_angle, "light_tree_triangles": light_tree_triangles,
+                         "light_receiver": light_receiver}
         for name, value in light_options.items():
             if value not in (0, 1):
                 raise ValueError(f"{name} is False or True, not {value!r}")
         if light_tree_triangles and not light_tree:
             raise ValueError("light_tree_triangles is the bottom level of the light tree: it needs light_tree=True")
+        if light_receiver and not (light_tree or light_solid_angle):
+            raise ValueError("light_receiver refines the light tree and solid-angle sampling: it needs light_tree=True or light_solid_angle=True")
         if type(light_candidates) is not int or not 0 <= light_candidates <= 32:
             raise ValueError(f"light_candidates is an int from 0 to 32, not {light_candidates!r}")
         self._lib = F.device_lib()

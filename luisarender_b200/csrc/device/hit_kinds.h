@@ -42,6 +42,14 @@ LRK_HIT_KINDS_FN uint32_t hit_kind_of(const lrk_surface &s) {
 // and thin Disney.  constexpr: the fast variant of shade.cu does not compile these kinds' kernels.
 LRK_HIT_KINDS_FN constexpr bool hit_kind_always_strict(uint32_t kind) { return (kind >= kHitMirror && kind <= kHitMix) || kind >= kHitLayered; }
 
+// Kinds whose closure returns f = 0 and pdf = 0 for every direction on the other side of the geometric normal from the outgoing one
+// (reflection only, and validate_surface_sides ties the shading frame's sides to the geometric normal's): their receiver word carries
+// the one-sided bit of the option "light_receiver" (receiver.h).  tests/test_light_receiver_cpu.py evaluates each kind's closure
+// on the host with wi behind ng.
+LRK_HIT_KINDS_FN constexpr bool hit_kind_one_sided(uint32_t kind) {
+    return kind == kHitMatte || kind == kHitDisney || kind == kHitMirror || kind == kHitPlastic || kind == kHitMetal;
+}
+
 // Calls f(std::integral_constant<uint32_t, kind>{}): the run-time kind as a compile-time one.  Host and device code call it with
 // their own kind of f.
 #ifdef __CUDACC__

@@ -10,6 +10,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "receiver.h"
+
 #ifdef __CUDACC__
 #define LRK_LIGHT_TREE_FN __host__ __device__ __forceinline__
 #else
@@ -34,9 +36,18 @@ static_assert(sizeof(LightTreeNode) == 48, "light tree node is 48 B");
 
 LRK_LIGHT_TREE_FN float light_tree_dequantize_cos(uint32_t q) { return 2.f * (static_cast<float>(q & 0xffffu) * (1.f / 32767.f)) - 1.f; }
 
-// pbrt-v4's LightBounds::Importance without the receiver-normal factor.  Conservative: 0 only when no point of the node's bounds
-// emits towards p.  p inside the bounding sphere of the bounds skips the orientation test; the cone angles are padded at the build.
-LRK_LIGHT_TREE_FN float light_tree_importance(const LightTreeNode &n, float px, float py, float pz) {
+// The receiver term's cull pad (option "light_receiver"): a one-sided receiver culls a node only when its bounding sphere lies behind
+// the receiver's plane by more than this angle, seen from p.  It covers the octahedral rounding of the normal (below 2e-4 rad,
+// receiver.h) and an evaluation point that is not the sampling point: an emitter hit evaluates the pmf from the offset ray origin,
+// a light sample from the surface point, which lie within 1 % of the distance to the node of each other.
+constexpr float kLightTreeReceiverPadSin = 0.01f;// sin of the pad
+
+// pbrt-v4's LightBounds::Importance.  Conservative: 0 only when no point of the node's bounds emits towards p (or, for a one-sided
+// receiver, lies in front of it).  p inside the bounding sphere of the bounds skips the orientation and receiver tests; the cone
+// angles are padded at the build.  The receiver term cos theta'_i = cos(max(theta_i - theta_b, 0)), theta_i the angle between the
+// receiver's normal and the direction to the node's centre: |cos theta_i| for a two-sided receiver, as pbrt-v4; none (the
+// expressions without it) for kReceiverNone.
+LRK_LIGHT_TREE_FN float light_tree_importance(const LightTreeNode &n, float px, float py, float pz, const Receiver &rcv = Receiver{0.f, 0.f, 0.f, kReceiverNone}) {
     const float ex = n.hi[0] - n.lo[0], ey = n.hi[1] - n.lo[1], ez = n.hi[2] - n.lo[2];
     const float dx = px - 0.5f * (n.lo[0] + n.hi[0]), dy = py - 0.5f * (n.lo[1] + n.hi[1]), dz = pz - 0.5f * (n.lo[2] + n.hi[2]);
     const float dist2 = dx * dx + dy * dy + dz * dz;
@@ -58,15 +69,28 @@ LRK_LIGHT_TREE_FN float light_tree_importance(const LightTreeNode &n, float px, 
         if (cos_p <= light_tree_dequantize_cos(n.cos_q >> 16u)) return 0.f;
     }
     const float d2 = fmaxf(dist2, 0.5f * sqrtf(diag2));
-    return n.phi * fmaxf(cos_p, kLightTreeMinCos) / d2;
+    if (rcv.kind == kReceiverNone) return n.phi * fmaxf(cos_p, kLightTreeMinCos) / d2;
+    float cos_r = 1.f;
+    if (dist2 > r2) {
+        const float inv_d = 1.f / sqrtf(dist2);
+        const float sin2_b = r2 / dist2;
+        const float cos_b = sqrtf(fmaxf(1.f - sin2_b, 0.f)), sin_b = sqrtf(sin2_b);
+        float cos_i = fminf(fmaxf(-(rcv.x * dx + rcv.y * dy + rcv.z * dz) * inv_d, -1.f), 1.f);
+        if (rcv.kind == kReceiverTwoSided) cos_i = fabsf(cos_i);
+        const float sin_i = sqrtf(fmaxf(1.f - cos_i * cos_i, 0.f));
+        cos_r = cos_i > cos_b ? 1.f : cos_i * cos_b + sin_i * sin_b;
+        if (cos_r < -kLightTreeReceiverPadSin) return 0.f;// one-sided only: cos_i >= 0 for a two-sided receiver
+    }
+    return n.phi * fmaxf(cos_p, kLightTreeMinCos) * fmaxf(cos_r, kLightTreeMinCos) / d2;
 }
 
 // The descent from the root.  SAMPLE: chooses with u in [0, 1) and returns the light; otherwise follows `trail` (bit d = 1: the
 // second child at depth d) and returns the leaf's light.  pmf: the probability of that choice, 0 with kLightTreeNone.  u_left: where
-// not null, receives u as the sampling descent left it at the leaf, remapped to [0, 1) by every choice on the way.
+// not null, receives u as the sampling descent left it at the leaf, remapped to [0, 1) by every choice on the way.  rcv: the receiver
+// of light_tree_importance (option "light_receiver"), the same for the sample and the evaluation of one point.
 template<bool SAMPLE>
 LRK_LIGHT_TREE_FN uint32_t light_tree_walk(const LightTreeNode *nodes, float px, float py, float pz, float u, unsigned long long trail, float &pmf,
-                                           float *u_left = nullptr) {
+                                           float *u_left = nullptr, const Receiver &rcv = Receiver{0.f, 0.f, 0.f, kReceiverNone}) {
     pmf = 1.f;
     uint32_t i = 0u;
     for (;;) {
@@ -75,7 +99,7 @@ LRK_LIGHT_TREE_FN uint32_t light_tree_walk(const LightTreeNode *nodes, float px,
             if (u_left != nullptr) *u_left = u;
             return index & ~kLightTreeLeaf;
         }
-        const float il = light_tree_importance(nodes[index], px, py, pz), ir = light_tree_importance(nodes[index + 1u], px, py, pz);
+        const float il = light_tree_importance(nodes[index], px, py, pz, rcv), ir = light_tree_importance(nodes[index + 1u], px, py, pz, rcv);
         const float total = il + ir;
         if (!(total > 0.f)) {
             pmf = 0.f;
@@ -97,7 +121,8 @@ LRK_LIGHT_TREE_FN uint32_t light_tree_walk(const LightTreeNode *nodes, float px,
 
 // The bottom level of the option "light_tree_triangles": one tree per emissive mesh over its triangles, in the mesh's object space.
 // The shading point enters it mapped by the instance's world-to-object rows w2o (row-major 3x4) with the expressions traversal uses
-// (traverse.cuh); facing is invariant under that map, so the orientation cull stays conservative for any invertible transform.
+// (traverse.cuh); facing is invariant under that map, so the orientation cull stays conservative for any invertible transform.  A
+// receiver enters it through receiver_to_object (receiver.h), which keeps the side of its plane for the same reason.
 LRK_LIGHT_TREE_FN void light_tree_object_point(const float *w2o, float px, float py, float pz, float &qx, float &qy, float &qz) {
     qx = fmaf(w2o[0], px, fmaf(w2o[1], py, fmaf(w2o[2], pz, w2o[3])));
     qy = fmaf(w2o[4], px, fmaf(w2o[5], py, fmaf(w2o[6], pz, w2o[7])));
@@ -106,9 +131,10 @@ LRK_LIGHT_TREE_FN void light_tree_object_point(const float *w2o, float px, float
 
 // pmf of triangle `prim` of a bottom tree at object-space point q, following its trail.  A triangle the build left out (no area)
 // has trail 0, which leads to another triangle's leaf: pmf 0.
-LRK_LIGHT_TREE_FN float light_tree_triangle_pmf_at(const LightTreeNode *nodes, float qx, float qy, float qz, unsigned long long trail, uint32_t prim) {
+LRK_LIGHT_TREE_FN float light_tree_triangle_pmf_at(const LightTreeNode *nodes, float qx, float qy, float qz, unsigned long long trail, uint32_t prim,
+                                                   const Receiver &rcv = Receiver{0.f, 0.f, 0.f, kReceiverNone}) {
     float pmf;
-    return light_tree_walk<false>(nodes, qx, qy, qz, 0.f, trail, pmf) == prim ? pmf : 0.f;
+    return light_tree_walk<false>(nodes, qx, qy, qz, 0.f, trail, pmf, nullptr, rcv) == prim ? pmf : 0.f;
 }
 
 }// namespace lrk

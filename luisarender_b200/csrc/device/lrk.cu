@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <chrono>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <limits>
@@ -142,9 +143,11 @@ struct lrk_ctx {
     bool gbuffer_option{false}, gbuffer_film{false};
     DeviceBuffer d_gb_albedo, d_gb_normal, d_gb_hits;// per pixel (sum albedo, S), (sum n, sum t), H
     DeviceBuffer d_dn_albedo_cov, d_dn_normal_depth, d_dn_variance, d_dn_ping[2];// lrk_denoise / lrk_download_gbuffer scratch
-    // next-event light sampling: light_requested holds the options "light_tree", "light_tree_triangles" and "light_solid_angle";
-    // lrk_upload_scene latches it into light_active, which selects the shade kernels' instantiations (upload_light_sampling)
+    // next-event light sampling: light_requested holds the options "light_tree", "light_tree_triangles", "light_solid_angle",
+    // "light_candidates" and "light_receiver"; lrk_upload_scene latches it into light_active, which selects the shade kernels'
+    // instantiations (upload_light_sampling)
     LightSampling light_requested, light_active;
+    uint32_t *receiver_words{nullptr};// in path_allocs while light_active.receiver (alloc_paths)
 
     ~lrk_ctx();
 };
@@ -198,12 +201,26 @@ int upload(lrk_ctx *ctx, DeviceBuffer &dst, const T *src, size_t count) {
     return LRK_OK;
 }
 
+// The receiver words' pointer in the record after the scene (DeviceLightTree::receiver): the path array while the option
+// "light_receiver" is active, else null.
+int write_receiver_record(lrk_ctx *ctx) {
+    if (ctx->arrays.scene_copy.get() == nullptr) return LRK_OK;
+    uint32_t *words = ctx->light_active.receiver ? ctx->receiver_words : nullptr;
+    LRK_CUDA(cudaMemcpyAsync(ctx->arrays.scene_copy.get<char>() + sizeof(DeviceScene) + offsetof(DeviceLightTree, receiver), &words, sizeof(words),
+                             cudaMemcpyHostToDevice, ctx->stream));
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));// `words` is a local
+    return LRK_OK;
+}
+
 int alloc_paths(lrk_ctx *ctx, uint64_t capacity) {
     const uint32_t kinds = ctx->used_kinds | 7u;// buckets 0..2 always, the others only for scenes that use them
-    if (ctx->capacity >= capacity && (!ctx->volume || ctx->volume_capacity >= capacity) && (ctx->allocated_kinds & kinds) == kinds) return LRK_OK;
+    if (ctx->capacity >= capacity && (!ctx->volume || ctx->volume_capacity >= capacity) && (ctx->allocated_kinds & kinds) == kinds &&
+        (!ctx->light_active.receiver || ctx->receiver_words != nullptr))
+        return LRK_OK;
     // all of the old path state is freed before any of the new one is allocated
     ctx->path_allocs.clear();
     ctx->pb = PathBuffers{};// no dangling pointers: lrk_film_clear / lrk_get_stats look at pb.stats
+    ctx->receiver_words = nullptr;
     ctx->capacity = 0;
     ctx->volume_capacity = 0;
     ctx->allocated_kinds = 0u;
@@ -244,6 +261,10 @@ int alloc_paths(lrk_ctx *ctx, uint64_t capacity) {
         LRK_CUDA(alloc(pb.occl1, capacity));
         LRK_CUDA(alloc(pb.s2_target, capacity));
         ctx->volume_capacity = capacity;
+    }
+    if (ctx->light_active.receiver) {// only while the option is active; the kernels find them through the scene's record
+        LRK_CUDA(alloc(ctx->receiver_words, capacity));
+        return write_receiver_record(ctx);
     }
     return LRK_OK;
 }
@@ -677,6 +698,7 @@ bool LightSampling::*light_sampling_option(const std::string &name) {
     if (name == "light_tree") return &LightSampling::tree;
     if (name == "light_tree_triangles") return &LightSampling::triangles;
     if (name == "light_solid_angle") return &LightSampling::solid_angle;
+    if (name == "light_receiver") return &LightSampling::receiver;
     return nullptr;
 }
 
@@ -697,6 +719,12 @@ int check_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
         return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: resampled next-event estimation (option light_candidates >= 2) serves the surface "
                                               "integrator only; the volume integrator traces every light sample it draws, since the "
                                               "occlusion of each advances its random stream");
+    if (want.receiver && volume)
+        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: receiver-aware light sampling (option light_receiver) serves the surface integrator "
+                                              "only; the volume integrator selects its lights uniformly by area");
+    if (want.receiver && !want.tree && !want.solid_angle)
+        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: receiver-aware light sampling (option light_receiver) refines the light tree "
+                                                   "and solid-angle sampling: set the option light_tree or light_solid_angle too");
     return LRK_OK;
 }
 
@@ -738,6 +766,9 @@ int upload_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
     rec.select = want.tree ? kLightSelectTree : kLightSelectUniform;
     rec.point = want.solid_angle ? kLightPointSolidAngle : kLightPointArea;
     rec.candidates = want.candidates;
+    if (want.receiver) {// null until alloc_paths allocates them (it then writes them here)
+        rec.receiver = ctx->receiver_words;
+    }
     LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get<char>() + sizeof(DeviceScene), &rec, sizeof(DeviceLightTree), cudaMemcpyHostToDevice, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));// the host arrays and `rec` are locals
     ctx->light_active = want;

@@ -86,6 +86,10 @@ struct DeviceLightTree {
     // The light sampling as the resampling shade kernels read it at run time (option "light_candidates" >= 2; the other kernels
     // have it as template values): LightSelect, LightPoint (shading.cuh) and the candidate count M.
     uint32_t select, point, candidates;
+    // The receiver words (option "light_receiver", receiver.h): one per path, indexed by its generation slot (id_rng.x); null unless
+    // the option was on at lrk_upload_scene.  The shade kernels of the tree and solid-angle light samplings and the resampling ones
+    // read the word of the previous vertex at the emitter hit, then overwrite it with their own where they sample a light.
+    uint32_t *receiver;
 };
 __device__ __forceinline__ const DeviceLightTree &light_tree_of(const DeviceScene &sc) {
     return *reinterpret_cast<const DeviceLightTree *>(sc.self + 1);

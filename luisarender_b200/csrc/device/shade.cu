@@ -40,13 +40,19 @@ int grid_of(Kernel kernel, int block, int sm_count) {
 // calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection, light point sampling), or with the
 // kind's resampling instantiation (RESAMPLE; none for emitter-only hits).  The fast variant has none for the kinds that always run
 // in strict arithmetic (hit_kind_always_strict): render_pass never launches them there.
-template<uint32_t SEL, uint32_t PT, bool RESAMPLE = false, typename F>
+template<uint32_t SEL, uint32_t PT, bool RESAMPLE = false, bool RECEIVER = false, typename F>
 void with_shade_kernel(uint32_t kind, bool textured, F &&f) {
     with_hit_kind(kind, [&](auto k) {
         constexpr uint32_t K = decltype(k)::value;
         if constexpr (!(kFastVariant && hit_kind_always_strict(K)) && !(RESAMPLE && K == kHitEmitter))
-            textured ? f(shade_kernel<K, true, SEL, PT, RESAMPLE>) : f(shade_kernel<K, false, SEL, PT, RESAMPLE>);
+            textured ? f(shade_kernel<K, true, SEL, PT, RESAMPLE, RECEIVER>) : f(shade_kernel<K, false, SEL, PT, RESAMPLE, RECEIVER>);
     });
+}
+// the light sampling <SEL, PT> with or without the option "light_receiver"
+template<uint32_t SEL, uint32_t PT, typename F>
+void with_light_kernel(uint32_t kind, bool textured, bool receiver, F &&f) {
+    if (receiver) with_shade_kernel<SEL, PT, false, true>(kind, textured, f);
+    else with_shade_kernel<SEL, PT>(kind, textured, f);
 }
 
 // the volume integrator's surface step exists for the kinds of config C4's closures: emitter-only, Matte and Disney
@@ -81,12 +87,13 @@ void launch_shade(uint32_t kind, bool textured, const LightSampling &light, int 
                   const PathBuffers &pb, uint32_t depth) {
     const auto launch = [&](auto kernel) { kernel<<<blocks, kShadeBlock, 0, stream>>>(sc, pb, depth); };
     if (light.candidates >= 2u && kind != kHitEmitter) {
-        with_shade_kernel<kLightSelectUniform, kLightPointArea, true>(kind, textured, launch);
+        if (light.receiver) with_shade_kernel<kLightSelectUniform, kLightPointArea, true, true>(kind, textured, launch);
+        else with_shade_kernel<kLightSelectUniform, kLightPointArea, true>(kind, textured, launch);
     } else if (light.solid_angle) {
-        if (light.tree) with_shade_kernel<kLightSelectTree, kLightPointSolidAngle>(kind, textured, launch);
-        else with_shade_kernel<kLightSelectUniform, kLightPointSolidAngle>(kind, textured, launch);
+        if (light.tree) with_light_kernel<kLightSelectTree, kLightPointSolidAngle>(kind, textured, light.receiver, launch);
+        else with_light_kernel<kLightSelectUniform, kLightPointSolidAngle>(kind, textured, light.receiver, launch);
     } else {
-        if (light.tree) with_shade_kernel<kLightSelectTree, kLightPointArea>(kind, textured, launch);
+        if (light.tree) with_light_kernel<kLightSelectTree, kLightPointArea>(kind, textured, light.receiver, launch);
         else with_shade_kernel<kLightSelectUniform, kLightPointArea>(kind, textured, launch);
     }
 }

@@ -68,13 +68,56 @@ __device__ __noinline__ LightEval evaluate_hit_configured(const DeviceScene &sc,
                                              : evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointArea>(sc, it, p_from, inst);
 }
 
+// The same for the resampling kernels of the option "light_receiver": `path`, the path's generation slot, where receiver_store left
+// the vertex's receiver word.
+template<bool TEXTURED>
+__device__ __noinline__ LightSample sample_light_configured_receiver(const DeviceScene &sc, const Interaction &it, float u_sel, float u0, float u1,
+                                                                     uint32_t path) {
+    if (sc.light_count == 0u && sc.env_prob == 0.f) {
+        LightSample ls;
+        ls.eval.L = v3(0.f);
+        ls.eval.pdf = 0.f;
+        ls.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
+        ls.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
+        return ls;
+    }
+    const DeviceLightTree &lt = light_tree_of(sc);
+    if (lt.select == kLightSelectTree)
+        return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectTree, kLightPointSolidAngle, true>(sc, it, u_sel, u0, u1, path)
+                                                 : sample_light<TEXTURED, kLightSelectTree, kLightPointArea, true>(sc, it, u_sel, u0, u1, path);
+    return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectUniform, kLightPointSolidAngle, true>(sc, it, u_sel, u0, u1, path)
+                                             : sample_light<TEXTURED, kLightSelectUniform, kLightPointArea>(sc, it, u_sel, u0, u1);
+}
+template<bool TEXTURED>
+__device__ __noinline__ LightEval evaluate_hit_configured_receiver(const DeviceScene &sc, const Interaction &it, V3 p_from, uint32_t inst, uint32_t path) {
+    const DeviceLightTree &lt = light_tree_of(sc);
+    if (lt.select == kLightSelectTree)
+        return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectTree, kLightPointSolidAngle, true>(sc, it, p_from, inst, path)
+                                                 : evaluate_hit<TEXTURED, kLightSelectTree, kLightPointArea, true>(sc, it, p_from, inst, path);
+    return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointSolidAngle, true>(sc, it, p_from, inst, path)
+                                             : evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointArea>(sc, it, p_from, inst);
+}
+
+// The receiver word of a surface vertex (option "light_receiver", receiver.h): its geometric normal on the side wo leaves from, with
+// the one-sided bit of its closure kind, stored at the path's generation slot `path` (light_tree_of(sc).receiver) for the light
+// samples of this vertex and the emitter hit of the next depth (receiver_word_of).  Out of line, like the light sampling it feeds.
+__device__ __noinline__ inline void receiver_store(const DeviceScene &sc, uint32_t path, V3 ng, V3 wo, bool one_sided) {
+    const V3 n = dot(wo, ng) < 0.f ? -ng : ng;
+    light_tree_of(sc).receiver[path] = receiver_encode(n.x, n.y, n.z, one_sided);
+}
+
 // Sorted-by-material dispatch, step 2: one shade kernel per closure kind, each over its own hit bucket.  SEL: the light selection
 // of next-event estimation (kLightSelectTree with the option "light_tree"); PT: its point sampling (kLightPointSolidAngle with the
 // option "light_solid_angle").  RESAMPLE: resampled next-event estimation (option "light_candidates" >= 2, every kind but
 // emitter-only): the light sampling and the candidate count come from light_tree_of(sc) at run time instead of SEL and PT.
-template<uint32_t KIND, bool TEXTURED = false, uint32_t SEL = kLightSelectUniform, uint32_t PT = kLightPointArea, bool RESAMPLE = false>
+// RECEIVER: the option "light_receiver" (receiver.h) with SEL or PT, or with RESAMPLE: its own instantiations, so that the others
+// keep their code.
+template<uint32_t KIND, bool TEXTURED = false, uint32_t SEL = kLightSelectUniform, uint32_t PT = kLightPointArea, bool RESAMPLE = false,
+         bool RECEIVER = false>
 __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kernel(DeviceScene sc, PathBuffers pb, uint32_t depth) {
     static_assert(!RESAMPLE || (KIND != kHitEmitter && SEL == kLightSelectUniform && PT == kLightPointArea), "one resampling kernel per kind");
+    static_assert(!RECEIVER || RESAMPLE || SEL == kLightSelectTree || PT == kLightPointSolidAngle, "the receiver refines the tree or solid angle");
+    constexpr bool kReceiver = RECEIVER;
     // the compaction is written out here rather than through block_append, which raises registers or spills of most instantiations
     __shared__ uint32_t s_warp_next[kShadeBlock / 32], s_warp_shadow[kShadeBlock / 32];
     __shared__ uint32_t s_base_next, s_base_shadow;
@@ -103,7 +146,10 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                 // emitter hit with MIS: mega_path.cpp:80-87, uniform.cpp:50-65
                 if (sc.light_count != 0u && it.shape.has_light()) {
                     LightEval e;
-                    if constexpr (RESAMPLE) e = evaluate_hit_configured<TEXTURED>(*sc.self, it, v3(ro.x, ro.y, ro.z), hit.x);
+                    const uint32_t path = depth != 0u ? ir.x : kNoReceiverPath;// the receiver word of the vertex the ray left
+                    if constexpr (RESAMPLE && kReceiver) e = evaluate_hit_configured_receiver<TEXTURED>(*sc.self, it, v3(ro.x, ro.y, ro.z), hit.x, path);
+                    else if constexpr (RESAMPLE) e = evaluate_hit_configured<TEXTURED>(*sc.self, it, v3(ro.x, ro.y, ro.z), hit.x);
+                    else if constexpr (kReceiver) e = evaluate_hit<TEXTURED, SEL, PT, true>(sc, it, v3(ro.x, ro.y, ro.z), hit.x, path);
                     else e = evaluate_hit<TEXTURED, SEL, PT>(sc, it, v3(ro.x, ro.y, ro.z), hit.x);
                     V3 add = beta * e.L * balance_heuristic(pdf_bsdf, e.pdf);
                     float4 li = pb.li[ir.x];
@@ -134,15 +180,23 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                     ls.eval.pdf = 0.f;
                     ls.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
                     ls.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
-                    if constexpr (!RESAMPLE)
+                    if constexpr (kReceiver) {// the word goes to memory here; the light sampling reads it back through the path's slot
+                        if (light_tree_of(sc).receiver != nullptr) receiver_store(*sc.self, ir.x, it.ng, wo, hit_kind_one_sided(KIND));
+                        if constexpr (!RESAMPLE)
+                            if (sc.light_count != 0u || sc.env_prob != 0.f) ls = sample_light<TEXTURED, SEL, PT, true>(sc, it, u_sel, ul0, ul1, ir.x);
+                    } else if constexpr (!RESAMPLE) {
                         if (sc.light_count != 0u || sc.env_prob != 0.f) ls = sample_light<TEXTURED, SEL, PT>(sc, it, u_sel, ul0, ul1);
+                    }
                     const lrk_surface *surf = sc.surfaces + it.shape.surface_tag;
                     V3 contrib, wi, f;
                     float pdf;
                     const float eta_scale = with_hit_closure<KIND, TEXTURED>(sc, surf, it, wo, [&] { return closure_frame<TEXTURED>(sc, surf, it, wo); },
                                                                            [&](auto &cl, const Frame &fr) {
                         if constexpr (RESAMPLE) {
-                            const auto draw_light = [&](float us, float u0, float u1) { return sample_light_configured<TEXTURED>(*sc.self, it, us, u0, u1); };
+                            const auto draw_light = [&](float us, float u0, float u1) {
+                                if constexpr (kReceiver) return sample_light_configured_receiver<TEXTURED>(*sc.self, it, us, u0, u1, ir.x);
+                                else return sample_light_configured<TEXTURED>(*sc.self, it, us, u0, u1);
+                            };
                             shade_surface_resampled(cl, it, fr, wo, draw_light, light_tree_of(sc).candidates, depth, u_sel, ul0, ul1, beta, u_lobe, ub0, ub1,
                                                     contrib, ls.ray_o_tmin, ls.ray_d_tmax, wi, f, pdf);
                         } else {

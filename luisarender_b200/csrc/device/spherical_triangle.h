@@ -114,4 +114,91 @@ LRK_SPHERICAL_FN SphVec sample_spherical_triangle(SphVec p, SphVec v0, SphVec v1
     return spherical_barycentrics(p, v0, v1, v2, sample_spherical_direction(p, v0, v1, v2, omega, u0, u1));
 }
 
+// ---- the receiver-cosine warp of the option "light_receiver" (DESIGN.md §4 (Receiver-aware light sampling)) -------------------------
+// pbrt-v4's Triangle::Sample with a receiver normal n: (u0, u1) is first warped by a bilinear density whose corner weights are
+// max(0.01, |n . w_k|) for the unit directions w_k to the vertices the corners map to (u1 = 0: v1; (0, 1): v0; (1, 1): v2), so that the
+// points follow the receiver's cosine roughly.  The pdf of a point is pdf[tri] / omega * spherical_warp_pdf(...) at the (u0, u1)
+// that pbrt-v4's InvertSphericalTriangleSample recovers from the point: the one function a sample and an emitter hit both call.
+
+struct SphWarp {
+    float w[4];// corner weights of (0, 0), (1, 0), (0, 1), (1, 1)
+};
+
+LRK_SPHERICAL_FN SphWarp spherical_warp_weights(SphVec p, SphVec n, SphVec v0, SphVec v1, SphVec v2) {
+    using namespace spherical_detail;
+    const float wa = fmaxf(0.01f, fabsf(dot(n, normalize(sub(v0, p)))));
+    const float wb = fmaxf(0.01f, fabsf(dot(n, normalize(sub(v1, p)))));
+    const float wc = fmaxf(0.01f, fabsf(dot(n, normalize(sub(v2, p)))));
+    return {{wb, wb, wa, wc}};
+}
+
+namespace spherical_detail {
+LRK_SPHERICAL_FN float lerp_t(float t, float a, float b) { return (1.f - t) * a + t * b; }
+// pbrt-v4's SampleLinear: x in [0, 1) with density proportional to lerp(x, a, b)
+LRK_SPHERICAL_FN float sample_linear(float u, float a, float b) {
+    if (u == 0.f && a == 0.f) return 0.f;
+    const float x = u * (a + b) / (a + sqrtf(lerp_t(u, a * a, b * b)));
+    return fminf(x, 0x1.fffffep-1f);
+}
+}// namespace spherical_detail
+
+// pbrt-v4's SampleBilinear and BilinearPDF
+LRK_SPHERICAL_FN void sample_bilinear(const SphWarp &w, float &u0, float &u1) {
+    using namespace spherical_detail;
+    const float y = sample_linear(u1, w.w[0] + w.w[1], w.w[2] + w.w[3]);
+    const float x = sample_linear(u0, lerp_t(y, w.w[0], w.w[2]), lerp_t(y, w.w[1], w.w[3]));
+    u0 = x;
+    u1 = y;
+}
+LRK_SPHERICAL_FN float bilinear_pdf(const SphWarp &w, float x, float y) {
+    if (x < 0.f || x > 1.f || y < 0.f || y > 1.f) return 0.f;
+    const float sum = w.w[0] + w.w[1] + w.w[2] + w.w[3];
+    if (sum == 0.f) return 1.f;
+    return 4.f * ((1.f - x) * (1.f - y) * w.w[0] + x * (1.f - y) * w.w[1] + (1.f - x) * y * w.w[2] + x * y * w.w[3]) / sum;
+}
+
+// pbrt-v4's InvertSphericalTriangleSample: the (u0, u1) for which sample_spherical_direction returns the unit direction w, with the
+// area of the triangle taken as omega (what the sampler uses).  (0.5, 0.5) where the construction degenerates, as pbrt-v4.
+LRK_SPHERICAL_FN void invert_spherical_triangle_sample(SphVec p, SphVec v0, SphVec v1, SphVec v2, float omega, SphVec w, float &u0, float &u1) {
+    using namespace spherical_detail;
+    const SphVec a = normalize(sub(v0, p)), b = normalize(sub(v1, p)), c = normalize(sub(v2, p));
+    SphVec n_ab = cross(a, b), n_ca = cross(c, a);
+    const float lab = dot(n_ab, n_ab), lca = dot(n_ca, n_ca);
+    u0 = 0.5f;
+    u1 = 0.5f;
+    if (lab == 0.f || lca == 0.f) return;
+    n_ab = scale(n_ab, 1.f / sqrtf(lab));
+    n_ca = scale(n_ca, 1.f / sqrtf(lca));
+    const float alpha = angle_between(n_ab, scale(n_ca, -1.f));
+    SphVec cp = cross(cross(b, w), n_ca);
+    const float lcp = dot(cp, cp);
+    if (lcp == 0.f) return;
+    cp = scale(cp, 1.f / sqrtf(lcp));
+    if (dot(cp, add(a, c)) < 0.f) cp = scale(cp, -1.f);
+    float x;
+    if (dot(a, cp) > 0.99999847691f) {// 0.1 degrees
+        x = 0.f;
+    } else {
+        SphVec n_cpb = cross(cp, b), n_acp = cross(a, cp);
+        const float l1 = dot(n_cpb, n_cpb), l2 = dot(n_acp, n_acp);
+        if (l1 == 0.f || l2 == 0.f) return;
+        n_cpb = scale(n_cpb, 1.f / sqrtf(l1));
+        n_acp = scale(n_acp, 1.f / sqrtf(l2));
+        const float ap = alpha + angle_between(n_ab, n_cpb) + angle_between(n_acp, scale(n_cpb, -1.f)) - kSphericalPi;
+        x = ap / omega;
+    }
+    const float y = (1.f - dot(w, b)) / (1.f - dot(cp, b));
+    u0 = fminf(fmaxf(x, 0.f), 1.f);
+    u1 = fminf(fmaxf(y, 0.f), 1.f);
+}
+
+// The warp's factor of the pdf of point x of the triangle seen from p with the receiver normal n (unit): BilinearPDF at the inverted
+// sample of the direction to x.  The caller multiplies pdf[tri] / omega by it; omega as use_spherical requires.
+LRK_SPHERICAL_FN float spherical_warp_pdf(SphVec p, SphVec n, SphVec v0, SphVec v1, SphVec v2, float omega, SphVec x) {
+    using namespace spherical_detail;
+    float u0, u1;
+    invert_spherical_triangle_sample(p, v0, v1, v2, omega, normalize(sub(x, p)), u0, u1);
+    return bilinear_pdf(spherical_warp_weights(p, n, v0, v1, v2), u0, u1);
+}
+
 }// namespace lrk

@@ -28,6 +28,10 @@
 // Resampled light sampling (an extension): `--light-candidates <n>` sets lrk_set_option("light_candidates", n) before the upload;
 // for n from 2 to 32, next-event estimation draws n candidates with the light sampling the flags above choose and traces the shadow
 // ray of one, picked by its unshadowed contribution.  0 and 1 keep one light sample.  Surface integrator only, as above.
+//
+// Receiver-aware light sampling (an extension): `--light-receiver` sets lrk_set_option("light_receiver", 1) before the upload, so
+// that the light tree and the solid-angle sampler also weigh by the shading point's normal.  With --light-tree, --light-tree-triangles
+// or --light-solid-angle; alone, the upload fails with the library's message.  Surface integrator only, as above.
 #include <sys/stat.h>
 #include <sys/wait.h>
 #include <unistd.h>
@@ -55,6 +59,7 @@ const LightFlag kLightFlags[] = {
     {"--light-tree", "Pick next-event lights from a light tree (power, distance, orientation)", {"light_tree"}},
     {"--light-solid-angle", "Sample next-event light points uniformly in solid angle, not by area", {"light_solid_angle"}},
     {"--light-tree-triangles", "Also pick the emissive triangle from the light tree (implies --light-tree)", {"light_tree", "light_tree_triangles"}},
+    {"--light-receiver", "Weigh tree lights and solid-angle points by the shading normal", {"light_receiver"}},
 };
 
 void usage() {

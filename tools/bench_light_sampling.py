@@ -1,6 +1,6 @@
 """Next-event light sampling options against what they replace, on cuda:0.  Prints one JSON line.
 
-    python tools/bench_light_sampling.py --compare {tree,solid_angle,triangles,candidates} [--spp 64] [--reference-spp 4096]
+    python tools/bench_light_sampling.py --compare {tree,solid_angle,triangles,candidates,receiver} [--spp 64] [--reference-spp 4096]
 
 A frame's comparison: a reference of `--reference-spp` samples of the indices [SPP, SPP + reference) rendered with the setting under
 test, then alternately, twice each, the renders of [0, SPP) under every setting of the comparison.  Device time (lrk_stats::
@@ -22,6 +22,10 @@ one over that of the other, since the error of an unbiased render falls as 1 / s
     spheres, two quads), C2's Cornell box (1024x1024), near_light (1024x1024), near_light with its glossy Disney desk (1024x1024:
     the frame where the closure decides which light samples matter) and the many-light frame (1920x1080) with the light tree on
     in every setting.
+  * receiver (option "light_receiver" on against off, with the light sampling it refines the same in both): near_light (1024x1024)
+    and C2's Cornell box (1024x1024) with solid-angle points; the many-light frame (1920x1080) with the tree, and with the tree and
+    its triangle level; the emissive globe (1024x1024) with the triangle level; C3 (1920x1080) with the tree, where there is
+    little to gain.
 The card's name and power limit are read in the same run.
 """
 from __future__ import annotations
@@ -139,7 +143,26 @@ def compare_candidates(r, desc, spp: int, ref_spp: int) -> dict:
             "many_lights_tree": candidates_frame(scenes.many_lights(resolution=(1920, 1080), spp=spp), light_tree=True)}
 
 
-COMPARE = {"tree": compare_tree, "solid_angle": compare_solid_angle, "triangles": compare_triangles, "candidates": compare_candidates}
+def compare_receiver(r, desc, spp: int, ref_spp: int) -> dict:
+    from luisarender_b200 import scenes
+
+    def receiver_frame(src, **base):
+        base = {"light_tree": 0, "light_tree_triangles": 0, "light_solid_angle": 0, "light_candidates": 0, **base}
+        settings = {"off": {**base, "light_receiver": 0}, "on": {**base, "light_receiver": 1}}
+        return frame(r, desc(src), settings, "off", spp, ref_spp, **{k: v for k, v in base.items() if v})
+
+    many = scenes.many_lights(resolution=(1920, 1080), spp=spp)
+    return {"near_light_solid_angle": receiver_frame(scenes.near_light(resolution=(1024, 1024), spp=spp), light_solid_angle=1),
+            "c2_cornell_solid_angle": receiver_frame(scenes.cornell_box(resolution=(1024, 1024), spp=spp), light_solid_angle=1),
+            "many_lights_tree": receiver_frame(many, light_tree=1),
+            "many_lights_triangles": receiver_frame(many, light_tree=1, light_tree_triangles=1),
+            "emissive_globe_triangles": receiver_frame(scenes.emissive_globe(resolution=(1024, 1024), spp=spp), light_tree=1,
+                                                       light_tree_triangles=1),
+            "c3_tree": receiver_frame(scenes.instanced_spheres(resolution=(1920, 1080), spp=spp, seed=1), light_tree=1)}
+
+
+COMPARE = {"tree": compare_tree, "solid_angle": compare_solid_angle, "triangles": compare_triangles, "candidates": compare_candidates,
+           "receiver": compare_receiver}
 
 
 def main():
