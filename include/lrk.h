@@ -13,6 +13,8 @@
  *   lrk_create          <- Context::create_device + Device::create_stream      src/apps/cli.cpp:167-181
  *   lrk_upload_scene    <- Pipeline::create (Geometry::build, register_surface/light,
  *                          Integrator::build)                                    src/base/pipeline.cpp:44-99
+ *   lrk_update_instances / lrk_update_camera
+ *                       <- (none: an extension, the reference rebuilds its pipeline per scene)  DESIGN.md §4 (Scene updates)
  *   lrk_set_shard       <- (none: the reference is single device)               SURVEY.md §8e
  *   lrk_comm_unique_id / lrk_comm_init / lrk_reduce_film
  *                       <- (none; sums the film of src/films/color.cpp:107-130 over ranks)  SURVEY.md §8e
@@ -499,6 +501,29 @@ void lrk_destroy(lrk_ctx *ctx);
 const char *lrk_last_error(const lrk_ctx *ctx);
 
 int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *scene);
+
+/* Scene updates (an extension: change an uploaded scene between renders without lrk_upload_scene; DESIGN.md §4 (Scene updates)).
+ * lrk_update_instances gives the instances ids[0 .. count) new object-to-world rows, 12 floats per id (row-major 3x4, as
+ * lrk_instance::object_to_world); an instance id is its index in lrk_scene_desc::instances, the host front-end's flattening order.
+ * lrk_update_camera replaces the camera record.
+ *   Equal to:  after a successful call every render, trace, G-buffer, denoise and adaptive call gives bit for bit what it gives on
+ *              a context that uploaded the updated description: the same scene with those rows as object_to_world and the
+ *              matching world_to_object (the flattening's double-precision inverse, computed here by the same code), or with that
+ *              camera record.  The instance level of the hierarchy is rebuilt on the device (an LBVH), so its node bytes differ
+ *              from the host's; closest hits do not depend on them.  With "light_tree" active, the light tree and its bottom
+ *              trees are rebuilt as lrk_upload_scene builds them when an emissive instance moves.
+ *   Film:      both calls end with lrk_film_clear, as lrk_upload_scene does: a new frame starts (the G-buffer latch and the
+ *              adaptive state reset as at any clear).
+ *   Refused:   LRK_ERR_INVALID_ARGUMENT for no scene, an id >= instance_count, a repeated id, a non-finite entry, a singular
+ *              linear part (determinant exactly 0, the flattening's rule), or a camera whose resolution differs from the uploaded
+ *              one (a new film size needs lrk_upload_scene).  Everything is checked before anything changes: a refused call
+ *              leaves the scene and the film as they were.
+ *   Stays:     handles, visibility, meshes, surfaces, lights, media, the environment, the sampler, and the shard assignment
+ *              (lrk_set_shard, a probed lrk_balance_shards table); the reduced film stays bit-identical to one GPU's.
+ * Both calls synchronise before they return: the caller's arrays can be freed afterwards.  Deforming meshes, adding or removing
+ * instances and changing what an instance carries need lrk_upload_scene. */
+int lrk_update_instances(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const float *object_to_world);
+int lrk_update_camera(lrk_ctx *ctx, const lrk_camera *camera);
 
 /* Pixel-tile sharding for multi-GPU (SURVEY.md §8e): this ctx renders the tiles with
  * lrk_tile_owner(tile_id, world) == rank, tiles are tile_size x tile_size pixels in row-major tile order.

@@ -139,6 +139,24 @@ class Renderer:
         self._check(self._lib.lrk_upload_scene(self._ctx, C.byref(desc)), "lrk_upload_scene")
         self._res = (desc.camera.resolution[0], desc.camera.resolution[1])
 
+    def update_instances(self, ids, object_to_world):
+        """lrk_update_instances: give the instances `ids` (indices into the description's instances) new object-to-world rows,
+        `object_to_world` [n, 3, 4] float32, without a re-upload.  Afterwards every render, trace, G-buffer, denoise and adaptive
+        call gives bit for bit what a context that uploaded the updated description gives: the same scene with these rows as
+        object_to_world and the matching world_to_object.  The film is cleared; a refused call (an id out of range or repeated, a
+        non-finite or singular transform) raises and leaves the scene and the film as they were."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint32).reshape(-1)
+        rows = np.ascontiguousarray(object_to_world, dtype=np.float32)
+        if rows.shape != (len(ids), 3, 4):
+            raise ValueError(f"object_to_world must be [{len(ids)}, 3, 4], not {list(rows.shape)}")
+        self._check(self._lib.lrk_update_instances(self._ctx, ids.ctypes.data, len(ids), rows.ctypes.data), "lrk_update_instances")
+
+    def update_camera(self, camera: F.Camera):
+        """lrk_update_camera: replace the camera record (an lrk_camera such as ``Scene.desc().camera``) without a re-upload.
+        Afterwards every call gives bit for bit what a context that uploaded the description with this camera gives.  The film is
+        cleared; a camera of another resolution is refused (a new film size needs an upload)."""
+        self._check(self._lib.lrk_update_camera(self._ctx, C.byref(camera)), "lrk_update_camera")
+
     def set_shard(self, rank: int, world: int, tile_size: int = 32):
         self._check(self._lib.lrk_set_shard(self._ctx, rank, world, tile_size), "lrk_set_shard")
 

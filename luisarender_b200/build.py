@@ -52,6 +52,7 @@ def build_host(force=False, verbose=False) -> Path:
     out = LIB / "libluisa_render_host.so"
     src_dir = PKG / "csrc" / "host"
     deps = list(src_dir.glob("*.cpp")) + list(src_dir.glob("*.h")) + list((REPO / "include").glob("*.h"))
+    deps.append(PKG / "csrc" / "device" / "affine_inverse.h")  # shared with the device library (flatten.cpp)
     if not force and _newer(out, deps):
         return out
     LIB.mkdir(exist_ok=True)

@@ -22,6 +22,7 @@
 #include "adaptive.cuh"
 #include "gbuffer.cuh"
 #include "denoise.cuh"
+#include "affine_inverse.h"
 #include <cub/device/device_scan.cuh>
 
 using namespace lrk;
@@ -64,7 +65,7 @@ private:
 struct DeviceArrays {
     DeviceBuffer vertices, triangles, alias, pdf, meshes, inst_handles, inst_kind, inst_o2w, inst_xform, bvh_nodes, traversal_overflow, sobol, vdc, vdc_inv, pmj, blue_noise, pmj_pixels, zsobol_hash, sampler, build_scratch, mesh_bounds, inst_mesh, visible_ids, scene_copy, media, textures, texels, env_alias, env_pdf,
         tri_verts, surfaces, lights, light_handles, camera, lt_nodes, lt_light_inst, lt_trail, lt_inst_light, lt_bottom_nodes, lt_inst_bottom,
-        lt_bottom_trail;
+        lt_bottom_trail, update_staging;
 };
 
 enum KernelCategory { CAT_TRACE_CLOSEST = 0, CAT_TRACE_SHADOW = 1, CAT_SHADE = 2, CAT_OTHER = 3, CAT_COUNT = 4 };
@@ -72,6 +73,19 @@ enum KernelCategory { CAT_TRACE_CLOSEST = 0, CAT_TRACE_SHADOW = 1, CAT_SHADE = 2
 struct TimedLaunch {
     int cat;
     cudaEvent_t start, stop;
+};
+
+// What the light tree of the option "light_tree" and its bottom trees are built from, copied from the scene description by
+// lrk_upload_scene so that lrk_update_instances rebuilds them with the same code: per instance that carries a light (in instance
+// order) its mesh, object-to-world rows, power (luminance of the emission x the light's scale) and sidedness, and per such mesh
+// the object-space positions of its triangles' vertices (9 floats per triangle).
+struct LightTreeSource {
+    uint32_t instance_count{0};
+    std::vector<uint32_t> inst, mesh;
+    std::vector<float> o2w;
+    std::vector<double> power;
+    std::vector<uint8_t> two_sided;
+    std::map<uint32_t, std::vector<float>> mesh_points;
 };
 
 }// namespace
@@ -148,6 +162,12 @@ struct lrk_ctx {
     // instantiations (upload_light_sampling)
     LightSampling light_requested, light_active;
     uint32_t *receiver_words{nullptr};// in path_allocs while light_active.receiver (alloc_paths)
+    LightTreeSource light_source;// while light_active.tree
+    // scene updates (lrk_update_instances): the instance level of the hierarchy is rebuilt on the device from these
+    std::vector<uint32_t> inst_mesh_host, visible_host;// per instance its mesh; the visible instances in order
+    uint32_t mesh_count{0};
+    uint64_t bvh_node_count{0};// of the uploaded hierarchy, whose last max(visible, 2) - 1 nodes are the instance level
+    bool tlas_inputs{false};// a.inst_mesh, a.visible_ids and a.mesh_bounds hold the scene's (device_bvh, or since the first update)
 
     ~lrk_ctx();
 };
@@ -509,15 +529,97 @@ int render_pass_volume(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_
     return LRK_OK;
 }
 
+// Scratch of the device hierarchy build (bvh_build.cuh) for sets of at most max_n primitives, carved out of a.build_scratch: boxes,
+// node boxes, keys / values (double buffered), radix nodes, leaf parents, visit counters, whole-set bounds, cub's temporary storage.
+struct BuildScratch {
+    BuildBox *boxes, *node_boxes;
+    uint32_t *keys, *keys2, *vals, *vals2;
+    RadixNode *radix;
+    uint32_t *leaf_parent, *visits, *whole;
+    void *cub;
+    size_t cub_bytes;
+};
+
+int reserve_build_scratch(lrk_ctx *ctx, uint64_t max_n, BuildScratch &b) {
+    size_t cub_bytes = 0u;
+    cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, static_cast<const uint32_t *>(nullptr), static_cast<uint32_t *>(nullptr),
+                                    static_cast<const uint32_t *>(nullptr), static_cast<uint32_t *>(nullptr), static_cast<int>(max_n), 0, 30, ctx->stream);
+    const size_t n8 = (max_n + 7u) & ~size_t{7u};
+    const size_t off_boxes = 0u, off_node_boxes = off_boxes + n8 * sizeof(BuildBox), off_keys = off_node_boxes + n8 * sizeof(BuildBox),
+                 off_keys2 = off_keys + n8 * 4u, off_vals = off_keys2 + n8 * 4u, off_vals2 = off_vals + n8 * 4u, off_radix = off_vals2 + n8 * 4u,
+                 off_leaf_parent = off_radix + n8 * sizeof(RadixNode), off_visits = off_leaf_parent + n8 * 4u, off_whole = off_visits + n8 * 4u,
+                 off_cub = off_whole + 64u, total = off_cub + cub_bytes;
+    LRK_CUDA(ctx->arrays.build_scratch.reserve(total));
+    auto base = ctx->arrays.build_scratch.get<char>();
+    b.boxes = reinterpret_cast<BuildBox *>(base + off_boxes);
+    b.node_boxes = reinterpret_cast<BuildBox *>(base + off_node_boxes);
+    b.keys = reinterpret_cast<uint32_t *>(base + off_keys);
+    b.keys2 = reinterpret_cast<uint32_t *>(base + off_keys2);
+    b.vals = reinterpret_cast<uint32_t *>(base + off_vals);
+    b.vals2 = reinterpret_cast<uint32_t *>(base + off_vals2);
+    b.radix = reinterpret_cast<RadixNode *>(base + off_radix);
+    b.leaf_parent = reinterpret_cast<uint32_t *>(base + off_leaf_parent);
+    b.visits = reinterpret_cast<uint32_t *>(base + off_visits);
+    b.whole = reinterpret_cast<uint32_t *>(base + off_whole);
+    b.cub = base + off_cub;
+    b.cub_bytes = cub_bytes;
+    return LRK_OK;
+}
+
+const uint32_t kWholeInit[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};// empty whole-set bounds (bvh_build.cuh: grow_whole)
+
+unsigned build_blocks(uint64_t n) { return static_cast<unsigned>((n + 255u) / 256u); }
+
+// The common tail of every hierarchy over the n boxes in b.boxes (whole-set bounds in b.whole): sort, radix tree, fit, emit.
+int build_hierarchy(lrk_ctx *ctx, const BuildScratch &b, uint32_t n, bool tlas, uint32_t node_base, uint32_t slot_base) {
+    auto &a = ctx->arrays;
+    auto out_nodes = a.bvh_nodes.get<float4>();
+    auto stream = ctx->stream;
+    if (n == 1u) {
+        if (tlas) build_single_kernel<true><<<1, 1, 0, stream>>>(b.boxes, b.whole, a.visible_ids.get<const uint32_t>(), node_base, slot_base, out_nodes);
+        else build_single_kernel<false><<<1, 1, 0, stream>>>(b.boxes, b.whole, nullptr, node_base, slot_base, out_nodes);
+        LRK_CUDA(cudaMemsetAsync(b.vals2, 0, 4u, stream));// sorted order of one primitive
+        return LRK_OK;
+    }
+    build_morton_kernel<<<build_blocks(n), 256, 0, stream>>>(b.boxes, n, b.whole, b.keys, b.vals);
+    size_t bytes = b.cub_bytes;
+    LRK_CUDA(cub::DeviceRadixSort::SortPairs(b.cub, bytes, b.keys, b.keys2, b.vals, b.vals2, static_cast<int>(n), 0, 30, stream));
+    LRK_CUDA(cudaMemsetAsync(b.visits, 0, static_cast<size_t>(n) * 4u, stream));
+    build_radix_tree_kernel<<<build_blocks(n - 1u), 256, 0, stream>>>(b.keys2, static_cast<int>(n), b.radix, b.leaf_parent);
+    build_fit_kernel<<<build_blocks(n), 256, 0, stream>>>(b.radix, b.leaf_parent, b.vals2, b.boxes, static_cast<int>(n), b.node_boxes, b.visits);
+    if (tlas) build_emit_kernel<true><<<build_blocks(n - 1u), 256, 0, stream>>>(b.radix, b.vals2, b.boxes, b.node_boxes, static_cast<int>(n), b.whole,
+                                                                                 a.visible_ids.get<const uint32_t>(), node_base, slot_base, out_nodes);
+    else build_emit_kernel<false><<<build_blocks(n - 1u), 256, 0, stream>>>(b.radix, b.vals2, b.boxes, b.node_boxes, static_cast<int>(n), b.whole, nullptr,
+                                                                            node_base, slot_base, out_nodes);
+    LRK_CUDA(cudaGetLastError());
+    return LRK_OK;
+}
+
+// The instance level over the nv visible instances (a.visible_ids) from their object-to-world rows (a.inst_o2w) and their meshes'
+// object-space bounds (a.inst_mesh, a.mesh_bounds): max(nv, 2) - 1 nodes from tlas_root on, the root first.
+int build_instance_level(lrk_ctx *ctx, const BuildScratch &b, uint32_t nv, uint32_t tlas_root) {
+    auto &a = ctx->arrays;
+    auto stream = ctx->stream;
+    if (nv == 0u) {// nothing to hit: a root with two empty children
+        const float inf = std::numeric_limits<float>::infinity();
+        lrk_bvh_node root{};
+        for (int k = 0; k < 3; k++) { root.lo0[k] = root.lo1[k] = inf; root.hi0[k] = root.hi1[k] = -inf; }
+        root.ref0 = root.ref1 = root.parent = LRK_BVH_EMPTY;
+        LRK_CUDA(cudaMemcpyAsync(a.bvh_nodes.get<float4>() + static_cast<size_t>(tlas_root) * 4u, &root, sizeof(root), cudaMemcpyHostToDevice, stream));
+        LRK_CUDA(cudaStreamSynchronize(stream));// `root` is a local
+        return LRK_OK;
+    }
+    LRK_CUDA(cudaMemcpyAsync(b.whole, kWholeInit, sizeof(kWholeInit), cudaMemcpyHostToDevice, stream));
+    build_instance_bounds_kernel<<<build_blocks(nv), 256, 0, stream>>>(a.inst_o2w.get<const float4>(), a.inst_mesh.get<const uint32_t>(),
+                                                                       a.visible_ids.get<const uint32_t>(), nv, a.mesh_bounds.get<const BuildBox>(), b.boxes, b.whole);
+    return build_hierarchy(ctx, b, nv, true, tlas_root, 0u);
+}
+
 // Hierarchy build on the device (bvh_build.cuh): fills a.bvh_nodes / a.tri_verts from the uploaded geometry, returns the root of
 // every mesh's BLAS and of the TLAS.  One round of kernels per unique mesh, one for the instances.
 int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint32_t> &mesh_root, uint32_t &tlas_root) {
     auto &a = ctx->arrays;
-    std::vector<uint32_t> visible, inst_mesh(s->instance_count);
-    for (uint32_t i = 0; i < s->instance_count; i++) {
-        inst_mesh[i] = s->instances[i].mesh;
-        if (s->instances[i].visible) visible.push_back(i);
-    }
+    const std::vector<uint32_t> &visible = ctx->visible_host, &inst_mesh = ctx->inst_mesh_host;
     // node layout: per mesh max(n - 1, 1) nodes, then the TLAS
     mesh_root.resize(s->mesh_count);
     uint64_t nodes = 0u, max_n = std::max<uint64_t>(visible.size(), 2u);
@@ -531,109 +633,89 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
     tlas_root = static_cast<uint32_t>(nodes);
     nodes += std::max<uint64_t>(visible.size(), 2u) - 1u;
     if (nodes >= 0x7fffffffull || s->triangle_count >= (1ull << 28)) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: scene too large for the BVH encoding");
+    ctx->bvh_node_count = nodes;
     int rc;
     LRK_CUDA(a.bvh_nodes.reserve(nodes * 64u));
     LRK_CUDA(a.tri_verts.reserve(std::max<uint64_t>(s->triangle_count, 1u) * 48u));
     LRK_CUDA(a.mesh_bounds.reserve(std::max<uint64_t>(s->mesh_count, 1u) * sizeof(BuildBox)));
     if ((rc = upload(ctx, a.inst_mesh, inst_mesh.data(), inst_mesh.size()))) return rc;
     if ((rc = upload(ctx, a.visible_ids, visible.data(), visible.size()))) return rc;
-    // scratch: boxes, node boxes, keys / values (double buffered), radix nodes, leaf parents, visit counters, whole-set bounds, cub
-    size_t cub_bytes = 0u;
-    cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, static_cast<const uint32_t *>(nullptr), static_cast<uint32_t *>(nullptr),
-                                    static_cast<const uint32_t *>(nullptr), static_cast<uint32_t *>(nullptr), static_cast<int>(max_n), 0, 30, ctx->stream);
-    const size_t n8 = (max_n + 7u) & ~size_t{7u};
-    const size_t off_boxes = 0u, off_node_boxes = off_boxes + n8 * sizeof(BuildBox), off_keys = off_node_boxes + n8 * sizeof(BuildBox),
-                 off_keys2 = off_keys + n8 * 4u, off_vals = off_keys2 + n8 * 4u, off_vals2 = off_vals + n8 * 4u, off_radix = off_vals2 + n8 * 4u,
-                 off_leaf_parent = off_radix + n8 * sizeof(RadixNode), off_visits = off_leaf_parent + n8 * 4u, off_whole = off_visits + n8 * 4u,
-                 off_cub = off_whole + 64u, total = off_cub + cub_bytes;
-    LRK_CUDA(a.build_scratch.reserve(total));
-    auto base = a.build_scratch.get<char>();
-    auto boxes = reinterpret_cast<BuildBox *>(base + off_boxes), node_boxes = reinterpret_cast<BuildBox *>(base + off_node_boxes);
-    auto keys = reinterpret_cast<uint32_t *>(base + off_keys), keys2 = reinterpret_cast<uint32_t *>(base + off_keys2);
-    auto vals = reinterpret_cast<uint32_t *>(base + off_vals), vals2 = reinterpret_cast<uint32_t *>(base + off_vals2);
-    auto radix = reinterpret_cast<RadixNode *>(base + off_radix);
-    auto leaf_parent = reinterpret_cast<uint32_t *>(base + off_leaf_parent), visits = reinterpret_cast<uint32_t *>(base + off_visits);
-    auto whole = reinterpret_cast<uint32_t *>(base + off_whole);
-    auto out_nodes = a.bvh_nodes.get<float4>();
+    BuildScratch b;
+    if ((rc = reserve_build_scratch(ctx, max_n, b))) return rc;
     auto stream = ctx->stream;
-    static const uint32_t whole_init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
-    auto blocks = [](uint64_t n) { return static_cast<unsigned>((n + 255u) / 256u); };
-    // common tail: sort, radix tree, fit, emit
-    auto hierarchy = [&](uint32_t n, bool tlas, uint32_t node_base, uint32_t slot_base) -> int {
-        if (n == 1u) {
-            if (tlas) build_single_kernel<true><<<1, 1, 0, stream>>>(boxes, whole, a.visible_ids.get<const uint32_t>(), node_base, slot_base, out_nodes);
-            else build_single_kernel<false><<<1, 1, 0, stream>>>(boxes, whole, nullptr, node_base, slot_base, out_nodes);
-            LRK_CUDA(cudaMemsetAsync(vals2, 0, 4u, stream));// sorted order of one primitive
-            return LRK_OK;
-        }
-        build_morton_kernel<<<blocks(n), 256, 0, stream>>>(boxes, n, whole, keys, vals);
-        size_t bytes = cub_bytes;
-        LRK_CUDA(cub::DeviceRadixSort::SortPairs(base + off_cub, bytes, keys, keys2, vals, vals2, static_cast<int>(n), 0, 30, stream));
-        LRK_CUDA(cudaMemsetAsync(visits, 0, static_cast<size_t>(n) * 4u, stream));
-        build_radix_tree_kernel<<<blocks(n - 1u), 256, 0, stream>>>(keys2, static_cast<int>(n), radix, leaf_parent);
-        build_fit_kernel<<<blocks(n), 256, 0, stream>>>(radix, leaf_parent, vals2, boxes, static_cast<int>(n), node_boxes, visits);
-        if (tlas) build_emit_kernel<true><<<blocks(n - 1u), 256, 0, stream>>>(radix, vals2, boxes, node_boxes, static_cast<int>(n), whole,
-                                                                               a.visible_ids.get<const uint32_t>(), node_base, slot_base, out_nodes);
-        else build_emit_kernel<false><<<blocks(n - 1u), 256, 0, stream>>>(radix, vals2, boxes, node_boxes, static_cast<int>(n), whole, nullptr, node_base,
-                                                                          slot_base, out_nodes);
-        LRK_CUDA(cudaGetLastError());
-        return LRK_OK;
-    };
     uint32_t slot_base = 0u;
     for (uint32_t m = 0; m < s->mesh_count; m++) {
         const auto &mesh = s->meshes[m];
         const uint32_t n = mesh.triangle_count;
         auto verts = a.vertices.get<const lrk_vertex>() + mesh.vertex_offset;
         auto tris = a.triangles.get<const lrk_triangle>() + mesh.triangle_offset;
-        LRK_CUDA(cudaMemcpyAsync(whole, whole_init, sizeof(whole_init), cudaMemcpyHostToDevice, stream));
-        build_triangle_bounds_kernel<<<blocks(n), 256, 0, stream>>>(verts, tris, n, boxes, whole);
-        build_store_mesh_bounds_kernel<<<1, 1, 0, stream>>>(whole, a.mesh_bounds.get<BuildBox>(), m);
-        if ((rc = hierarchy(n, false, mesh_root[m], slot_base))) return rc;
-        build_tri_verts_kernel<<<blocks(n), 256, 0, stream>>>(verts, tris, vals2, n, a.tri_verts.get<float4>() + static_cast<size_t>(slot_base) * 3u);
+        LRK_CUDA(cudaMemcpyAsync(b.whole, kWholeInit, sizeof(kWholeInit), cudaMemcpyHostToDevice, stream));
+        build_triangle_bounds_kernel<<<build_blocks(n), 256, 0, stream>>>(verts, tris, n, b.boxes, b.whole);
+        build_store_mesh_bounds_kernel<<<1, 1, 0, stream>>>(b.whole, a.mesh_bounds.get<BuildBox>(), m);
+        if ((rc = build_hierarchy(ctx, b, n, false, mesh_root[m], slot_base))) return rc;
+        build_tri_verts_kernel<<<build_blocks(n), 256, 0, stream>>>(verts, tris, b.vals2, n, a.tri_verts.get<float4>() + static_cast<size_t>(slot_base) * 3u);
         slot_base += n;
     }
-    const uint32_t nv = static_cast<uint32_t>(visible.size());
-    if (nv == 0u) {// nothing to hit: a root with two empty children
-        const float inf = std::numeric_limits<float>::infinity();
-        lrk_bvh_node root{};
-        for (int k = 0; k < 3; k++) { root.lo0[k] = root.lo1[k] = inf; root.hi0[k] = root.hi1[k] = -inf; }
-        root.ref0 = root.ref1 = root.parent = LRK_BVH_EMPTY;
-        LRK_CUDA(cudaMemcpyAsync(out_nodes + static_cast<size_t>(tlas_root) * 4u, &root, sizeof(root), cudaMemcpyHostToDevice, stream));
-    } else {
-        LRK_CUDA(cudaMemcpyAsync(whole, whole_init, sizeof(whole_init), cudaMemcpyHostToDevice, stream));
-        build_instance_bounds_kernel<<<blocks(nv), 256, 0, stream>>>(a.inst_o2w.get<const float4>(), a.inst_mesh.get<const uint32_t>(),
-                                                                    a.visible_ids.get<const uint32_t>(), nv, a.mesh_bounds.get<const BuildBox>(), boxes, whole);
-        if ((rc = hierarchy(nv, true, tlas_root, 0u))) return rc;
-    }
-    LRK_CUDA(cudaStreamSynchronize(stream));// host vectors (visible, inst_mesh) and the static init block are done with
+    if ((rc = build_instance_level(ctx, b, static_cast<uint32_t>(visible.size()), tlas_root))) return rc;
+    LRK_CUDA(cudaStreamSynchronize(stream));// the static init block is done with
     LRK_CUDA(cudaGetLastError());
+    ctx->tlas_inputs = true;
     return LRK_OK;
 }
 
-// The triangles of `mesh`, 9 doubles each: in world space through the row-major 3x4 object-to-world matrix m, or in object space
-// when m is null.
-void gather_triangles(const lrk_scene_desc *s, const lrk_mesh &mesh, const float *m, std::vector<double> &tris) {
-    tris.clear();
-    for (uint32_t t = 0; t < mesh.triangle_count; t++) {
-        const lrk_triangle &tri = s->triangles[mesh.triangle_offset + t];
-        for (uint32_t v : {tri.i0, tri.i1, tri.i2}) {
-            const float *p = s->vertices[mesh.vertex_offset + v].p;
-            for (int r = 0; r < 3; r++)
-                tris.push_back(m == nullptr ? static_cast<double>(p[r])
-                                            : static_cast<double>(m[4 * r]) * p[0] + static_cast<double>(m[4 * r + 1]) * p[1] +
-                                                  static_cast<double>(m[4 * r + 2]) * p[2] + m[4 * r + 3]);
-        }
+// One entry of lrk_update_instances' staging buffer: the instance and its new object-to-world rows.
+struct InstanceUpdate {
+    uint32_t id;
+    float o2w[12];
+};
+
+// The instance records of an update: object-to-world rows and rows 0-2 of inst_xform (world-to-object, through the flattening's
+// own inverse, affine_inverse.h); row 3, the BLAS root, stays.  The host has refused singular rows.
+__global__ void __launch_bounds__(256) update_instances_kernel(const InstanceUpdate *__restrict__ updates, uint32_t count, float4 *__restrict__ inst_o2w,
+                                                               float4 *__restrict__ inst_xform) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= count) return;
+    const InstanceUpdate u = updates[k];
+    float w2o[12];
+    inverse_affine_rows(u.o2w, w2o);
+    for (uint32_t r = 0; r < 3u; r++) {
+        inst_o2w[u.id * 3u + r] = make_float4(u.o2w[4u * r], u.o2w[4u * r + 1u], u.o2w[4u * r + 2u], u.o2w[4u * r + 3u]);
+        inst_xform[u.id * 4u + r] = make_float4(w2o[4u * r], w2o[4u * r + 1u], w2o[4u * r + 2u], w2o[4u * r + 3u]);
     }
 }
 
-// The light tree of the option "light_tree" (light_tree.h) over every instance that carries a light - not only the first light_count
-// handles - from the scene's own arrays: world-space triangles, the emission (the mean of max(texel, 0) of an image emission) and the
-// sidedness.  tree_inst: per tree light its instance; inst_light: per instance its tree light, kLightTreeNone for instances without
-// a light or without power.
-int build_light_tree(lrk_ctx *ctx, const lrk_scene_desc *s, LightTreeBuild &tree, std::vector<uint32_t> &tree_inst, std::vector<uint32_t> &inst_light) {
-    std::vector<LightTreeEmitter> emitters;
-    inst_light.assign(s->instance_count, kLightTreeNone);
-    std::vector<double> tris;
+// Object-space bounds of every mesh of a host-built hierarchy, for the instance-level rebuild: the union of its BLAS root's two
+// child boxes, which contain the mesh (padded like every box of that hierarchy; an empty child is +inf / -inf).
+__global__ void __launch_bounds__(256) blas_root_bounds_kernel(const lrk_mesh *__restrict__ meshes, const float4 *__restrict__ nodes, uint32_t mesh_count,
+                                                               BuildBox *__restrict__ mesh_bounds) {
+    const uint32_t m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= mesh_count) return;
+    const float4 *n = nodes + static_cast<size_t>(meshes[m].bvh_root) * 4u;
+    const float4 a = n[0], b = n[1], c = n[2];// lo0, hi0, lo1, hi1 (lrk_bvh_node)
+    BuildBox box;
+    box.lo[0] = fminf(a.x, b.z), box.lo[1] = fminf(a.y, b.w), box.lo[2] = fminf(a.z, c.x);
+    box.hi[0] = fmaxf(a.w, c.y), box.hi[1] = fmaxf(b.x, c.z), box.hi[2] = fmaxf(b.y, c.w);
+    mesh_bounds[m] = box;
+}
+
+// The triangles of an emissive mesh (LightTreeSource::mesh_points), 9 doubles each: in world space through the row-major 3x4
+// object-to-world matrix m, or in object space when m is null.
+void gather_triangles(const std::vector<float> &points, const float *m, std::vector<double> &tris) {
+    tris.clear();
+    for (size_t k = 0; k < points.size(); k += 3u) {
+        const float *p = &points[k];
+        for (int r = 0; r < 3; r++)
+            tris.push_back(m == nullptr ? static_cast<double>(p[r])
+                                        : static_cast<double>(m[4 * r]) * p[0] + static_cast<double>(m[4 * r + 1]) * p[1] +
+                                              static_cast<double>(m[4 * r + 2]) * p[2] + m[4 * r + 3]);
+    }
+}
+
+// The light tree's input from the scene's own arrays: every instance that carries a light - not only the first light_count
+// handles -, the emission (the mean of max(texel, 0) of an image emission), the sidedness and the emissive meshes' triangles.
+int capture_light_source(lrk_ctx *ctx, const lrk_scene_desc *s, LightTreeSource &src) {
+    src = LightTreeSource{};
+    src.instance_count = s->instance_count;
     for (uint32_t i = 0; i < s->instance_count; i++) {
         const auto &inst = s->instances[i];
         if (!(inst.handle[0] & LRK_SHAPE_HAS_LIGHT)) continue;
@@ -651,40 +733,63 @@ int build_light_tree(lrk_ctx *ctx, const lrk_scene_desc *s, LightTreeBuild &tree
         }
         for (double &c : rgb) c = std::max(c, 0.0);
         const double lum = 0.2126 * rgb[0] + 0.7152 * rgb[1] + 0.0722 * rgb[2];
-        gather_triangles(s, s->meshes[inst.mesh], inst.object_to_world, tris);
-        inst_light[i] = static_cast<uint32_t>(emitters.size());
-        tree_inst.push_back(i);
-        emitters.push_back(light_tree_emitter(tris, lum * light.scale, light.two_sided != 0u));
+        src.inst.push_back(i);
+        src.mesh.push_back(inst.mesh);
+        src.o2w.insert(src.o2w.end(), inst.object_to_world, inst.object_to_world + 12);
+        src.power.push_back(lum * light.scale);
+        src.two_sided.push_back(light.two_sided != 0u ? 1u : 0u);
+        auto &points = src.mesh_points[inst.mesh];
+        if (!points.empty()) continue;
+        const lrk_mesh &mesh = s->meshes[inst.mesh];
+        for (uint32_t t = 0; t < mesh.triangle_count; t++) {
+            const lrk_triangle &tri = s->triangles[mesh.triangle_offset + t];
+            for (uint32_t v : {tri.i0, tri.i1, tri.i2}) points.insert(points.end(), s->vertices[mesh.vertex_offset + v].p, s->vertices[mesh.vertex_offset + v].p + 3);
+        }
+    }
+    return LRK_OK;
+}
+
+// The light tree of the option "light_tree" (light_tree.h) over the emitters of `src`: world-space triangles, power and sidedness.
+// tree_inst: per tree light its instance; inst_light: per instance its tree light, kLightTreeNone for instances without a light or
+// without power.
+void build_light_tree(const LightTreeSource &src, LightTreeBuild &tree, std::vector<uint32_t> &tree_inst, std::vector<uint32_t> &inst_light) {
+    std::vector<LightTreeEmitter> emitters;
+    inst_light.assign(src.instance_count, kLightTreeNone);
+    std::vector<double> tris;
+    for (size_t e = 0; e < src.inst.size(); e++) {
+        gather_triangles(src.mesh_points.at(src.mesh[e]), &src.o2w[12u * e], tris);
+        inst_light[src.inst[e]] = static_cast<uint32_t>(emitters.size());
+        tree_inst.push_back(src.inst[e]);
+        emitters.push_back(light_tree_emitter(tris, src.power[e], src.two_sided[e] != 0u));
     }
     tree = light_tree_build(emitters);
-    for (uint32_t i = 0; i < s->instance_count; i++)
+    for (uint32_t i = 0; i < src.instance_count; i++)
         if (inst_light[i] != kLightTreeNone && !(emitters[inst_light[i]].phi > 0.0)) inst_light[i] = kLightTreeNone;
-    return LRK_OK;
 }
 
 // The bottom trees of the option "light_tree_triangles" (light_tree_build_triangles): one per distinct (mesh, side) pair among the
 // instances of the top tree, shared by all of them.  nodes: the trees one after the other; inst_bottom: per instance {root, first
 // trail} (2 words), root kLightTreeNone for none; trail: per tree, one trail per triangle of its mesh.
-void build_bottom_light_trees(const lrk_scene_desc *s, const std::vector<uint32_t> &inst_light, std::vector<LightTreeNode> &nodes,
+void build_bottom_light_trees(const LightTreeSource &src, const std::vector<uint32_t> &inst_light, std::vector<LightTreeNode> &nodes,
                               std::vector<uint32_t> &inst_bottom, std::vector<unsigned long long> &trail) {
-    inst_bottom.assign(2u * s->instance_count, 0u);
+    inst_bottom.assign(2u * src.instance_count, 0u);
+    for (uint32_t i = 0; i < src.instance_count; i++) inst_bottom[2u * i] = kLightTreeNone;
     std::map<std::pair<uint32_t, uint32_t>, std::pair<uint32_t, uint32_t>> built;// (mesh, side) -> (root, first trail)
     std::vector<double> tris;
-    for (uint32_t i = 0; i < s->instance_count; i++) {
-        inst_bottom[2u * i] = kLightTreeNone;
+    for (size_t e = 0; e < src.inst.size(); e++) {
+        const uint32_t i = src.inst[e];
         if (inst_light[i] == kLightTreeNone) continue;
-        const auto &inst = s->instances[i];
-        const float *m = inst.object_to_world;// row-major 3x4
+        const float *m = &src.o2w[12u * e];// row-major 3x4
         const double det = static_cast<double>(m[0]) * (static_cast<double>(m[5]) * m[10] - static_cast<double>(m[6]) * m[9]) -
                            static_cast<double>(m[1]) * (static_cast<double>(m[4]) * m[10] - static_cast<double>(m[6]) * m[8]) +
                            static_cast<double>(m[2]) * (static_cast<double>(m[4]) * m[9] - static_cast<double>(m[5]) * m[8]);
-        const LightTreeSide side = s->lights[inst.handle[1] & 4095u].two_sided ? kLightTreeTwoSided : det < 0.0 ? kLightTreeMirrored : kLightTreeOneSided;
-        auto it = built.find({inst.mesh, side});
+        const LightTreeSide side = src.two_sided[e] ? kLightTreeTwoSided : det < 0.0 ? kLightTreeMirrored : kLightTreeOneSided;
+        auto it = built.find({src.mesh[e], side});
         if (it == built.end()) {
-            gather_triangles(s, s->meshes[inst.mesh], nullptr, tris);
+            gather_triangles(src.mesh_points.at(src.mesh[e]), nullptr, tris);
             const LightTreeBuild b = light_tree_build_triangles(tris, side);
             const uint32_t root = b.nodes.empty() ? kLightTreeNone : static_cast<uint32_t>(nodes.size());
-            it = built.emplace(std::make_pair(inst.mesh, static_cast<uint32_t>(side)), std::make_pair(root, static_cast<uint32_t>(trail.size()))).first;
+            it = built.emplace(std::make_pair(src.mesh[e], static_cast<uint32_t>(side)), std::make_pair(root, static_cast<uint32_t>(trail.size()))).first;
             nodes.insert(nodes.end(), b.nodes.begin(), b.nodes.end());
             trail.insert(trail.end(), b.trail.begin(), b.trail.end());
         }
@@ -728,18 +833,18 @@ int check_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
     return LRK_OK;
 }
 
-// lrk_upload_scene's part for the requested light sampling, once the scene record is in a.scene_copy: builds and uploads the light
-// tree and its bottom trees where requested, writes the record the kernels find them through (scene.cuh: null arrays for what is
-// off) after the scene record, and latches the request into ctx->light_active.
-int upload_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
-    const LightSampling want = ctx->light_requested;
+// The light sampling `want` of the uploaded scene, once the scene record is in a.scene_copy (lrk_upload_scene: the requested one,
+// lrk_update_instances: the active one): builds and uploads the light tree and its bottom trees from ctx->light_source where
+// requested, writes the record the kernels find them through (scene.cuh: null arrays for what is off) after the scene record,
+// and latches `want` into ctx->light_active.
+int upload_light_sampling(lrk_ctx *ctx, const LightSampling want) {
     auto &a = ctx->arrays;
     int rc;
     DeviceLightTree rec{};
     LightTreeBuild tree;
     std::vector<uint32_t> tree_inst, inst_light;
     if (want.tree) {
-        if ((rc = build_light_tree(ctx, s, tree, tree_inst, inst_light))) return rc;
+        build_light_tree(ctx->light_source, tree, tree_inst, inst_light);
         if ((rc = upload(ctx, a.lt_nodes, tree.nodes.data(), tree.nodes.size()))) return rc;
         if ((rc = upload(ctx, a.lt_light_inst, tree_inst.data(), tree_inst.size()))) return rc;
         if ((rc = upload(ctx, a.lt_trail, tree.trail.data(), tree.trail.size()))) return rc;
@@ -753,7 +858,7 @@ int upload_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
     std::vector<uint32_t> inst_bottom;
     std::vector<unsigned long long> bottom_trail;
     if (want.triangles) {
-        build_bottom_light_trees(s, inst_light, bottom_nodes, inst_bottom, bottom_trail);
+        build_bottom_light_trees(ctx->light_source, inst_light, bottom_nodes, inst_bottom, bottom_trail);
         if ((rc = upload(ctx, a.lt_bottom_nodes, bottom_nodes.data(), bottom_nodes.size()))) return rc;
         if ((rc = upload(ctx, a.lt_inst_bottom, inst_bottom.data(), inst_bottom.size()))) return rc;
         if ((rc = upload(ctx, a.lt_bottom_trail, bottom_trail.data(), bottom_trail.size()))) return rc;
@@ -1009,8 +1114,13 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     ctx->used_kinds = 1u;
     ctx->any_non_opaque = false;
     std::vector<float> o2w(static_cast<size_t>(s->instance_count) * 12u), xform(static_cast<size_t>(s->instance_count) * 16u);
+    ctx->tlas_inputs = false;
+    ctx->inst_mesh_host.resize(s->instance_count);
+    ctx->visible_host.clear();
     for (uint32_t i = 0; i < s->instance_count; i++) {
         const auto &inst = s->instances[i];
+        ctx->inst_mesh_host[i] = inst.mesh;
+        if (inst.visible) ctx->visible_host.push_back(i);
         std::memcpy(&handles[i * 4u], inst.handle, 16);
         {// closure kind of the instance: the bucket key of the material sort
             const uint32_t flags = inst.handle[0] & 1023u, surface_tag = (inst.handle[1] >> 12u) & 4095u;
@@ -1040,7 +1150,9 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         ctx->bvh_build_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     } else {
         for (uint32_t m = 0; m < s->mesh_count; m++) mesh_root[m] = s->meshes[m].bvh_root;
+        ctx->bvh_node_count = s->bvh_node_count;
     }
+    ctx->mesh_count = s->mesh_count;
     for (uint32_t i = 0; i < s->instance_count; i++) std::memcpy(&xform[i * 16u + 12u], &mesh_root[s->instances[i].mesh], 4);
     if ((rc = upload(ctx, a.inst_xform, xform.data(), xform.size()))) return rc;
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1125,7 +1237,9 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         LRK_CUDA(a.scene_copy.reserve(sizeof(DeviceScene) + sizeof(DeviceLightTree)));
         sc.self = a.scene_copy.get<const DeviceScene>();
         LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get(), &sc, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
-        if ((rc = upload_light_sampling(ctx, s))) return rc;
+        ctx->light_source = LightTreeSource{};
+        if (ctx->light_requested.tree && (rc = capture_light_source(ctx, s, ctx->light_source))) return rc;
+        if ((rc = upload_light_sampling(ctx, ctx->light_requested))) return rc;
     }
     ctx->has_scene = true;
     // a balanced assignment stays a valid partition for any scene of the same film size (a frame loop re-uploads per frame and
@@ -1135,6 +1249,87 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         if (ctx->tile_owner.size() != tiles) ctx->tile_owner.clear();
     }
     if ((rc = build_pixel_list(ctx))) return rc;
+    return lrk_film_clear(ctx);
+}
+
+int lrk_update_instances(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const float *object_to_world) {
+    if (!ctx) return LRK_ERR_INVALID_ARGUMENT;
+    if (!ctx->has_scene) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: no scene");
+    if (count != 0u && (!ids || !object_to_world)) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: null array");
+    // everything is checked before anything changes
+    const uint32_t instances = ctx->scene.instance_count;
+    std::vector<InstanceUpdate> updates(count);
+    std::vector<uint8_t> seen(instances, 0u);
+    for (uint32_t k = 0; k < count; k++) {
+        const uint32_t id = ids[k];
+        if (id >= instances) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: instance id " + std::to_string(id) + " out of range");
+        if (seen[id]) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: instance id " + std::to_string(id) + " repeated");
+        seen[id] = 1u;
+        const float *m = object_to_world + 12u * static_cast<size_t>(k);
+        for (int j = 0; j < 12; j++)
+            if (!std::isfinite(m[j])) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: non-finite transform of instance " + std::to_string(id));
+        float w2o[12];
+        if (!inverse_affine_rows(m, w2o)) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: singular transform of instance " + std::to_string(id));
+        updates[k].id = id;
+        std::memcpy(updates[k].o2w, m, sizeof(updates[k].o2w));
+    }
+    // the instance level is rebuilt in place: the host's SAH build with one instance per leaf and the device's LBVH both emit
+    // max(visible, 2) - 1 nodes, behind every mesh's BLAS
+    const uint32_t visible = static_cast<uint32_t>(ctx->visible_host.size());
+    if (static_cast<uint64_t>(ctx->scene.tlas_root) + std::max(visible, 2u) - 1u != ctx->bvh_node_count)
+        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_update_instances: the uploaded hierarchy's instance level is not its last max(visible instances, 2) - 1 "
+                                              "nodes, so it cannot be rebuilt in place");
+    LRK_CUDA(cudaSetDevice(ctx->device));
+    auto &a = ctx->arrays;
+    auto stream = ctx->stream;
+    int rc;
+    bool emitter_moved = false;
+    if (ctx->light_active.tree) {
+        auto &src = ctx->light_source;
+        for (const auto &u : updates) {
+            const auto it = std::lower_bound(src.inst.begin(), src.inst.end(), u.id);
+            if (it == src.inst.end() || *it != u.id) continue;
+            std::memcpy(&src.o2w[12u * static_cast<size_t>(it - src.inst.begin())], u.o2w, sizeof(u.o2w));
+            emitter_moved = true;
+        }
+    }
+    if (count != 0u) {// a pageable copy of a local: not through upload(), which may page-lock what it copies from
+        LRK_CUDA(a.update_staging.reserve(updates.size() * sizeof(InstanceUpdate)));
+        LRK_CUDA(cudaMemcpyAsync(a.update_staging.get(), updates.data(), updates.size() * sizeof(InstanceUpdate), cudaMemcpyHostToDevice, stream));
+        update_instances_kernel<<<build_blocks(count), 256, 0, stream>>>(a.update_staging.get<const InstanceUpdate>(), count, a.inst_o2w.get<float4>(),
+                                                                        a.inst_xform.get<float4>());
+        LRK_CUDA(cudaGetLastError());
+    }
+    if (!ctx->tlas_inputs) {// a host-built hierarchy, first update: the per-instance meshes, the visible ids and the meshes' bounds
+        LRK_CUDA(a.inst_mesh.reserve(std::max<size_t>(ctx->inst_mesh_host.size() * sizeof(uint32_t), 16u)));
+        LRK_CUDA(a.visible_ids.reserve(std::max<size_t>(ctx->visible_host.size() * sizeof(uint32_t), 16u)));
+        LRK_CUDA(a.mesh_bounds.reserve(std::max<size_t>(ctx->mesh_count, 1u) * sizeof(BuildBox)));
+        LRK_CUDA(cudaMemcpyAsync(a.inst_mesh.get(), ctx->inst_mesh_host.data(), ctx->inst_mesh_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        LRK_CUDA(cudaMemcpyAsync(a.visible_ids.get(), ctx->visible_host.data(), ctx->visible_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        blas_root_bounds_kernel<<<build_blocks(ctx->mesh_count), 256, 0, stream>>>(a.meshes.get<const lrk_mesh>(), a.bvh_nodes.get<const float4>(), ctx->mesh_count,
+                                                                                  a.mesh_bounds.get<BuildBox>());
+        LRK_CUDA(cudaGetLastError());
+        ctx->tlas_inputs = true;
+    }
+    BuildScratch b;
+    if ((rc = reserve_build_scratch(ctx, std::max(visible, 2u), b))) return rc;
+    if ((rc = build_instance_level(ctx, b, visible, ctx->scene.tlas_root))) return rc;
+    if (emitter_moved && (rc = upload_light_sampling(ctx, ctx->light_active))) return rc;
+    LRK_CUDA(cudaStreamSynchronize(stream));// `updates` is a local; the caller may free its arrays
+    LRK_CUDA(cudaGetLastError());
+    return lrk_film_clear(ctx);
+}
+
+int lrk_update_camera(lrk_ctx *ctx, const lrk_camera *camera) {
+    if (!ctx) return LRK_ERR_INVALID_ARGUMENT;
+    if (!camera) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_camera: null camera");
+    if (!ctx->has_scene) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_camera: no scene");
+    if (camera->resolution[0] != ctx->scene.width || camera->resolution[1] != ctx->scene.height)
+        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_camera: the film size differs from the uploaded camera's (a new film size needs lrk_upload_scene)");
+    LRK_CUDA(cudaSetDevice(ctx->device));
+    LRK_CUDA(cudaMemcpyAsync(ctx->arrays.camera.get(), camera, sizeof(lrk_camera), cudaMemcpyHostToDevice, ctx->stream));
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));
+    ctx->spp_hint = camera->spp;
     return lrk_film_clear(ctx);
 }
 

@@ -14,6 +14,7 @@
 #include <map>
 #include <unordered_map>
 
+#include "../device/affine_inverse.h"
 #include "bvh.h"
 
 namespace lrh {
@@ -453,7 +454,7 @@ struct Flattener {
             encode_handle(inst.handle, mesh_index * 4u, properties, surface_tag, light_tag, medium_tag, mesh.triangle_count,
                           fixed16(has_normal ? shape->shadow_terminator : 0.f), fixed16(shape->intersection_offset));
             to_rows_3x4(o2w, inst.object_to_world);
-            if (!inverse_affine_rows(o2w, inst.world_to_object))
+            if (!lrk::inverse_affine_rows(inst.object_to_world, inst.world_to_object))
                 throw Error("Singular instance transform. [" + shape->desc()->location() + "]");
             inst.mesh = mesh_index;
             inst.visible = visible ? 1u : 0u;

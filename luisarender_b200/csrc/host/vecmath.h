@@ -75,34 +75,6 @@ inline void to_rows_3x4(const float4x4 &m, float out[12]) {
         for (int col = 0; col < 4; col++) out[r * 4 + col] = m.c[col][r];
 }
 
-// inverse of an affine transform in double precision, result as row-major 3x4
-inline bool inverse_affine_rows(const float4x4 &m, float out[12]) {
-    double a[3][3], t[3];
-    for (int r = 0; r < 3; r++) {
-        for (int col = 0; col < 3; col++) a[r][col] = m.c[col][r];
-        t[r] = m.c[3][r];
-    }
-    double det = a[0][0] * (a[1][1] * a[2][2] - a[1][2] * a[2][1]) -
-                 a[0][1] * (a[1][0] * a[2][2] - a[1][2] * a[2][0]) +
-                 a[0][2] * (a[1][0] * a[2][1] - a[1][1] * a[2][0]);
-    if (det == 0.0) return false;
-    double id = 1.0 / det, inv[3][3];
-    inv[0][0] = (a[1][1] * a[2][2] - a[1][2] * a[2][1]) * id;
-    inv[0][1] = (a[0][2] * a[2][1] - a[0][1] * a[2][2]) * id;
-    inv[0][2] = (a[0][1] * a[1][2] - a[0][2] * a[1][1]) * id;
-    inv[1][0] = (a[1][2] * a[2][0] - a[1][0] * a[2][2]) * id;
-    inv[1][1] = (a[0][0] * a[2][2] - a[0][2] * a[2][0]) * id;
-    inv[1][2] = (a[0][2] * a[1][0] - a[0][0] * a[1][2]) * id;
-    inv[2][0] = (a[1][0] * a[2][1] - a[1][1] * a[2][0]) * id;
-    inv[2][1] = (a[0][1] * a[2][0] - a[0][0] * a[2][1]) * id;
-    inv[2][2] = (a[0][0] * a[1][1] - a[0][1] * a[1][0]) * id;
-    for (int r = 0; r < 3; r++) {
-        for (int col = 0; col < 3; col++) out[r * 4 + col] = static_cast<float>(inv[r][col]);
-        out[r * 4 + 3] = static_cast<float>(-(inv[r][0] * t[0] + inv[r][1] * t[1] + inv[r][2] * t[2]));
-    }
-    return true;
-}
-
 constexpr float kPi = 3.14159265358979323846264338327950288f;
 // host-side radians(): src/compute/include/luisa/core/mathematics.h:70 (left-to-right: (deg*pi)/180)
 inline float radians(float deg) { return deg * kPi / 180.0f; }

@@ -106,14 +106,19 @@ def cornell_box(resolution=(512, 512), spp=16, depth=10, rr_depth=0, rr_threshol
 def instanced_spheres(resolution=(1920, 1080), spp=1024, seed=1, depth=10, rr_depth=0, rr_threshold=0.95,
                       big_subdivision=7, big_count=4, small_subdivision=3, small_count=60, medium=False,
                       integrator=None, sampler_seed=19980810, output="spheres.exr", emissive=0, shared_light_node=False,
-                      emission_spread=True) -> str:
+                      emission_spread=True, time=0.0) -> str:
     """Configs C3 (1920x1080 @1024), C4 (+ homogeneous medium, depth 8, 3840x2160 @4096) and C5.
     4 x 327 680 + 60 x 1 280 + 2 (ground) + 4 (lights) = 1 387 526 instanced triangles.
 
     ``emissive=K`` also makes the first K small spheres one-sided emitters (see ``many_lights``): each with its own Light node whose
     emission is log-uniform over two orders of magnitude (``emission_spread``) or 4.0, or all K sharing one node of emission 4.0
-    (``shared_light_node``).  The defaults emit the scene without them, unchanged."""
+    (``shared_light_node``).  The defaults emit the scene without them, unchanged.
+
+    ``time`` makes the scene one frame of an animation: every ``big_*`` / ``small_*`` instance is translated by ``time`` x its own
+    horizontal velocity (up to 1 unit per unit of time per axis, from a random stream of its own), so that the frames of one
+    ``seed`` share their meshes, surfaces, lights and instance order.  ``time=0.0`` emits the text of the still scene."""
     rng = np.random.default_rng(seed)
+    velocity_rng = np.random.default_rng([seed, 2])
     out = []
     emitter_of = {}
     if emissive:
@@ -165,6 +170,10 @@ def instanced_spheres(resolution=(1920, 1080), spp=1024, seed=1, depth=10, rr_de
         axis = rng.normal(size=3)
         axis /= np.linalg.norm(axis)
         angle = rng.uniform(0.0, 360.0)
+        velocity = velocity_rng.uniform(-1.0, 1.0, 2)
+        if time != 0.0:
+            p[0] += time * velocity[0]
+            p[2] += time * velocity[1]
         out.append(
             f"Shape {name} : Instance {{\n"
             f"  shape {{ @{base} }}\n"
