@@ -13,7 +13,7 @@
  *   lrk_create          <- Context::create_device + Device::create_stream      src/apps/cli.cpp:167-181
  *   lrk_upload_scene    <- Pipeline::create (Geometry::build, register_surface/light,
  *                          Integrator::build)                                    src/base/pipeline.cpp:44-99
- *   lrk_update_instances / lrk_update_camera
+ *   lrk_update_instances / lrk_update_camera / lrk_update_meshes
  *                       <- (none: an extension, the reference rebuilds its pipeline per scene)  DESIGN.md §4 (Scene updates)
  *   lrk_set_shard       <- (none: the reference is single device)               SURVEY.md §8e
  *   lrk_comm_unique_id / lrk_comm_init / lrk_reduce_film
@@ -520,10 +520,35 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *scene);
  *              leaves the scene and the film as they were.
  *   Stays:     handles, visibility, meshes, surfaces, lights, media, the environment, the sampler, and the shard assignment
  *              (lrk_set_shard, a probed lrk_balance_shards table); the reduced film stays bit-identical to one GPU's.
- * Both calls synchronise before they return: the caller's arrays can be freed afterwards.  Deforming meshes, adding or removing
- * instances and changing what an instance carries need lrk_upload_scene. */
+ * Both calls synchronise before they return: the caller's arrays can be freed afterwards.  Adding or removing instances and
+ * changing what an instance carries need lrk_upload_scene; deforming meshes needs lrk_update_meshes. */
 int lrk_update_instances(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const float *object_to_world);
 int lrk_update_camera(lrk_ctx *ctx, const lrk_camera *camera);
+
+/* Give the meshes ids[0 .. count) new vertex records; an id is an index into lrk_scene_desc::meshes. `vertices` holds, for
+ * each id in the order given, exactly meshes[id].vertex_count records (p, n, uv); `vertex_count` is their total.
+ *   Equal to:  after a successful call every render, trace, G-buffer, denoise and adaptive call gives bit for bit what it gives on
+ *              a context that uploaded the updated description: the uploaded one with each updated mesh's vertex range
+ *              vertices[vertex_offset .. +vertex_count) replaced, its tri_verts positions re-derived from the new vertices and,
+ *              for a mesh that an instance with a light uses, its alias / pdf what the flattening computes from the new triangle
+ *              areas (nothing reads the area tables of other meshes; they stay).  Only the hierarchy's bytes differ: each
+ *              updated mesh's hierarchy is refit on the device (same nodes, references and slot order, new boxes padded as the
+ *              builders pad them) and the instance level is rebuilt as lrk_update_instances rebuilds it; closest hits do not
+ *              depend on them, with the traversal's one exception: a hit that the triangle test places outside its triangle's
+ *              padded box (a grazing ray) may be kept by one hierarchy's box test and culled by another's, as between the host's
+ *              and the device's hierarchies (DESIGN.md §4).  With "light_tree" active, the light tree and its bottom trees are
+ *              rebuilt as lrk_upload_scene builds them when an emissive mesh deforms.
+ *   Shared:    a mesh id is the flattening's deduplicated mesh: every instance of that mesh deforms, including instances of
+ *              distinct scene-file shapes that the flattening merged because their vertices and triangles were equal.
+ *   Film:      the call ends with lrk_film_clear; shard assignments, a probed lrk_balance_shards table included, stay.
+ *   Refused:   LRK_ERR_INVALID_ARGUMENT for no scene, a null array with count != 0, an id >= mesh_count, a repeated id, a
+ *              vertex_count other than the sum of the meshes' vertex counts, or a non-finite position; LRK_ERR_UNSUPPORTED when the
+ *              instance level is not the hierarchy's last max(visible instances, 2) - 1 nodes.  Everything is checked before
+ *              anything changes: a refused call leaves the scene and the film as they were.
+ *   Stays:     triangles and topology, handles, visibility, surfaces, lights, media, the environment, the sampler, the camera and
+ *              the instance transforms.  A change of topology or vertex count needs lrk_upload_scene.
+ * The call synchronises before it returns: the caller's arrays can be freed afterwards. */
+int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const lrk_vertex *vertices, uint64_t vertex_count);
 
 /* Pixel-tile sharding for multi-GPU (SURVEY.md §8e): this ctx renders the tiles with
  * lrk_tile_owner(tile_id, world) == rank, tiles are tile_size x tile_size pixels in row-major tile order.

@@ -151,6 +151,32 @@ class Renderer:
             raise ValueError(f"object_to_world must be [{len(ids)}, 3, 4], not {list(rows.shape)}")
         self._check(self._lib.lrk_update_instances(self._ctx, ids.ctypes.data, len(ids), rows.ctypes.data), "lrk_update_instances")
 
+    def update_meshes(self, ids, vertices):
+        """lrk_update_meshes: give the meshes `ids` (indices into the description's meshes, the flattening's deduplicated meshes:
+        every instance of one deforms) new vertex records without a re-upload.  `vertices` has one array per id, each
+        [vertex_count of that mesh, 8] float32 (p, n, uv) or an array of the F.Vertex layout.  Afterwards every render, trace,
+        G-buffer, denoise and adaptive call gives bit for bit what a context that uploaded the updated description gives: the same
+        scene with these vertices, the triangle records and the emissive meshes' area tables derived from them.  The meshes'
+        hierarchies are refit on the device and the instance level is rebuilt; triangles and vertex counts stay.  The film is
+        cleared; a refused call (an id out of range or repeated, a wrong vertex count, a non-finite position) raises and leaves
+        the scene and the film as they were."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint32).reshape(-1)
+        vertices = list(vertices)
+        if len(vertices) != len(ids):
+            raise ValueError(f"vertices must have one array per id ({len(ids)}), not {len(vertices)}")
+        parts = []
+        for k, v in enumerate(vertices):
+            v = np.asarray(v)
+            if v.dtype.fields is not None or v.dtype == np.void:
+                if v.dtype.itemsize != C.sizeof(F.Vertex) or v.ndim != 1:
+                    raise ValueError(f"vertices[{k}] must be a 1-d array of the F.Vertex layout ({C.sizeof(F.Vertex)} bytes per record)")
+                v = np.ascontiguousarray(v).view(np.float32).reshape(-1, 8)
+            elif v.ndim != 2 or v.shape[1] != 8 or v.dtype != np.float32:
+                raise ValueError(f"vertices[{k}] must be [vertex_count, 8] float32 (p, n, uv), not {list(v.shape)} {v.dtype}")
+            parts.append(v)
+        flat = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0, 8), np.float32), dtype=np.float32)
+        self._check(self._lib.lrk_update_meshes(self._ctx, ids.ctypes.data, len(ids), flat.ctypes.data, len(flat)), "lrk_update_meshes")
+
     def update_camera(self, camera: F.Camera):
         """lrk_update_camera: replace the camera record (an lrk_camera such as ``Scene.desc().camera``) without a re-upload.
         Afterwards every call gives bit for bit what a context that uploaded the description with this camera gives.  The film is

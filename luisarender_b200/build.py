@@ -53,6 +53,7 @@ def build_host(force=False, verbose=False) -> Path:
     src_dir = PKG / "csrc" / "host"
     deps = list(src_dir.glob("*.cpp")) + list(src_dir.glob("*.h")) + list((REPO / "include").glob("*.h"))
     deps.append(PKG / "csrc" / "device" / "affine_inverse.h")  # shared with the device library (flatten.cpp)
+    deps.append(PKG / "csrc" / "device" / "alias_table.h")  # shared with the device library (flatten.cpp, geomutil users)
     if not force and _newer(out, deps):
         return out
     LIB.mkdir(exist_ok=True)
@@ -78,7 +79,8 @@ def build_device(force=False, verbose=False, name="libb200pt.so", extra_flags=()
     if os.environ.get("LRK_SHADE_FLAGS"):  # experiments (tools/build_variants.sh)
         shade_math = os.environ["LRK_SHADE_FLAGS"].split()
     objects = [obj / "lrk.o", obj / "shade_fast.o", obj / "shade_strict.o"]
-    steps = [([_nvcc(), *NVCC_ARCH, *common, "-fmad=false", "-c", src_dir / "lrk.cu", "-o", objects[0]], None),
+    # lrk.cu's host code rebuilds alias tables (alias_table.h) as the host library computes them: no FMA contraction there either
+    steps = [([_nvcc(), *NVCC_ARCH, *common, "-fmad=false", "-Xcompiler", "-ffp-contract=off", "-c", src_dir / "lrk.cu", "-o", objects[0]], None),
              ([_nvcc(), *NVCC_ARCH, *common, *shade_math, "-DLRK_SHADE_VARIANT=fast", "-c", src_dir / "shade.cu", "-o", objects[1]], None),
              ([_nvcc(), *NVCC_ARCH, *common, "-fmad=false", "-DLRK_SHADE_VARIANT=strict", "-c", src_dir / "shade.cu", "-o", objects[2]], None)]
     procs = []

@@ -17,13 +17,10 @@
 #pragma once
 #include <cub/device/device_radix_sort.cuh>
 
+#include "bvh_refit.h"
 #include "scene.cuh"
 
 namespace lrk {
-
-struct BuildBox {
-    float lo[3], hi[3];
-};
 
 // order-preserving float <-> uint mapping for atomicMin / atomicMax
 __device__ __forceinline__ uint32_t float_key(float f) {

@@ -23,6 +23,7 @@
 #include "gbuffer.cuh"
 #include "denoise.cuh"
 #include "affine_inverse.h"
+#include "alias_table.h"
 #include <cub/device/device_scan.cuh>
 
 using namespace lrk;
@@ -65,7 +66,7 @@ private:
 struct DeviceArrays {
     DeviceBuffer vertices, triangles, alias, pdf, meshes, inst_handles, inst_kind, inst_o2w, inst_xform, bvh_nodes, traversal_overflow, sobol, vdc, vdc_inv, pmj, blue_noise, pmj_pixels, zsobol_hash, sampler, build_scratch, mesh_bounds, inst_mesh, visible_ids, scene_copy, media, textures, texels, env_alias, env_pdf,
         tri_verts, surfaces, lights, light_handles, camera, lt_nodes, lt_light_inst, lt_trail, lt_inst_light, lt_bottom_nodes, lt_inst_bottom,
-        lt_bottom_trail, update_staging;
+        lt_bottom_trail, update_staging, mesh_staging, mesh_refit, refit_starts, refit_scratch, refit_visits;
 };
 
 enum KernelCategory { CAT_TRACE_CLOSEST = 0, CAT_TRACE_SHADOW = 1, CAT_SHADE = 2, CAT_OTHER = 3, CAT_COUNT = 4 };
@@ -76,7 +77,7 @@ struct TimedLaunch {
 };
 
 // What the light tree of the option "light_tree" and its bottom trees are built from, copied from the scene description by
-// lrk_upload_scene so that lrk_update_instances rebuilds them with the same code: per instance that carries a light (in instance
+// lrk_upload_scene so that lrk_update_instances / lrk_update_meshes rebuild them with the same code: per instance that carries a light (in instance
 // order) its mesh, object-to-world rows, power (luminance of the emission x the light's scale) and sidedness, and per such mesh
 // the object-space positions of its triangles' vertices (9 floats per triangle).
 struct LightTreeSource {
@@ -168,6 +169,14 @@ struct lrk_ctx {
     uint32_t mesh_count{0};
     uint64_t bvh_node_count{0};// of the uploaded hierarchy, whose last max(visible, 2) - 1 nodes are the instance level
     bool tlas_inputs{false};// a.inst_mesh, a.visible_ids and a.mesh_bounds hold the scene's (device_bvh, or since the first update)
+    // mesh updates (lrk_update_meshes): the uploaded mesh table and, per mesh, whether an instance with a light uses it; derived on a
+    // mesh's first update and kept until the next upload: its refit's start nodes (the reachable inner nodes of its hierarchy
+    // without inner children) at refit_start[m] in a.refit_starts, and an emissive mesh's triangles
+    std::vector<lrk_mesh> meshes_host;
+    std::vector<uint8_t> mesh_emissive;
+    std::vector<uint32_t> refit_starts_host;
+    std::vector<std::pair<uint32_t, uint32_t>> refit_start;// (first, count); count 0: not derived yet
+    std::map<uint32_t, std::vector<lrk_triangle>> emissive_triangles;
 
     ~lrk_ctx();
 };
@@ -698,6 +707,118 @@ __global__ void __launch_bounds__(256) blas_root_bounds_kernel(const lrk_mesh *_
     mesh_bounds[m] = box;
 }
 
+// One entry of lrk_update_meshes' table, one per updated mesh in call order.  The call's vertices, triangle slots and refit start
+// nodes are numbered consecutively over the entries: entry k owns those from its *_begin to the next entry's.
+struct MeshRefit {
+    uint32_t mesh, vertex_offset, triangle_offset, slot_offset;// the mesh and its records (lrk_mesh)
+    uint32_t vertex_begin, slot_begin, start_begin;// its first staged vertex, call slot and call start node
+    uint32_t start_first;// its start nodes in a.refit_starts
+};
+
+// The entry that owns item i of the call: the last entry whose `begin` is <= i (entry 0 begins at 0)
+template<uint32_t MeshRefit::*Begin>
+__device__ __forceinline__ uint32_t refit_entry(const MeshRefit *__restrict__ entries, uint32_t count, uint32_t i) {
+    uint32_t lo = 0u, hi = count;
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) / 2u;
+        if (entries[mid].*Begin <= i) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// The staged vertices of every updated mesh into its vertex range
+__global__ void __launch_bounds__(256) update_vertices_kernel(const MeshRefit *__restrict__ entries, uint32_t count, const lrk_vertex *__restrict__ staged,
+                                                              uint32_t n, lrk_vertex *__restrict__ vertices) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const MeshRefit e = entries[refit_entry<&MeshRefit::vertex_begin>(entries, count, i)];
+    vertices[e.vertex_offset + (i - e.vertex_begin)] = staged[i];
+}
+
+// The triangle records of every slot of the updated meshes, in their uploaded BVH order (v0.w keeps the primitive id), from the new
+// vertices as build_tri_verts_kernel writes them; the slot's triangle box goes to slot_boxes[call slot] and grows the mesh's bounds
+// (6 keys per entry, grow_whole)
+__global__ void __launch_bounds__(256) refit_triangles_kernel(const MeshRefit *__restrict__ entries, uint32_t count, uint32_t n,
+                                                              const lrk_vertex *__restrict__ vertices, const lrk_triangle *__restrict__ triangles,
+                                                              float4 *__restrict__ tri_verts, BuildBox *__restrict__ slot_boxes, uint32_t *whole) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t k = refit_entry<&MeshRefit::slot_begin>(entries, count, i);
+    const MeshRefit e = entries[k];
+    float4 *dst = tri_verts + static_cast<size_t>(e.slot_offset + (i - e.slot_begin)) * 3u;
+    const uint32_t prim = __float_as_uint(dst[0].w);
+    const lrk_triangle t = triangles[e.triangle_offset + prim];
+    const lrk_vertex *v = vertices + e.vertex_offset;
+    const float *p0 = v[t.i0].p, *p1 = v[t.i1].p, *p2 = v[t.i2].p;
+    dst[0] = make_float4(p0[0], p0[1], p0[2], __uint_as_float(prim));
+    dst[1] = make_float4(p1[0], p1[1], p1[2], 0.f);
+    dst[2] = make_float4(p2[0], p2[1], p2[2], 0.f);
+    const BuildBox b = refit_triangle_box(p0, p1, p2);
+    slot_boxes[i] = b;
+    grow_whole(whole + 6u * k, b);
+}
+
+__device__ __forceinline__ bool refit_inner(uint32_t ref) { return (ref & LRK_BVH_LEAF) == 0u; }// LRK_BVH_EMPTY has the leaf bit
+
+// A box another thread of this launch wrote: through L2, never a stale L1 line
+__device__ __forceinline__ BuildBox refit_load_box(const BuildBox *b) {
+    const float *f = b->lo;
+    BuildBox r;
+    for (int a = 0; a < 3; a++) { r.lo[a] = __ldcg(f + a); r.hi[a] = __ldcg(f + 3 + a); }
+    return r;
+}
+
+// The bottom-up refit of the updated meshes' hierarchies (bvh_refit.h), with build_fit_kernel's arrival counters: one thread per
+// start node (a reachable inner node without inner children) walks towards the root; a node with two inner children is computed
+// by the second thread to arrive.  Every node keeps its references and parent and gets new padded child boxes; its unpadded
+// box goes to node_boxes[node] for its parent.  Only nodes reachable from a mesh's root are read or written: a device-built
+// hierarchy's range also holds Karras nodes of collapsed subtrees that were never written.  The thread that computes a counter's
+// node resets the counter, so `visits` is all zero again when the launch ends.  At the root, the mesh's bounds for the instance
+// level: the union of the root's stored boxes, as blas_root_bounds_kernel derives them.
+__global__ void __launch_bounds__(256) refit_nodes_kernel(const MeshRefit *__restrict__ entries, uint32_t count, uint32_t n,
+                                                          const uint32_t *__restrict__ starts, const uint32_t *__restrict__ whole,
+                                                          const BuildBox *__restrict__ slot_boxes, BuildBox *node_boxes, uint32_t *visits, float4 *nodes,
+                                                          BuildBox *__restrict__ mesh_bounds) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t k = refit_entry<&MeshRefit::start_begin>(entries, count, i);
+    const MeshRefit e = entries[k];
+    BuildBox bounds;
+    for (int a = 0; a < 3; a++) { bounds.lo[a] = key_float(whole[6u * k + a]); bounds.hi[a] = key_float(whole[6u * k + 3u + a]); }
+    const float pad = refit_pad(refit_extent(bounds));
+    uint32_t node = starts[e.start_first + (i - e.start_begin)];
+    for (;;) {
+        float4 *dst = nodes + static_cast<size_t>(node) * 4u;
+        const float4 r = dst[3];
+        const uint32_t ref[2] = {__float_as_uint(r.x), __float_as_uint(r.y)}, parent = __float_as_uint(r.z);
+        BuildBox box[2];
+        for (int c = 0; c < 2; c++) {
+            if (ref[c] == LRK_BVH_EMPTY) box[c] = refit_empty_box();
+            else if (ref[c] & LRK_BVH_LEAF) box[c] = refit_leaf_box(slot_boxes + e.slot_begin + ((ref[c] & 0x0fffffffu) - e.slot_offset), ((ref[c] >> 28u) & 7u) + 1u);
+            else box[c] = refit_load_box(node_boxes + ref[c]);
+        }
+        node_boxes[node] = refit_union(box[0], box[1]);
+        const BuildBox s0 = refit_padded(box[0], pad), s1 = refit_padded(box[1], pad);
+        float f[12];
+        refit_node_boxes(s0, s1, f);
+        dst[0] = make_float4(f[0], f[1], f[2], f[3]);
+        dst[1] = make_float4(f[4], f[5], f[6], f[7]);
+        dst[2] = make_float4(f[8], f[9], f[10], f[11]);
+        if (parent == LRK_BVH_EMPTY) {
+            mesh_bounds[e.mesh] = refit_union(s0, s1);
+            return;
+        }
+        __threadfence();// the box written above is visible before the arrival is counted
+        const float4 pr = nodes[static_cast<size_t>(parent) * 4u + 3u];
+        const uint32_t inner = (refit_inner(__float_as_uint(pr.x)) ? 1u : 0u) + (refit_inner(__float_as_uint(pr.y)) ? 1u : 0u);
+        if (atomicAdd(visits + parent, 1u) + 1u < inner) return;
+        visits[parent] = 0u;
+        __threadfence();
+        node = parent;
+    }
+}
+
 // The triangles of an emissive mesh (LightTreeSource::mesh_points), 9 doubles each: in world space through the row-major 3x4
 // object-to-world matrix m, or in object space when m is null.
 void gather_triangles(const std::vector<float> &points, const float *m, std::vector<double> &tris) {
@@ -877,6 +998,78 @@ int upload_light_sampling(lrk_ctx *ctx, const LightSampling want) {
     LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get<char>() + sizeof(DeviceScene), &rec, sizeof(DeviceLightTree), cudaMemcpyHostToDevice, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));// the host arrays and `rec` are locals
     ctx->light_active = want;
+    return LRK_OK;
+}
+
+// Scene updates rebuild the instance level in place: the host's SAH build with one instance per leaf and the device's LBVH both
+// emit max(visible, 2) - 1 nodes, behind every mesh's BLAS.  Checked before an update changes anything.
+int check_instance_level(lrk_ctx *ctx, const char *call) {
+    const uint32_t visible = static_cast<uint32_t>(ctx->visible_host.size());
+    if (static_cast<uint64_t>(ctx->scene.tlas_root) + std::max(visible, 2u) - 1u != ctx->bvh_node_count)
+        return fail(ctx, LRK_ERR_UNSUPPORTED, std::string(call) + ": the uploaded hierarchy's instance level is not its last max(visible instances, 2) - 1 "
+                                                                 "nodes, so it cannot be rebuilt in place");
+    return LRK_OK;
+}
+
+// The common end of lrk_update_instances and lrk_update_meshes, once the instances' rows or the meshes' vertices and hierarchies
+// are new: the first update's instance-level inputs (a host-built hierarchy: the per-instance meshes, the visible ids and the
+// meshes' bounds from their BLAS roots), the instance level, the light sampling when an emitter changed, and the film clear.
+int finish_scene_update(lrk_ctx *ctx, bool lights_changed) {
+    auto &a = ctx->arrays;
+    auto stream = ctx->stream;
+    int rc;
+    if (!ctx->tlas_inputs) {
+        LRK_CUDA(a.inst_mesh.reserve(std::max<size_t>(ctx->inst_mesh_host.size() * sizeof(uint32_t), 16u)));
+        LRK_CUDA(a.visible_ids.reserve(std::max<size_t>(ctx->visible_host.size() * sizeof(uint32_t), 16u)));
+        LRK_CUDA(a.mesh_bounds.reserve(std::max<size_t>(ctx->mesh_count, 1u) * sizeof(BuildBox)));
+        LRK_CUDA(cudaMemcpyAsync(a.inst_mesh.get(), ctx->inst_mesh_host.data(), ctx->inst_mesh_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        LRK_CUDA(cudaMemcpyAsync(a.visible_ids.get(), ctx->visible_host.data(), ctx->visible_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        blas_root_bounds_kernel<<<build_blocks(ctx->mesh_count), 256, 0, stream>>>(a.meshes.get<const lrk_mesh>(), a.bvh_nodes.get<const float4>(), ctx->mesh_count,
+                                                                                  a.mesh_bounds.get<BuildBox>());
+        LRK_CUDA(cudaGetLastError());
+        ctx->tlas_inputs = true;
+    }
+    const uint32_t visible = static_cast<uint32_t>(ctx->visible_host.size());
+    BuildScratch b;
+    if ((rc = reserve_build_scratch(ctx, std::max(visible, 2u), b))) return rc;
+    if ((rc = build_instance_level(ctx, b, visible, ctx->scene.tlas_root))) return rc;
+    if (lights_changed && (rc = upload_light_sampling(ctx, ctx->light_active))) return rc;
+    LRK_CUDA(cudaStreamSynchronize(stream));// the callers' staged locals; the caller may free its arrays
+    LRK_CUDA(cudaGetLastError());
+    return lrk_film_clear(ctx);
+}
+
+// What a mesh's first update derives from the uploaded hierarchy (one download of the mesh's node range; the caller's bvh_nodes
+// may be gone): the refit's start nodes, i.e. the inner nodes reachable from its root that have no inner child.  The range ends
+// at the next mesh's root or at the instance level: both builders lay the meshes' hierarchies out one after the other.
+int derive_refit_starts(lrk_ctx *ctx, uint32_t mesh) {
+    const uint32_t root = ctx->meshes_host[mesh].bvh_root;
+    uint32_t end = ctx->scene.tlas_root;
+    for (const auto &m : ctx->meshes_host)
+        if (m.bvh_root > root && m.bvh_root < end) end = m.bvh_root;
+    std::vector<lrk_bvh_node> nodes(end - root);
+    LRK_CUDA(cudaMemcpyAsync(nodes.data(), ctx->arrays.bvh_nodes.get<const lrk_bvh_node>() + root, nodes.size() * sizeof(lrk_bvh_node), cudaMemcpyDeviceToHost,
+                             ctx->stream));
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));
+    const uint32_t first = static_cast<uint32_t>(ctx->refit_starts_host.size());
+    std::vector<uint32_t> stack{root};
+    size_t walked = 0u;
+    while (!stack.empty()) {
+        const uint32_t n = stack.back();
+        stack.pop_back();
+        if (++walked > nodes.size()) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_update_meshes: the hierarchy of mesh " + std::to_string(mesh) + " is not a tree");
+        const lrk_bvh_node &nd = nodes[n - root];
+        uint32_t inner = 0u;
+        for (const uint32_t ref : {nd.ref0, nd.ref1}) {
+            if (ref & LRK_BVH_LEAF) continue;// a leaf, or LRK_BVH_EMPTY
+            if (ref < root || ref >= end)
+                return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_update_meshes: the hierarchy of mesh " + std::to_string(mesh) + " leaves its node range");
+            stack.push_back(ref);
+            inner++;
+        }
+        if (inner == 0u) ctx->refit_starts_host.push_back(n);
+    }
+    ctx->refit_start[mesh] = {first, static_cast<uint32_t>(ctx->refit_starts_host.size()) - first};
     return LRK_OK;
 }
 
@@ -1117,6 +1310,7 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     ctx->tlas_inputs = false;
     ctx->inst_mesh_host.resize(s->instance_count);
     ctx->visible_host.clear();
+    ctx->mesh_emissive.assign(s->mesh_count, 0u);
     for (uint32_t i = 0; i < s->instance_count; i++) {
         const auto &inst = s->instances[i];
         ctx->inst_mesh_host[i] = inst.mesh;
@@ -1134,6 +1328,7 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
             if ((flags & LRK_SHAPE_MAYBE_NON_OPAQUE) && (flags & LRK_SHAPE_HAS_SURFACE)) ctx->any_non_opaque = true;
         }
         if (inst.mesh >= s->mesh_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: mesh index out of range");
+        if (inst.handle[0] & LRK_SHAPE_HAS_LIGHT) ctx->mesh_emissive[inst.mesh] = 1u;
         std::memcpy(&o2w[i * 12u], inst.object_to_world, 48);
         std::memcpy(&xform[i * 16u], inst.world_to_object, 48);
         xform[i * 16u + 12u] = xform[i * 16u + 13u] = xform[i * 16u + 14u] = xform[i * 16u + 15u] = 0.f;
@@ -1153,6 +1348,11 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         ctx->bvh_node_count = s->bvh_node_count;
     }
     ctx->mesh_count = s->mesh_count;
+    ctx->meshes_host.assign(s->meshes, s->meshes + s->mesh_count);
+    for (uint32_t m = 0; m < s->mesh_count; m++) ctx->meshes_host[m].bvh_root = mesh_root[m];// the device builder's roots with device_bvh
+    ctx->refit_starts_host.clear();
+    ctx->refit_start.assign(s->mesh_count, {0u, 0u});
+    ctx->emissive_triangles.clear();
     for (uint32_t i = 0; i < s->instance_count; i++) std::memcpy(&xform[i * 16u + 12u], &mesh_root[s->instances[i].mesh], 4);
     if ((rc = upload(ctx, a.inst_xform, xform.data(), xform.size()))) return rc;
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1273,16 +1473,10 @@ int lrk_update_instances(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, cons
         updates[k].id = id;
         std::memcpy(updates[k].o2w, m, sizeof(updates[k].o2w));
     }
-    // the instance level is rebuilt in place: the host's SAH build with one instance per leaf and the device's LBVH both emit
-    // max(visible, 2) - 1 nodes, behind every mesh's BLAS
-    const uint32_t visible = static_cast<uint32_t>(ctx->visible_host.size());
-    if (static_cast<uint64_t>(ctx->scene.tlas_root) + std::max(visible, 2u) - 1u != ctx->bvh_node_count)
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_update_instances: the uploaded hierarchy's instance level is not its last max(visible instances, 2) - 1 "
-                                              "nodes, so it cannot be rebuilt in place");
+    if (const int rc = check_instance_level(ctx, "lrk_update_instances")) return rc;
     LRK_CUDA(cudaSetDevice(ctx->device));
     auto &a = ctx->arrays;
     auto stream = ctx->stream;
-    int rc;
     bool emitter_moved = false;
     if (ctx->light_active.tree) {
         auto &src = ctx->light_source;
@@ -1300,24 +1494,121 @@ int lrk_update_instances(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, cons
                                                                         a.inst_xform.get<float4>());
         LRK_CUDA(cudaGetLastError());
     }
-    if (!ctx->tlas_inputs) {// a host-built hierarchy, first update: the per-instance meshes, the visible ids and the meshes' bounds
-        LRK_CUDA(a.inst_mesh.reserve(std::max<size_t>(ctx->inst_mesh_host.size() * sizeof(uint32_t), 16u)));
-        LRK_CUDA(a.visible_ids.reserve(std::max<size_t>(ctx->visible_host.size() * sizeof(uint32_t), 16u)));
-        LRK_CUDA(a.mesh_bounds.reserve(std::max<size_t>(ctx->mesh_count, 1u) * sizeof(BuildBox)));
-        LRK_CUDA(cudaMemcpyAsync(a.inst_mesh.get(), ctx->inst_mesh_host.data(), ctx->inst_mesh_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-        LRK_CUDA(cudaMemcpyAsync(a.visible_ids.get(), ctx->visible_host.data(), ctx->visible_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-        blas_root_bounds_kernel<<<build_blocks(ctx->mesh_count), 256, 0, stream>>>(a.meshes.get<const lrk_mesh>(), a.bvh_nodes.get<const float4>(), ctx->mesh_count,
-                                                                                  a.mesh_bounds.get<BuildBox>());
-        LRK_CUDA(cudaGetLastError());
-        ctx->tlas_inputs = true;
+    return finish_scene_update(ctx, emitter_moved);
+}
+
+int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const lrk_vertex *vertices, uint64_t vertex_count) {
+    if (!ctx) return LRK_ERR_INVALID_ARGUMENT;
+    if (!ctx->has_scene) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: no scene");
+    if (count != 0u && (!ids || !vertices)) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: null array");
+    // everything is checked before anything changes
+    std::vector<MeshRefit> entries(count);
+    std::vector<uint8_t> seen(ctx->mesh_count, 0u);
+    uint64_t total = 0u, slots = 0u;
+    for (uint32_t k = 0; k < count; k++) {
+        const uint32_t id = ids[k];
+        if (id >= ctx->mesh_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: mesh id " + std::to_string(id) + " out of range");
+        if (seen[id]) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: mesh id " + std::to_string(id) + " repeated");
+        seen[id] = 1u;
+        const lrk_mesh &m = ctx->meshes_host[id];
+        entries[k] = MeshRefit{id, m.vertex_offset, m.triangle_offset, m.tri_slot_offset, static_cast<uint32_t>(total), static_cast<uint32_t>(slots), 0u, 0u};
+        total += m.vertex_count;
+        slots += m.triangle_count;
     }
-    BuildScratch b;
-    if ((rc = reserve_build_scratch(ctx, std::max(visible, 2u), b))) return rc;
-    if ((rc = build_instance_level(ctx, b, visible, ctx->scene.tlas_root))) return rc;
-    if (emitter_moved && (rc = upload_light_sampling(ctx, ctx->light_active))) return rc;
-    LRK_CUDA(cudaStreamSynchronize(stream));// `updates` is a local; the caller may free its arrays
-    LRK_CUDA(cudaGetLastError());
-    return lrk_film_clear(ctx);
+    if (vertex_count != total)
+        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: vertex_count is " + std::to_string(vertex_count) + ", the meshes have " +
+                                                       std::to_string(total) + " vertices");
+    for (uint32_t k = 0; k < count; k++) {
+        const uint64_t end = k + 1u < count ? entries[k + 1u].vertex_begin : total;
+        for (uint64_t v = entries[k].vertex_begin; v < end; v++)
+            for (int j = 0; j < 3; j++)
+                if (!std::isfinite(vertices[v].p[j])) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: non-finite position in mesh " + std::to_string(ids[k]));
+    }
+    if (const int rc = check_instance_level(ctx, "lrk_update_meshes")) return rc;
+    LRK_CUDA(cudaSetDevice(ctx->device));
+    auto &a = ctx->arrays;
+    auto stream = ctx->stream;
+    int rc;
+    // a mesh's first update derives its refit's start nodes and, for an emissive mesh, downloads its triangles: nothing changes yet
+    bool new_starts = false;
+    for (const auto &e : entries) {
+        if (ctx->refit_start[e.mesh].second == 0u) {
+            if ((rc = derive_refit_starts(ctx, e.mesh))) return rc;
+            new_starts = true;
+        }
+        if (ctx->mesh_emissive[e.mesh] && ctx->emissive_triangles.count(e.mesh) == 0u) {
+            const lrk_mesh &m = ctx->meshes_host[e.mesh];
+            std::vector<lrk_triangle> tris(m.triangle_count);
+            LRK_CUDA(cudaMemcpyAsync(tris.data(), a.triangles.get<const lrk_triangle>() + m.triangle_offset, tris.size() * sizeof(lrk_triangle),
+                                     cudaMemcpyDeviceToHost, stream));
+            LRK_CUDA(cudaStreamSynchronize(stream));
+            ctx->emissive_triangles.emplace(e.mesh, std::move(tris));
+        }
+    }
+    if (new_starts) {// a pageable copy (not through upload(), which may page-lock the context's own vector)
+        LRK_CUDA(a.refit_starts.reserve(ctx->refit_starts_host.size() * sizeof(uint32_t)));
+        LRK_CUDA(cudaMemcpyAsync(a.refit_starts.get(), ctx->refit_starts_host.data(), ctx->refit_starts_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+    }
+    bool lights_changed = false;
+    std::vector<std::vector<lrk_alias_entry>> tables(count);// sent asynchronously: alive until finish_scene_update synchronises
+    std::vector<std::vector<float>> pdfs(count);
+    if (count != 0u) {
+        uint32_t starts = 0u;
+        for (auto &e : entries) {
+            e.start_begin = starts;
+            e.start_first = ctx->refit_start[e.mesh].first;
+            starts += ctx->refit_start[e.mesh].second;
+        }
+        std::vector<uint32_t> whole(6u * static_cast<size_t>(count));
+        for (uint32_t k = 0; k < count; k++) std::memcpy(&whole[6u * k], kWholeInit, sizeof(kWholeInit));
+        // scratch: per entry the bounds keys, per call slot its triangle box, per node of the meshes' hierarchies its unpadded box
+        const size_t whole_bytes = (whole.size() * sizeof(uint32_t) + 15u) & ~size_t{15u}, slot_bytes = slots * sizeof(BuildBox),
+                     node_bytes = static_cast<size_t>(ctx->scene.tlas_root) * sizeof(BuildBox);
+        LRK_CUDA(a.refit_scratch.reserve(whole_bytes + slot_bytes + node_bytes));
+        auto *d_whole = a.refit_scratch.get<uint32_t>();
+        auto *slot_boxes = reinterpret_cast<BuildBox *>(a.refit_scratch.get<char>() + whole_bytes);
+        auto *node_boxes = reinterpret_cast<BuildBox *>(a.refit_scratch.get<char>() + whole_bytes + slot_bytes);
+        const size_t visit_bytes = std::max<size_t>(static_cast<size_t>(ctx->scene.tlas_root) * sizeof(uint32_t), 16u);
+        if (a.refit_visits.bytes() < visit_bytes) {// zero once: every refit leaves its counters at zero
+            LRK_CUDA(a.refit_visits.reserve(visit_bytes));
+            LRK_CUDA(cudaMemsetAsync(a.refit_visits.get(), 0, visit_bytes, stream));
+        }
+        LRK_CUDA(a.mesh_staging.reserve(vertex_count * sizeof(lrk_vertex)));
+        LRK_CUDA(a.mesh_refit.reserve(entries.size() * sizeof(MeshRefit)));
+        LRK_CUDA(cudaMemcpyAsync(a.mesh_staging.get(), vertices, vertex_count * sizeof(lrk_vertex), cudaMemcpyHostToDevice, stream));
+        LRK_CUDA(cudaMemcpyAsync(a.mesh_refit.get(), entries.data(), entries.size() * sizeof(MeshRefit), cudaMemcpyHostToDevice, stream));
+        LRK_CUDA(cudaMemcpyAsync(d_whole, whole.data(), whole.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        const auto *d_entries = a.mesh_refit.get<const MeshRefit>();
+        update_vertices_kernel<<<build_blocks(vertex_count), 256, 0, stream>>>(d_entries, count, a.mesh_staging.get<const lrk_vertex>(),
+                                                                               static_cast<uint32_t>(vertex_count), a.vertices.get<lrk_vertex>());
+        refit_triangles_kernel<<<build_blocks(slots), 256, 0, stream>>>(d_entries, count, static_cast<uint32_t>(slots), a.vertices.get<const lrk_vertex>(),
+                                                                        a.triangles.get<const lrk_triangle>(), a.tri_verts.get<float4>(), slot_boxes, d_whole);
+        LRK_CUDA(a.mesh_bounds.reserve(std::max<size_t>(ctx->mesh_count, 1u) * sizeof(BuildBox)));
+        refit_nodes_kernel<<<build_blocks(starts), 256, 0, stream>>>(d_entries, count, starts, a.refit_starts.get<const uint32_t>(), d_whole, slot_boxes,
+                                                                     node_boxes, a.refit_visits.get<uint32_t>(), a.bvh_nodes.get<float4>(),
+                                                                     a.mesh_bounds.get<BuildBox>());
+        LRK_CUDA(cudaGetLastError());
+        // the emissive meshes' area alias tables, and their triangles in the light tree's source
+        for (uint32_t k = 0; k < count; k++) {
+            const uint32_t id = entries[k].mesh;
+            if (!ctx->mesh_emissive[id]) continue;
+            const auto &tris = ctx->emissive_triangles.at(id);
+            const lrk_vertex *v = vertices + entries[k].vertex_begin;
+            mesh_area_alias_table(v, tris.data(), tris.size(), tables[k], pdfs[k]);
+            LRK_CUDA(cudaMemcpyAsync(a.alias.get<lrk_alias_entry>() + entries[k].triangle_offset, tables[k].data(), tables[k].size() * sizeof(lrk_alias_entry),
+                                     cudaMemcpyHostToDevice, stream));
+            LRK_CUDA(cudaMemcpyAsync(a.pdf.get<float>() + entries[k].triangle_offset, pdfs[k].data(), pdfs[k].size() * sizeof(float), cudaMemcpyHostToDevice, stream));
+            if (!ctx->light_active.tree) continue;
+            const auto it = ctx->light_source.mesh_points.find(id);
+            if (it == ctx->light_source.mesh_points.end()) continue;
+            auto &points = it->second;
+            points.clear();
+            for (const lrk_triangle &t : tris)
+                for (uint32_t i : {t.i0, t.i1, t.i2}) points.insert(points.end(), v[i].p, v[i].p + 3);
+            lights_changed = true;
+        }
+    }
+    return finish_scene_update(ctx, lights_changed);
 }
 
 int lrk_update_camera(lrk_ctx *ctx, const lrk_camera *camera) {

@@ -326,7 +326,7 @@ struct Flattener {
         for (size_t i = 0; i < t.size(); i++) {
             if (t[i].i0 >= v.size() || t[i].i1 >= v.size() || t[i].i2 >= v.size()) throw Error("Triangle index out of range.");
             auto p0 = pos(t[i].i0), p1 = pos(t[i].i1), p2 = pos(t[i].i2);
-            areas[i] = std::abs(length(cross(p1 - p0, p2 - p0)));
+            areas[i] = lrk::triangle_area_weight(v[t[i].i0].p, v[t[i].i1].p, v[t[i].i2].p);
             tri_bounds[i].grow(p0); tri_bounds[i].grow(p1); tri_bounds[i].grow(p2);
             mb.grow(tri_bounds[i]);
         }

@@ -1,4 +1,4 @@
-// Host geometry helpers: alias tables and the procedural sphere.
+// Host geometry helpers: the procedural sphere (the alias tables are in ../device/alias_table.h).
 #include <algorithm>
 #include <cmath>
 #include <map>
@@ -6,40 +6,6 @@
 #include "scene.h"
 
 namespace lrh {
-
-// Alias table construction, restating src/util/sampling.cpp:38-87 (sum in double, table in float,
-// LIFO over/under work lists, leftovers forced to probability 1).
-void create_alias_table(const float *values, size_t n, std::vector<lrk_alias_entry> &table, std::vector<float> &pdf) {
-    double sum = 0.0;
-    for (size_t i = 0; i < n; i++) sum += std::abs(values[i]);
-    pdf.resize(n);
-    if (sum == 0.0) {
-        std::fill(pdf.begin(), pdf.end(), static_cast<float>(1.0 / static_cast<double>(n)));
-    } else {
-        auto inv_sum = 1.0 / sum;
-        for (size_t i = 0; i < n; i++) pdf[i] = static_cast<float>(std::abs(values[i]) * inv_sum);
-    }
-    auto ratio = static_cast<double>(n) / sum;
-    std::vector<uint32_t> over, under;
-    table.resize(n);
-    for (uint32_t i = 0; i < n; i++) {
-        auto p = static_cast<float>(values[i] * ratio);
-        table[i] = {p, i};
-        (p > 1.0f ? over : under).push_back(i);
-    }
-    while (!over.empty() && !under.empty()) {
-        auto o = over.back();
-        auto u = under.back();
-        over.pop_back();
-        under.pop_back();
-        table[o].prob -= 1.0f - table[u].prob;
-        table[u].alias = o;
-        if (table[o].prob > 1.0f) over.push_back(o);
-        else if (table[o].prob < 1.0f) under.push_back(o);
-    }
-    for (auto i : over) table[i] = {1.0f, i};
-    for (auto i : under) table[i] = {1.0f, i};
-}
 
 // ---------------------------------------------------------------- Loop subdivision (index based)
 //

@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "../../../include/lrk.h"
+#include "../device/alias_table.h"
 #include "sdl.h"
 #include "vecmath.h"
 
@@ -262,8 +263,8 @@ private:
 
 // ---- helpers shared with flatten ---------------------------------------------------------------
 
-// alias table exactly as src/util/sampling.cpp:38-87
-void create_alias_table(const float *values, size_t n, std::vector<lrk_alias_entry> &table, std::vector<float> &pdf);
+// alias table exactly as src/util/sampling.cpp:38-87 (shared with the device library's mesh updates)
+using lrk::create_alias_table;
 
 // icosphere by Loop subdivision, then projection to the unit sphere (src/shapes/sphere.cpp:60-101)
 void make_sphere(uint32_t subdivision, std::vector<lrk_vertex> &vertices, std::vector<lrk_triangle> &triangles);

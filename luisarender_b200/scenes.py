@@ -347,33 +347,45 @@ def _icosphere(subdivision: int):
 
 
 def emissive_globe(resolution=(512, 512), spp=16, subdivision=5, transform="uniform", depth=10, rr_depth=0, rr_threshold=0.95,
-                   seed=19980810, output="emissive_globe.exr") -> str:
+                   seed=19980810, output="emissive_globe.exr", wobble=None) -> str:
     """The frame of the triangle-level light trees (option "light_tree_triangles"): ``near_light``'s Matte room lit only by a
     one-sided emissive icosphere of radius 0.25 (``subdivision`` levels) whose lowest point hangs 0.15 above the desk top.  Seen
     from the desk, most of the globe faces away: an emitter whose triangles are picked by area wastes most of its shadow rays.
 
     ``transform`` places the globe: "uniform" (an SRT of uniform scale), "stretched" (a Matrix of non-uniform scale 0.3 / 0.2 /
     0.25 under a rotation) or "mirrored" (a Matrix of negative determinant that mirrors x, applied to an icosphere wound inwards,
-    so that its world-space triangles face outwards as the others do)."""
+    so that its world-space triangles face outwards as the others do).
+
+    ``wobble`` (a float) deforms the globe: it is ``_icosphere``'s InlineMesh with every vertex v scaled radially by
+    1 + wobble * sin(3 v.x + 2 v.y) * cos(4 v.z), under the same ``transform``.  Frames of different ``wobble`` share their mesh
+    layout and triangles (lrk_update_meshes); None keeps the text of the undeformed globe."""
     out = []
     shapes = _matte_room(out, "Light globe_light : Diffuse { emission : Constant { v { 9.0, 8.0, 6.5 } } two_sided { false } }")
     desk_top, gap = 0.7, 0.15
+
+    def globe_mesh(inwards=False):
+        if wobble is None and not inwards:
+            return f"Shape globe_mesh : Sphere {{ subdivision {{ {int(subdivision)} }} }}"
+        v, f = _icosphere(subdivision)
+        if wobble is not None:
+            v = v * (1.0 + float(wobble) * np.sin(3.0 * v[:, 0] + 2.0 * v[:, 1]) * np.cos(4.0 * v[:, 2]))[:, None]
+        pos = ", ".join(_fmt(c) for c in v.reshape(-1))
+        idx = ", ".join(str(int(i)) for i in (f[:, ::-1] if inwards else f).reshape(-1))
+        return f"Shape globe_mesh : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} }}"
+
     if transform == "uniform":
         r = 0.25
-        out.append(f"Shape globe_mesh : Sphere {{ subdivision {{ {int(subdivision)} }} }}")
+        out.append(globe_mesh())
         place = f"transform : SRT {{ scale {{ {_fmt(r)} }} translate {{ 0.0, {_fmt(desk_top + gap + r)}, -0.4 }} }}"
     elif transform in ("stretched", "mirrored"):
         if transform == "stretched":
-            out.append(f"Shape globe_mesh : Sphere {{ subdivision {{ {int(subdivision)} }} }}")
+            out.append(globe_mesh())
             a, b = np.radians(35.0), np.radians(20.0)
             rz = np.array([[np.cos(a), -np.sin(a), 0.0], [np.sin(a), np.cos(a), 0.0], [0.0, 0.0, 1.0]])
             ry = np.array([[np.cos(b), 0.0, np.sin(b)], [0.0, 1.0, 0.0], [-np.sin(b), 0.0, np.cos(b)]])
             m = ry @ rz @ np.diag([0.3, 0.2, 0.25])
         else:
-            v, f = _icosphere(subdivision)
-            pos = ", ".join(_fmt(c) for c in v.reshape(-1))
-            idx = ", ".join(str(int(i)) for i in f[:, ::-1].reshape(-1))  # wound inwards: the mirror turns them outwards
-            out.append(f"Shape globe_mesh : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} }}")
+            out.append(globe_mesh(inwards=True))  # wound inwards: the mirror turns them outwards
             m = np.diag([-0.25, 0.25, 0.25])
         low = np.linalg.norm(m[1])  # the lowest point of the ellipsoid lies |row y| below its centre
         t = (0.0, desk_top + gap + low, -0.4)
@@ -383,6 +395,54 @@ def emissive_globe(resolution=(512, 512), spp=16, subdivision=5, transform="unif
         raise ValueError(f"transform is 'uniform', 'stretched' or 'mirrored', not {transform!r}")
     out.append(f"Shape globe : Instance {{ shape {{ @globe_mesh }} light {{ @globe_light }} {place} }}")
     shapes.append("@globe")
+    return _matte_room_render(out, shapes, _MATTE_ROOM_CAMERA, resolution, spp, depth, rr_depth, rr_threshold, seed, output)
+
+
+def wavy_sheet_grid(segments, amplitude, time):
+    """The sheet of ``wavy_sheet``: (positions [v, 3], normals [v, 3], uvs [v, 2], triangles [t, 3]) of a grid of ``segments``
+    quads over [-0.5, 0.5]^2 in the x-z plane, raised by the wave y = amplitude sin(kx x + w t) cos(kz z + w t / 2)."""
+    nx, nz = int(segments[0]), int(segments[1])
+    x, z = np.meshgrid(np.linspace(-0.5, 0.5, nx + 1), np.linspace(-0.5, 0.5, nz + 1))
+    kx, kz, w = 2.0 * np.pi * 1.5, 2.0 * np.pi, 2.0 * np.pi * 0.5
+    y = amplitude * np.sin(kx * x + w * time) * np.cos(kz * z + 0.5 * w * time)
+    dydx = amplitude * kx * np.cos(kx * x + w * time) * np.cos(kz * z + 0.5 * w * time)
+    dydz = -amplitude * kz * np.sin(kx * x + w * time) * np.sin(kz * z + 0.5 * w * time)
+    n = np.stack([-dydx, np.ones_like(y), -dydz], axis=-1)
+    n /= np.linalg.norm(n, axis=-1, keepdims=True)
+    p = np.stack([x, y, z], axis=-1)
+    uv = np.stack([x + 0.5, z + 0.5], axis=-1)
+    a = (np.arange(nz)[:, None] * (nx + 1) + np.arange(nx)[None, :]).reshape(-1)
+    b, c, d = a + 1, a + nx + 2, a + nx + 1
+    tris = np.stack([np.stack([a, d, c], -1), np.stack([a, c, b], -1)], axis=1).reshape(-1, 3)  # cross(p1 - p0, p2 - p0) points up
+    return p.reshape(-1, 3), n.reshape(-1, 3), uv.reshape(-1, 2), tris
+
+
+def wavy_sheet(resolution=(64, 48), spp=4, segments=(24, 16), amplitude=0.08, time=0.0, emissive=False, depth=6, rr_depth=0,
+               rr_threshold=0.95, seed=19980810, output="wavy_sheet.exr") -> str:
+    """The frame of mesh deformation (lrk_update_meshes): ``near_light``'s Matte room with one Matte sheet of ``segments`` quads
+    (an InlineMesh with normals and uvs) instanced twice through one mesh - above the desk and leaning on the floor - lit by a
+    quad light under the ceiling.  ``time`` moves only the sheet's vertex positions and normals, by a travelling wave of height
+    ``amplitude``: every frame of one parameter set has the same mesh layout, triangles and instance order.  ``emissive=True``
+    makes the sheet a two-sided light and drops the ceiling light."""
+    out = []
+    light = "Light sheet_light : Diffuse { emission : Constant { v { 4.0, 3.6, 3.0 } } two_sided { true } }" if emissive else \
+        "Light lamp_light : Diffuse { emission : Constant { v { 14.0, 12.0, 9.0 } } }"
+    shapes = _matte_room(out, light)
+    if not emissive:
+        pos, idx = _mesh_props([[(-0.3, 1.98, 0.2), (-0.3, 1.98, -0.3), (0.3, 1.98, -0.3), (0.3, 1.98, 0.2)]])
+        out.append(f"Shape lamp : InlineMesh {{ positions {{ {pos} }} indices {{ {idx} }} light {{ @lamp_light }} }}")
+        shapes.append("@lamp")
+        out.append("Surface sheet : Matte { Kd : Constant { v { 0.3, 0.45, 0.7 } } }")
+    p, n, uv, tris = wavy_sheet_grid(segments, amplitude, time)
+    fmt = lambda arr: ", ".join(_fmt(c) for c in np.asarray(arr).reshape(-1))  # noqa: E731
+    out.append(f"Shape sheet_mesh : InlineMesh {{ positions {{ {fmt(p)} }} normals {{ {fmt(n)} }} uvs {{ {fmt(uv)} }} "
+               f"indices {{ {', '.join(str(int(i)) for i in tris.reshape(-1))} }} }}")
+    carry = "light { @sheet_light }" if emissive else "surface { @sheet }"
+    places = ["scale { 0.9 } rotate { 1.0, 0.0, 0.0, 12.0 } translate { -0.2, 1.15, -0.35 }",
+              "scale { 0.8 } rotate { 0.0, 0.0, 1.0, 35.0 } translate { 0.55, 0.3, 0.35 }"]
+    for k, place in enumerate(places):
+        out.append(f"Shape sheet_{k} : Instance {{ shape {{ @sheet_mesh }} {carry} transform : SRT {{ {place} }} }}")
+        shapes.append(f"@sheet_{k}")
     return _matte_room_render(out, shapes, _MATTE_ROOM_CAMERA, resolution, spp, depth, rr_depth, rr_threshold, seed, output)
 
 
