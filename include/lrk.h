@@ -519,7 +519,9 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *scene);
  *              one (a new film size needs lrk_upload_scene).  Everything is checked before anything changes: a refused call
  *              leaves the scene and the film as they were.
  *   Stays:     handles, visibility, meshes, surfaces, lights, media, the environment, the sampler, and the shard assignment
- *              (lrk_set_shard, a probed lrk_balance_shards table); the reduced film stays bit-identical to one GPU's.
+ *              (lrk_set_shard, a probed lrk_balance_shards table); the reduced film stays bit-identical to one GPU's.  The
+ *              sampler record stays the uploaded one whatever camera->spp says: with a table-driven sampler, renders stay
+ *              limited to the uploaded lrk_sampler::spp (lrk_render), and a larger spp needs lrk_upload_scene.
  * Both calls synchronise before they return: the caller's arrays can be freed afterwards.  Adding or removing instances and
  * changing what an instance carries need lrk_upload_scene; deforming meshes needs lrk_update_meshes. */
 int lrk_update_instances(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const float *object_to_world);
@@ -572,7 +574,8 @@ int lrk_set_shard(lrk_ctx *ctx, uint32_t rank, uint32_t world, uint32_t tile_siz
  * same table without talking to each other), counts the rays traced for the pixels of every tile, assigns the tiles to ranks with
  * lrk_assign_tiles, and makes this context render rank `rank`'s tiles from then on (until the next lrk_set_shard /
  * lrk_upload_scene); the film is cleared.  The probe costs probe_spp / spp of a frame; the reduced film is bit-identical to a
- * single-GPU render whatever the assignment.
+ * single-GPU render whatever the assignment.  probe_spp > lrk_sampler::spp for a table-driven sampler returns
+ * LRK_ERR_INVALID_ARGUMENT before the shard assignment changes (the sample range of lrk_render).
  * lrk_assign_tiles (host only, no GPU): longest-processing-time-first - tiles in order of decreasing cost (ties: lower tile id)
  * each go to the rank with the smallest load so far (ties: lower rank); owner[t] = rank of tile t. */
 int lrk_balance_shards(lrk_ctx *ctx, uint32_t rank, uint32_t world, uint32_t tile_size, uint32_t probe_spp);
@@ -651,7 +654,11 @@ int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value);
 int lrk_film_clear(lrk_ctx *ctx);
 
 /* Render sample indices [spp_begin, spp_end) of every pixel of this ctx's shard and add
- * them to the film.  Asynchronous work is synchronised before returning. */
+ * them to the film.  Asynchronous work is synchronised before returning.
+ * Sample range: the table-driven samplers (PMJ02BN, SOBOL, PADDED_SOBOL, ZSOBOL) are defined for the indices [0, spp) of the
+ * uploaded lrk_sampler::spp only; spp_end > spp returns LRK_ERR_INVALID_ARGUMENT (the message names the sampler and its spp)
+ * before anything runs, on every shard alike, and the film, stats and shard assignment stay.  An empty range with spp_end <= spp
+ * is valid.  The INDEPENDENT sampler takes any range. */
 int lrk_render(lrk_ctx *ctx, uint32_t spp_begin, uint32_t spp_end);
 
 /* Adaptive sampling (an extension: the reference has none; DESIGN.md §4 (Adaptive sampling)).  lrk_render_adaptive clears the film and renders
@@ -667,7 +674,8 @@ int lrk_render(lrk_ctx *ctx, uint32_t spp_begin, uint32_t spp_end);
  *           stops when the maximum e over its pixels is strictly below `threshold`.  threshold = 0 never stops a block before
  *           max_spp, even one without any noise.  Decisions depend on the block's own pixels only, so a sharded, reduced render
  *           equals a single-GPU one bit for bit.
- * LRK_ERR_INVALID_ARGUMENT: min_spp < 2, max_spp < min_spp, a negative or non-finite threshold.  lrk_stats::samples counts the
+ * LRK_ERR_INVALID_ARGUMENT: min_spp < 2, max_spp < min_spp, a negative or non-finite threshold, and max_spp > lrk_sampler::spp
+ * for a table-driven sampler (the sample range of lrk_render), all before the film is cleared.  lrk_stats::samples counts the
  * samples rendered.  The moments buffer (8 B per pixel) and the count buffer are allocated by the first call. */
 typedef struct lrk_adaptive {
     uint32_t min_spp, max_spp;

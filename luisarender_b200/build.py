@@ -10,6 +10,7 @@ import os
 import shutil
 import subprocess
 import sys
+import time
 from pathlib import Path
 
 PKG = Path(__file__).resolve().parent
@@ -17,6 +18,9 @@ REPO = PKG.parent
 LIB = PKG / "lib"
 HOST_SRC = ["sdl.cpp", "scene.cpp", "geomutil.cpp", "bvh.cpp", "flatten.cpp", "imageio.cpp", "imageload.cpp", "jpegload.cpp", "meshload.cpp", "envmap.cpp", "lrh.cpp"]
 NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+# the strict shade.cu object takes about 12 minutes on 8 cores: the device build reports progress at this interval, so that a
+# caller watching its output can tell a long compile from a hung one
+PROGRESS_SECONDS = 60
 # -fmad=false: expressions evaluate as written (see csrc/device/vecmath.cuh); FMAs are explicit fmaf().
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-fmad=false", "--shared", "-Xcompiler", "-fPIC"]
 SHADE_MATH = ["--use_fast_math"]  # arithmetic of shade.cu (see its header)
@@ -84,12 +88,20 @@ def build_device(force=False, verbose=False, name="libb200pt.so", extra_flags=()
              ([_nvcc(), *NVCC_ARCH, *common, *shade_math, "-DLRK_SHADE_VARIANT=fast", "-c", src_dir / "shade.cu", "-o", objects[1]], None),
              ([_nvcc(), *NVCC_ARCH, *common, "-fmad=false", "-DLRK_SHADE_VARIANT=strict", "-c", src_dir / "shade.cu", "-o", objects[2]], None)]
     procs = []
+    start = time.monotonic()
     for cmd, _ in steps:  # the three objects compile side by side
         if verbose:
             print("+", " ".join(str(c) for c in cmd), flush=True)
         procs.append((cmd, subprocess.Popen([str(c) for c in cmd], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
+    print(f"[build] compiling {', '.join(o.name for o in objects)} for sm_90a", flush=True)
     for cmd, proc in procs:
-        text, _ = proc.communicate()
+        while True:
+            try:
+                text, _ = proc.communicate(timeout=PROGRESS_SECONDS)
+                break
+            except subprocess.TimeoutExpired:
+                print(f"[build] still compiling {Path(cmd[-1]).name} ({time.monotonic() - start:.0f} s)", flush=True)
+        print(f"[build] {Path(cmd[-1]).name} done ({time.monotonic() - start:.0f} s)", flush=True)
         if proc.returncode != 0:
             sys.stderr.write(text)
             raise RuntimeError(f"build step failed: {' '.join(str(c) for c in cmd[:3])} ...")

@@ -100,6 +100,7 @@ struct lrk_ctx {
     DeviceArrays arrays;
     DeviceScene scene{};
     uint32_t spp_hint{0};
+    uint32_t sampler_spp{0};// lrk_sampler::spp of the uploaded scene: the table-driven samplers take the sample indices [0, spp)
     // sharding
     uint32_t rank{0}, world{1}, tile_size{32};
     DeviceBuffer d_pixel_list;
@@ -1413,6 +1414,7 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     sc.width = s->camera.resolution[0];
     sc.height = s->camera.resolution[1];
     ctx->spp_hint = s->camera.spp;
+    ctx->sampler_spp = s->sampler.spp;
     if (sc.refill_below == 0u) sc.refill_below = static_cast<uint32_t>(kRefillBelow);
     if (sc.inner_min == 0u) sc.inner_min = static_cast<uint32_t>(kInnerMin);
     ctx->volume = s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH;
@@ -1611,6 +1613,17 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
     return finish_scene_update(ctx, lights_changed);
 }
 
+// The table-driven samplers are defined for the sample indices [0, lrk_sampler::spp) that the uploaded record was derived for: past
+// them PMJ02BN reads another tile position's pixel samples (past the end of its table for the last one) and ZSobol's index runs into
+// the Morton bits of the next pixel.  Independent takes any index.
+static int check_sample_range(lrk_ctx *ctx, uint32_t spp_end, const char *what) {
+    static const char *const names[] = {"Independent", "PMJ02BN", "Sobol", "PaddedSobol", "ZSobol"};
+    if (ctx->scene.sampler_type == LRK_SAMPLER_INDEPENDENT || spp_end <= ctx->sampler_spp) return LRK_OK;
+    return fail(ctx, LRK_ERR_INVALID_ARGUMENT, std::string(what) + ": sample index " + std::to_string(spp_end - 1u) + " is outside the " +
+                names[ctx->scene.sampler_type] + " sampler's spp " + std::to_string(ctx->sampler_spp) +
+                " (a larger spp needs lrk_upload_scene)");
+}
+
 int lrk_update_camera(lrk_ctx *ctx, const lrk_camera *camera) {
     if (!ctx) return LRK_ERR_INVALID_ARGUMENT;
     if (!camera) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_camera: null camera");
@@ -1644,6 +1657,7 @@ int lrk_balance_shards(lrk_ctx *ctx, uint32_t rank, uint32_t world, uint32_t til
         return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_balance_shards: invalid arguments");
     if (!ctx->has_scene) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_balance_shards: no scene");
     if (ctx->volume) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_balance_shards: the cost probe runs the surface integrator's kernels");
+    if (int rc = check_sample_range(ctx, probe_spp, "lrk_balance_shards")) return rc;
     LRK_CUDA(cudaSetDevice(ctx->device));
     // the probe: the whole frame on this context
     ctx->tile_owner.clear();
@@ -1813,6 +1827,7 @@ static int finish_render(lrk_ctx *ctx, const std::string &what, uint64_t samples
 int lrk_render(lrk_ctx *ctx, uint32_t spp_begin, uint32_t spp_end) {
     if (!ctx || !ctx->has_scene) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_render: no scene");
     if (spp_end < spp_begin) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_render: spp_end < spp_begin");
+    if (int rc = check_sample_range(ctx, spp_end, "lrk_render")) return rc;
     LRK_CUDA(cudaSetDevice(ctx->device));
     const uint32_t npix = ctx->npix_owned;
     if (npix == 0u || spp_end == spp_begin) return LRK_OK;
@@ -1853,7 +1868,9 @@ int lrk_render_adaptive(lrk_ctx *ctx, const lrk_adaptive *p) {
     if (!ctx || !ctx->has_scene) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_render_adaptive: no scene");
     if (!p || p->min_spp < 2u || p->max_spp < p->min_spp || !(p->threshold >= 0.f) || !std::isfinite(p->threshold))
         return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_render_adaptive: needs 2 <= min_spp <= max_spp and a finite threshold >= 0");
-    int rc = check_gbuffer_supported(ctx, ctx->gbuffer_option, "lrk_render_adaptive");
+    int rc = check_sample_range(ctx, p->max_spp, "lrk_render_adaptive");
+    if (rc) return rc;
+    rc = check_gbuffer_supported(ctx, ctx->gbuffer_option, "lrk_render_adaptive");
     if (rc) return rc;
     if ((rc = lrk_film_clear(ctx))) return rc;
     if (rc) return rc;

@@ -78,6 +78,7 @@ def lib() -> C.CDLL:
         _lib.oracle_texture_evaluate.restype = None
         _lib.oracle_resolve_surface.argtypes = [vp, C.c_uint32, f32p, vp]
         _lib.oracle_resolve_surface.restype = None
+        _lib.oracle_sampler_state.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint32, C.c_uint32, vp, vp, vp]
     return _lib
 
 
@@ -94,6 +95,9 @@ def render(desc, spp_begin: int, spp_end: int, threads: int = 0, rank: int = 0, 
     c = Counters()
     rc = lib().oracle_render(C.byref(desc), spp_begin, spp_end, threads, rank, world, tile_size,
                              film_raw.ctypes.data, C.byref(c))
+    if rc == -2:
+        raise ValueError(f"oracle_render: sample indices [{spp_begin}, {spp_end}) exceed the table-driven sampler's spp "
+                         f"{desc.sampler.spp}")
     if rc != 0:
         raise RuntimeError(f"oracle_render failed: {rc}")
     return film_raw, c.as_dict()
@@ -116,6 +120,23 @@ def li(desc, px: int, py: int, sample: int) -> np.ndarray:
     out = np.zeros(3, dtype=np.float32)
     lib().oracle_li(C.byref(desc), px, py, sample, _fp(out))
     return out
+
+
+def sampler_state(desc, points, dims=(), bounces: int = 0):
+    """oracle_sampler_state at points [n,3] (px, py, sample index).  Returns (derived index uint64[n], scrambled ZSobol index
+    uint64[n, len(dims)] at the dimensions `dims`, draws float32[n, 2 + 6 * bounces]: the pixel 2D, then 1D, 2D, 1D, 2D per
+    bounce)."""
+    points = np.ascontiguousarray(points, dtype=np.uint32).reshape(-1, 3)
+    dims = np.ascontiguousarray(dims, dtype=np.uint32)
+    n = points.shape[0]
+    index = np.zeros(n, dtype=np.uint64)
+    zsobol = np.zeros((n, dims.size), dtype=np.uint64)
+    draws = np.zeros((n, 2 + 6 * bounces), dtype=np.float32)
+    rc = lib().oracle_sampler_state(C.byref(desc), points.ctypes.data, n, dims.ctypes.data, dims.size, bounces, index.ctypes.data,
+                                    zsobol.ctypes.data, draws.ctypes.data)
+    if rc != 0:
+        raise ValueError(f"oracle_sampler_state failed: {rc}")
+    return index, zsobol, draws
 
 
 def trace(desc, rays: np.ndarray, any_hit: bool = False, brute: bool = False):

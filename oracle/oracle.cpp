@@ -2864,6 +2864,8 @@ int oracle_render(const lrk_scene_desc *scene, uint32_t spp_begin, uint32_t spp_
     } else if (scene->integrator.type != LRK_INTEGRATOR_PATH || scene->environment_medium.present) {
         return -5;
     }
+    // the table-driven samplers are defined for the sample indices [0, spp) that Sampler::Instance::reset prepared them for
+    if (scene->sampler.type != LRK_SAMPLER_INDEPENDENT && spp_end > scene->sampler.spp) return -2;
     const uint32_t W = scene->camera.resolution[0], H = scene->camera.resolution[1];
     if (threads == 0u) threads = std::max(1u, std::thread::hardware_concurrency());
     // Work items: the 8x8-pixel blocks this shard OWNS, listed up front and handed out through one atomic cursor.  (Round 1
@@ -2999,6 +3001,38 @@ void oracle_generate_ray(const lrk_scene_desc *scene, uint32_t px, uint32_t py, 
     *ray = generate_camera_ray(scene->camera, px, py, u0, u1, w);
     weight[0] = weight[1] = weight[2] = w;
     if (rng_state) *rng_state = s.state;
+}
+
+int oracle_sampler_state(const lrk_scene_desc *scene, const uint32_t *points, uint64_t n, const uint32_t *dims, uint32_t dim_count,
+                         uint32_t bounces, uint64_t *index_out, uint64_t *zsobol_out, float *draws_out) {
+    if (!scene || !points || !index_out || !zsobol_out || !draws_out || (dim_count != 0u && !dims)) return -1;
+    const lrk_sampler &cfg = scene->sampler;
+    for (uint64_t i = 0; i < n; i++)// PMJ02BN's pixel samples exist for [0, spp) only
+        if (cfg.type == LRK_SAMPLER_PMJ02BN && points[3u * i + 2u] >= cfg.spp) return -2;
+    const uint32_t per_point = 2u + 6u * bounces;
+    for (uint64_t i = 0; i < n; i++) {
+        Sampler s;
+        s.start(*scene, points[3u * i], points[3u * i + 1u], points[3u * i + 2u]);
+        index_out[i] = cfg.type == LRK_SAMPLER_SOBOL || cfg.type == LRK_SAMPLER_ZSOBOL ? s.sobol_index : 0u;
+        for (uint32_t j = 0; j < dim_count; j++) {
+            uint64_t v = 0u;
+            if (cfg.type == LRK_SAMPLER_ZSOBOL) {
+                Sampler d = s;
+                d.dimension = dims[j];
+                v = d.zsobol_sample_index();
+            }
+            zsobol_out[i * dim_count + j] = v;
+        }
+        float *u = draws_out + i * per_point;
+        s.generate_pixel_2d(u[0], u[1]);
+        for (uint32_t b = 0; b < bounces; b++, u += 6) {// path_li: light selection, light point, lobe, BSDF direction
+            u[2] = s.generate_1d();
+            s.generate_2d(u[3], u[4]);
+            u[5] = s.generate_1d();
+            s.generate_2d(u[6], u[7]);
+        }
+    }
+    return 0;
 }
 
 void oracle_offset_ray_origin(const float p[3], const float n[3], float out[3]) {
@@ -3148,6 +3182,7 @@ extern "C" int oracle_unit(const char *name_c, const uint32_t *in, uint32_t *out
     Words w{in, out};
     for (int n = 0; n < count; n++) {
         if (name == "xxhash32_4") { uint32_t a = w.u(), b = w.u(), c = w.u(), d = w.u(); w.put(xxhash32_uint4(a, b, c, d)); }
+        else if (name == "permutation_element") { uint32_t i = w.u(), l = w.u(), m = w.u(), p = w.u(); w.put(Sampler::permutation_element(i, l, m, p)); }
         else if (name == "uniform_uint_to_float") { w.put(std::fmin(kOneMinusEpsilon, static_cast<float>(w.u()) * 0x1p-32f)); }
         else if (name == "lcg") { uint32_t st = w.u(); float u = lcg(st); w.put(u); w.put(st); }
         else if (name == "pcg32_seq") {
