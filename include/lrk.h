@@ -13,7 +13,7 @@
  *   lrk_create          <- Context::create_device + Device::create_stream      src/apps/cli.cpp:167-181
  *   lrk_upload_scene    <- Pipeline::create (Geometry::build, register_surface/light,
  *                          Integrator::build)                                    src/base/pipeline.cpp:44-99
- *   lrk_update_instances / lrk_update_camera / lrk_update_meshes
+ *   lrk_update_instances / lrk_update_camera / lrk_update_meshes / lrk_replace_meshes
  *                       <- (none: an extension, the reference rebuilds its pipeline per scene)  DESIGN.md §4 (Scene updates)
  *   lrk_set_shard       <- (none: the reference is single device)               SURVEY.md §8e
  *   lrk_comm_unique_id / lrk_comm_init / lrk_reduce_film
@@ -548,9 +548,41 @@ int lrk_update_camera(lrk_ctx *ctx, const lrk_camera *camera);
  *              instance level is not the hierarchy's last max(visible instances, 2) - 1 nodes.  Everything is checked before
  *              anything changes: a refused call leaves the scene and the film as they were.
  *   Stays:     triangles and topology, handles, visibility, surfaces, lights, media, the environment, the sampler, the camera and
- *              the instance transforms.  A change of topology or vertex count needs lrk_upload_scene.
+ *              the instance transforms.  A change of topology or vertex count needs lrk_replace_meshes.
  * The call synchronises before it returns: the caller's arrays can be freed afterwards. */
 int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const lrk_vertex *vertices, uint64_t vertex_count);
+
+/* Give the meshes ids[0 .. count) new vertices and triangles of any count; an id is an index into lrk_scene_desc::meshes.  Mesh
+ * ids[k] gets vertex_counts[k] vertex records (p, n, uv) and triangle_counts[k] triangles; `vertices` and `triangles` hold them
+ * for each id in the order given, one after the other.  Triangle indices are local to their mesh, as in lrk_scene_desc::triangles.
+ *   Equal to:  after a successful call every render, trace, G-buffer, denoise and adaptive call gives bit for bit what it gives on
+ *              a context that uploaded the replaced description: the uploaded one with each replaced mesh's vertex and triangle
+ *              ranges replaced and the vertex, triangle, alias, pdf and tri_verts arrays laid out again in mesh order, so that
+ *              vertex_offset, triangle_offset and tri_slot_offset are prefix sums over the meshes' new counts; each replaced mesh's
+ *              lrk_mesh counts are the new ones, the handles of its instances carry its new triangle count (handle[2]), and, for a
+ *              mesh that an instance with a light uses, its alias / pdf are what the flattening computes from the new triangle
+ *              areas.  Only two things differ.  The hierarchy's bytes: each replaced mesh gets a hierarchy built on the device (an
+ *              LBVH), the other meshes' hierarchies move unchanged, and the instance level is rebuilt as lrk_update_instances
+ *              rebuilds it; closest hits do not depend on them, with the traversal's one exception: a hit that the triangle test
+ *              places outside its triangle's padded box (a grazing ray) may be kept by one hierarchy's box test and culled by
+ *              another's, as between the host's and the device's hierarchies (DESIGN.md §4).  And the area table of a replaced mesh
+ *              that no instance with a light uses, which nothing reads: it may hold zeros.  With "light_tree" active, the light
+ *              tree and its bottom trees are rebuilt as lrk_upload_scene builds them when an emissive mesh is replaced.
+ *   Shared:    a mesh id is the flattening's deduplicated mesh: every instance of that mesh changes.
+ *   Film:      the call ends with lrk_film_clear; shard assignments, a probed lrk_balance_shards table included, stay.
+ *   Refused:   LRK_ERR_INVALID_ARGUMENT for no scene, a null array with count != 0, an id >= mesh_count, a repeated id, a mesh
+ *              of 0 vertices or 0 triangles, a triangle index >= its mesh's new vertex count, or a non-finite position;
+ *              LRK_ERR_UNSUPPORTED when the new totals do not fit the node encoding (2^28 triangles, 2^31 - 1 nodes) or the
+ *              instance level is not the hierarchy's last max(visible instances, 2) - 1 nodes; LRK_ERR_OUT_OF_MEMORY when the
+ *              new arrays cannot be allocated.  Everything is checked and allocated before anything changes: a refused call leaves
+ *              the scene and the film as they were.
+ *   Stays:     instances, transforms, visibility, surfaces, lights, media, the environment, the sampler and the camera; mesh ids
+ *              and handle[0] (buffer_base = 4 x mesh id).  The vertex-normal and vertex-uv flags stay with the instances: a mesh
+ *              uploaded without normals still ignores n.
+ * The call synchronises before it returns: the caller's arrays can be freed afterwards.  Passing a mesh's own vertices and
+ * triangles gives it a fresh hierarchy, for example after a large deformation by lrk_update_meshes. */
+int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const uint32_t *vertex_counts, const lrk_vertex *vertices,
+                       const uint32_t *triangle_counts, const lrk_triangle *triangles);
 
 /* Pixel-tile sharding for multi-GPU (SURVEY.md §8e): this ctx renders the tiles with
  * lrk_tile_owner(tile_id, world) == rank, tiles are tile_size x tile_size pixels in row-major tile order.

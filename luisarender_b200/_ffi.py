@@ -159,7 +159,7 @@ LRK_SYMBOLS = [
     "lrk_film_device_ptr", "lrk_film_normalize_to_host", "lrk_trace", "lrk_trace_device", "lrk_get_stats",
     "lrk_stream", "lrk_comm_unique_id", "lrk_comm_init", "lrk_reduce_film", "lrk_balance_shards", "lrk_assign_tiles",
     "lrk_render_adaptive", "lrk_download_sample_counts", "lrk_download_film_variance", "lrk_download_gbuffer", "lrk_denoise",
-    "lrk_update_instances", "lrk_update_camera", "lrk_update_meshes",
+    "lrk_update_instances", "lrk_update_camera", "lrk_update_meshes", "lrk_replace_meshes",
 ]
 LRH_SYMBOLS = [
     "lrh_last_error", "lrh_scene_load", "lrh_scene_load_source", "lrh_scene_destroy", "lrh_scene_get_info",
@@ -237,5 +237,6 @@ def device_lib() -> C.CDLL:
         lib.lrk_update_instances.argtypes = [C.c_void_p, C.c_void_p, u32, C.c_void_p]
         lib.lrk_update_camera.argtypes = [C.c_void_p, C.POINTER(Camera)]
         lib.lrk_update_meshes.argtypes = [C.c_void_p, C.c_void_p, u32, C.c_void_p, C.c_uint64]
+        lib.lrk_replace_meshes.argtypes = [C.c_void_p, C.c_void_p, u32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib._lrk_typed = True
     return lib

@@ -82,6 +82,25 @@ def _macro_arrays(macros):
     return keys, vals, n
 
 
+def _vertex_parts(ids, vertices):
+    """The vertex arrays of Renderer.update_meshes / replace_meshes, one per id, each as [n, 8] float32 (p, n, uv): given so, or as
+    a 1-d array of the F.Vertex layout."""
+    vertices = list(vertices)
+    if len(vertices) != len(ids):
+        raise ValueError(f"vertices must have one array per id ({len(ids)}), not {len(vertices)}")
+    parts = []
+    for k, v in enumerate(vertices):
+        v = np.asarray(v)
+        if v.dtype.fields is not None or v.dtype == np.void:
+            if v.dtype.itemsize != C.sizeof(F.Vertex) or v.ndim != 1:
+                raise ValueError(f"vertices[{k}] must be a 1-d array of the F.Vertex layout ({C.sizeof(F.Vertex)} bytes per record)")
+            v = np.ascontiguousarray(v).view(np.float32).reshape(-1, 8)
+        elif v.ndim != 2 or v.shape[1] != 8 or v.dtype != np.float32:
+            raise ValueError(f"vertices[{k}] must be [vertex_count, 8] float32 (p, n, uv), not {list(v.shape)} {v.dtype}")
+        parts.append(v)
+    return parts
+
+
 def save_image(path: str | Path, rgba: np.ndarray) -> None:
     rgba = np.ascontiguousarray(rgba, dtype=np.float32)
     h, w = rgba.shape[0], rgba.shape[1]
@@ -161,21 +180,38 @@ class Renderer:
         cleared; a refused call (an id out of range or repeated, a wrong vertex count, a non-finite position) raises and leaves
         the scene and the film as they were."""
         ids = np.ascontiguousarray(ids, dtype=np.uint32).reshape(-1)
-        vertices = list(vertices)
-        if len(vertices) != len(ids):
-            raise ValueError(f"vertices must have one array per id ({len(ids)}), not {len(vertices)}")
-        parts = []
-        for k, v in enumerate(vertices):
-            v = np.asarray(v)
-            if v.dtype.fields is not None or v.dtype == np.void:
-                if v.dtype.itemsize != C.sizeof(F.Vertex) or v.ndim != 1:
-                    raise ValueError(f"vertices[{k}] must be a 1-d array of the F.Vertex layout ({C.sizeof(F.Vertex)} bytes per record)")
-                v = np.ascontiguousarray(v).view(np.float32).reshape(-1, 8)
-            elif v.ndim != 2 or v.shape[1] != 8 or v.dtype != np.float32:
-                raise ValueError(f"vertices[{k}] must be [vertex_count, 8] float32 (p, n, uv), not {list(v.shape)} {v.dtype}")
-            parts.append(v)
+        parts = _vertex_parts(ids, vertices)
         flat = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0, 8), np.float32), dtype=np.float32)
         self._check(self._lib.lrk_update_meshes(self._ctx, ids.ctypes.data, len(ids), flat.ctypes.data, len(flat)), "lrk_update_meshes")
+
+    def replace_meshes(self, ids, vertices, triangles):
+        """lrk_replace_meshes: give the meshes `ids` (indices into the description's meshes, the flattening's deduplicated meshes:
+        every instance of one changes) new vertices and triangles of any count without a re-upload.  `vertices` has one array per
+        id, each [n, 8] float32 (p, n, uv) or an array of the F.Vertex layout; `triangles` has one [m, 3] integer array per id,
+        indices local to that mesh.  Afterwards every render, trace, G-buffer, denoise and adaptive call gives bit for bit what a
+        context that uploaded the replaced description gives (the geometry arrays laid out again in mesh order).  The replaced
+        meshes' hierarchies are built on the device and the instance level is rebuilt; passing a mesh's own arrays gives it a
+        fresh hierarchy.  The film is cleared; a refused call (an id out of range or repeated, an empty mesh, a triangle index past
+        its mesh's vertices, a non-finite position) raises and leaves the scene and the film as they were."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint32).reshape(-1)
+        parts = _vertex_parts(ids, vertices)
+        triangles = list(triangles)
+        if len(triangles) != len(ids):
+            raise ValueError(f"triangles must have one array per id ({len(ids)}), not {len(triangles)}")
+        tri_parts = []
+        for k, t in enumerate(triangles):
+            t = np.asarray(t)
+            if t.ndim != 2 or t.shape[1] != 3 or t.dtype.kind not in "iu":
+                raise ValueError(f"triangles[{k}] must be [triangle_count, 3] integers, not {list(t.shape)} {t.dtype}")
+            if t.size and (t.min() < 0 or t.max() > 0xFFFFFFFF):
+                raise ValueError(f"triangles[{k}] has entries outside [0, 2^32)")
+            tri_parts.append(t.astype(np.uint32))
+        vertex_counts = np.array([len(v) for v in parts], np.uint32)
+        triangle_counts = np.array([len(t) for t in tri_parts], np.uint32)
+        flat = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0, 8), np.float32), dtype=np.float32)
+        tris = np.ascontiguousarray(np.concatenate(tri_parts) if tri_parts else np.zeros((0, 3), np.uint32), dtype=np.uint32)
+        self._check(self._lib.lrk_replace_meshes(self._ctx, ids.ctypes.data, len(ids), vertex_counts.ctypes.data, flat.ctypes.data,
+                                                 triangle_counts.ctypes.data, tris.ctypes.data), "lrk_replace_meshes")
 
     def update_camera(self, camera: F.Camera):
         """lrk_update_camera: replace the camera record (an lrk_camera such as ``Scene.desc().camera``) without a re-upload.

@@ -5,6 +5,9 @@
 // once by 5e-7 x the deformed mesh's extent.  Closest hits do not depend on the boxes as long as they contain their triangles, so
 // a refit hierarchy finds what a fresh build over the deformed mesh finds.
 //
+// The reference arithmetic of a hierarchy that moves to another place in bvh_nodes when lrk_replace_meshes lays the meshes out
+// again is here too (relayout_node_refs).
+//
 // Plain C++ without CUDA built-ins: tests/host_device compiles it for the host too.
 #pragma once
 #include <cmath>
@@ -78,6 +81,20 @@ LRK_REFIT_FN void refit_node_boxes(const BuildBox &c0, const BuildBox &c1, float
         out[6 + a] = c1.lo[a];
         out[9 + a] = c1.hi[a];
     }
+}
+
+// The references of one node of a mesh hierarchy that lrk_replace_meshes moves to a new place in bvh_nodes: words[0..2] are the
+// node's ref0, ref1 and parent (lrk_bvh_node).  The whole hierarchy moves by node_delta nodes and its triangle slots by
+// slot_delta (both modulo 2^32, so a move towards the front is a wrapped negative delta): an inner reference and the parent gain
+// node_delta, a leaf keeps its count bits 28..31 and its first slot gains slot_delta.  An unused child and a root's parent are
+// LRK_BVH_EMPTY (0xffffffff), which has the leaf bit: it is tested first and stays.  Boxes do not move.
+LRK_REFIT_FN void relayout_node_refs(uint32_t words[3], uint32_t node_delta, uint32_t slot_delta) {
+    for (int c = 0; c < 2; c++) {
+        const uint32_t ref = words[c];
+        if (ref == 0xffffffffu) continue;
+        words[c] = (ref & 0x80000000u) ? (ref & 0xf0000000u) | ((ref + slot_delta) & 0x0fffffffu) : ref + node_delta;
+    }
+    if (words[2] != 0xffffffffu) words[2] += node_delta;
 }
 
 }// namespace lrk

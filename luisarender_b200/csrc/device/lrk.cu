@@ -54,6 +54,10 @@ public:
         ptr_ = nullptr;
         bytes_ = 0u;
     }
+    void swap(DeviceBuffer &o) noexcept {
+        std::swap(ptr_, o.ptr_);
+        std::swap(bytes_, o.bytes_);
+    }
     template<typename T = void>
     T *get() const { return static_cast<T *>(ptr_); }
     size_t bytes() const { return bytes_; }
@@ -66,7 +70,7 @@ private:
 struct DeviceArrays {
     DeviceBuffer vertices, triangles, alias, pdf, meshes, inst_handles, inst_kind, inst_o2w, inst_xform, bvh_nodes, traversal_overflow, sobol, vdc, vdc_inv, pmj, blue_noise, pmj_pixels, zsobol_hash, sampler, build_scratch, mesh_bounds, inst_mesh, visible_ids, scene_copy, media, textures, texels, env_alias, env_pdf,
         tri_verts, surfaces, lights, light_handles, camera, lt_nodes, lt_light_inst, lt_trail, lt_inst_light, lt_bottom_nodes, lt_inst_bottom,
-        lt_bottom_trail, update_staging, mesh_staging, mesh_refit, refit_starts, refit_scratch, refit_visits;
+        lt_bottom_trail, update_staging, mesh_staging, mesh_refit, refit_starts, refit_scratch, refit_visits, node_runs;
 };
 
 enum KernelCategory { CAT_TRACE_CLOSEST = 0, CAT_TRACE_SHADOW = 1, CAT_SHADE = 2, CAT_OTHER = 3, CAT_COUNT = 4 };
@@ -625,6 +629,22 @@ int build_instance_level(lrk_ctx *ctx, const BuildScratch &b, uint32_t nv, uint3
     return build_hierarchy(ctx, b, nv, true, tlas_root, 0u);
 }
 
+// The hierarchy of mesh `m` (its records `mesh` in a.vertices / a.triangles): its bounds into a.mesh_bounds[m], its BLAS from node
+// `root` on and its triangle records from slot `slot_base` on.  b holds scratch for at least mesh.triangle_count primitives.
+int build_mesh_hierarchy(lrk_ctx *ctx, const BuildScratch &b, uint32_t m, const lrk_mesh &mesh, uint32_t root, uint32_t slot_base) {
+    auto &a = ctx->arrays;
+    auto stream = ctx->stream;
+    const uint32_t n = mesh.triangle_count;
+    auto verts = a.vertices.get<const lrk_vertex>() + mesh.vertex_offset;
+    auto tris = a.triangles.get<const lrk_triangle>() + mesh.triangle_offset;
+    LRK_CUDA(cudaMemcpyAsync(b.whole, kWholeInit, sizeof(kWholeInit), cudaMemcpyHostToDevice, stream));
+    build_triangle_bounds_kernel<<<build_blocks(n), 256, 0, stream>>>(verts, tris, n, b.boxes, b.whole);
+    build_store_mesh_bounds_kernel<<<1, 1, 0, stream>>>(b.whole, a.mesh_bounds.get<BuildBox>(), m);
+    if (const int rc = build_hierarchy(ctx, b, n, false, root, slot_base)) return rc;
+    build_tri_verts_kernel<<<build_blocks(n), 256, 0, stream>>>(verts, tris, b.vals2, n, a.tri_verts.get<float4>() + static_cast<size_t>(slot_base) * 3u);
+    return LRK_OK;
+}
+
 // Hierarchy build on the device (bvh_build.cuh): fills a.bvh_nodes / a.tri_verts from the uploaded geometry, returns the root of
 // every mesh's BLAS and of the TLAS.  One round of kernels per unique mesh, one for the instances.
 int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint32_t> &mesh_root, uint32_t &tlas_root) {
@@ -652,22 +672,13 @@ int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint3
     if ((rc = upload(ctx, a.visible_ids, visible.data(), visible.size()))) return rc;
     BuildScratch b;
     if ((rc = reserve_build_scratch(ctx, max_n, b))) return rc;
-    auto stream = ctx->stream;
     uint32_t slot_base = 0u;
     for (uint32_t m = 0; m < s->mesh_count; m++) {
-        const auto &mesh = s->meshes[m];
-        const uint32_t n = mesh.triangle_count;
-        auto verts = a.vertices.get<const lrk_vertex>() + mesh.vertex_offset;
-        auto tris = a.triangles.get<const lrk_triangle>() + mesh.triangle_offset;
-        LRK_CUDA(cudaMemcpyAsync(b.whole, kWholeInit, sizeof(kWholeInit), cudaMemcpyHostToDevice, stream));
-        build_triangle_bounds_kernel<<<build_blocks(n), 256, 0, stream>>>(verts, tris, n, b.boxes, b.whole);
-        build_store_mesh_bounds_kernel<<<1, 1, 0, stream>>>(b.whole, a.mesh_bounds.get<BuildBox>(), m);
-        if ((rc = build_hierarchy(ctx, b, n, false, mesh_root[m], slot_base))) return rc;
-        build_tri_verts_kernel<<<build_blocks(n), 256, 0, stream>>>(verts, tris, b.vals2, n, a.tri_verts.get<float4>() + static_cast<size_t>(slot_base) * 3u);
-        slot_base += n;
+        if ((rc = build_mesh_hierarchy(ctx, b, m, s->meshes[m], mesh_root[m], slot_base))) return rc;
+        slot_base += s->meshes[m].triangle_count;
     }
     if ((rc = build_instance_level(ctx, b, static_cast<uint32_t>(visible.size()), tlas_root))) return rc;
-    LRK_CUDA(cudaStreamSynchronize(stream));// the static init block is done with
+    LRK_CUDA(cudaStreamSynchronize(ctx->stream));// the static init block is done with
     LRK_CUDA(cudaGetLastError());
     ctx->tlas_inputs = true;
     return LRK_OK;
@@ -818,6 +829,49 @@ __global__ void __launch_bounds__(256) refit_nodes_kernel(const MeshRefit *__res
         __threadfence();
         node = parent;
     }
+}
+
+// One run of lrk_replace_meshes' node move: the node ranges of consecutive unchanged meshes, which move together from old_first to
+// new_first while their triangle slots move by slot_delta.  The call's moved nodes are numbered consecutively over the runs: run k
+// owns those from its `begin` to the next run's.
+struct NodeRun {
+    uint32_t old_first, new_first, slot_delta, begin;
+};
+
+// Every node of the runs from the old bvh_nodes into the new, its references moved (bvh_refit.h: relayout_node_refs) and its boxes
+// as they are.  A device-built range also holds Karras nodes that nothing references; they are moved like the others and never read.
+__global__ void __launch_bounds__(256) relayout_nodes_kernel(const NodeRun *__restrict__ runs, uint32_t count, uint32_t n, const float4 *__restrict__ old_nodes,
+                                                             float4 *__restrict__ new_nodes) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t lo = 0u, hi = count;// the last run whose begin is <= i
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) / 2u;
+        if (runs[mid].begin <= i) lo = mid;
+        else hi = mid;
+    }
+    const NodeRun r = runs[lo];
+    const float4 *src = old_nodes + static_cast<size_t>(r.old_first + (i - r.begin)) * 4u;
+    float4 *dst = new_nodes + static_cast<size_t>(r.new_first + (i - r.begin)) * 4u;
+    const float4 w = src[3];
+    uint32_t refs[3] = {__float_as_uint(w.x), __float_as_uint(w.y), __float_as_uint(w.z)};
+    relayout_node_refs(refs, r.new_first - r.old_first, r.slot_delta);
+    dst[0] = src[0];
+    dst[1] = src[1];
+    dst[2] = src[2];
+    dst[3] = make_float4(__uint_as_float(refs[0]), __uint_as_float(refs[1]), __uint_as_float(refs[2]), w.w);
+}
+
+// The instance records that follow their meshes to a new layout (lrk_replace_meshes), from the new mesh table: the BLAS root in
+// row 3 of inst_xform, as lrk_upload_scene stores it, and the triangle count in handle[2], from which the uniform light sampler
+// picks a triangle.  An instance's mesh is its handle's buffer_base / 4, as the shade kernels decode it.
+__global__ void __launch_bounds__(256) rebase_instances_kernel(const lrk_mesh *__restrict__ meshes, uint32_t n, uint4 *__restrict__ inst_handles,
+                                                               float4 *__restrict__ inst_xform) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const lrk_mesh m = meshes[(inst_handles[i].x >> 10u) >> 2u];
+    inst_handles[i].z = m.triangle_count;
+    inst_xform[i * 4u + 3u] = make_float4(__uint_as_float(m.bvh_root), 0.f, 0.f, 0.f);
 }
 
 // The triangles of an emissive mesh (LightTreeSource::mesh_points), 9 doubles each: in world space through the row-major 3x4
@@ -1609,6 +1663,226 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
                 for (uint32_t i : {t.i0, t.i1, t.i2}) points.insert(points.end(), v[i].p, v[i].p + 3);
             lights_changed = true;
         }
+    }
+    return finish_scene_update(ctx, lights_changed);
+}
+
+int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const uint32_t *vertex_counts, const lrk_vertex *vertices,
+                       const uint32_t *triangle_counts, const lrk_triangle *triangles) {
+    if (!ctx) return LRK_ERR_INVALID_ARGUMENT;
+    if (!ctx->has_scene) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_replace_meshes: no scene");
+    if (count != 0u && (!ids || !vertex_counts || !vertices || !triangle_counts || !triangles))
+        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_replace_meshes: null array");
+    // everything is checked before anything changes
+    const uint32_t mesh_count = ctx->mesh_count;
+    std::vector<uint32_t> entry(mesh_count, ~0u);// per mesh the index k of its id, ~0u for an unchanged mesh
+    std::vector<uint64_t> vertex_begin(count + 1u, 0u), triangle_begin(count + 1u, 0u);// where id k's records start in the caller's arrays
+    for (uint32_t k = 0; k < count; k++) {
+        const uint32_t id = ids[k];
+        const std::string mesh = "lrk_replace_meshes: mesh id " + std::to_string(id);
+        if (id >= mesh_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, mesh + " out of range");
+        if (entry[id] != ~0u) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, mesh + " repeated");
+        if (vertex_counts[k] == 0u || triangle_counts[k] == 0u) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, mesh + " gets no vertices or no triangles");
+        entry[id] = k;
+        vertex_begin[k + 1u] = vertex_begin[k] + vertex_counts[k];
+        triangle_begin[k + 1u] = triangle_begin[k] + triangle_counts[k];
+    }
+    for (uint32_t k = 0; k < count; k++) {
+        for (uint64_t v = vertex_begin[k]; v < vertex_begin[k + 1u]; v++)
+            for (int j = 0; j < 3; j++)
+                if (!std::isfinite(vertices[v].p[j])) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_replace_meshes: non-finite position in mesh " + std::to_string(ids[k]));
+        for (uint64_t t = triangle_begin[k]; t < triangle_begin[k + 1u]; t++)
+            if (std::max({triangles[t].i0, triangles[t].i1, triangles[t].i2}) >= vertex_counts[k])
+                return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_replace_meshes: triangle index out of range in mesh " + std::to_string(ids[k]) + " (" +
+                                                               std::to_string(vertex_counts[k]) + " vertices)");
+    }
+    if (const int rc = check_instance_level(ctx, "lrk_replace_meshes")) return rc;
+    // the new layout, in mesh order: an unchanged mesh keeps the size of its node range (from its root to the next root, or to the
+    // instance level), a replaced one gets the device builder's max(n - 1, 1) nodes; the instance level goes last
+    const uint32_t old_tlas = ctx->scene.tlas_root;
+    std::vector<uint32_t> roots(mesh_count);
+    for (uint32_t m = 0; m < mesh_count; m++) roots[m] = ctx->meshes_host[m].bvh_root;
+    std::sort(roots.begin(), roots.end());
+    std::vector<lrk_mesh> layout(ctx->meshes_host);
+    std::vector<uint32_t> node_count(mesh_count);
+    uint64_t vertex_total = 0u, triangle_total = 0u, node_total = 0u, max_n = 0u;
+    for (uint32_t m = 0; m < mesh_count; m++) {
+        lrk_mesh &r = layout[m];
+        if (entry[m] == ~0u) {
+            const auto next = std::upper_bound(roots.begin(), roots.end(), r.bvh_root);
+            node_count[m] = (next == roots.end() ? old_tlas : *next) - r.bvh_root;
+        } else {
+            r.vertex_count = vertex_counts[entry[m]];
+            r.triangle_count = triangle_counts[entry[m]];
+            node_count[m] = std::max(r.triangle_count, 2u) - 1u;
+            max_n = std::max<uint64_t>(max_n, r.triangle_count);
+        }
+        r.vertex_offset = static_cast<uint32_t>(vertex_total);
+        r.triangle_offset = r.tri_slot_offset = static_cast<uint32_t>(triangle_total);
+        r.bvh_root = static_cast<uint32_t>(node_total);
+        vertex_total += r.vertex_count;
+        triangle_total += r.triangle_count;
+        node_total += node_count[m];
+        if (vertex_total > 0xffffffffull || triangle_total >= (1ull << 28) || node_total >= 0x7fffffffull)
+            return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_replace_meshes: scene too large for the BVH encoding");
+    }
+    const uint32_t visible = static_cast<uint32_t>(ctx->visible_host.size());
+    const uint32_t tlas_root = static_cast<uint32_t>(node_total);
+    node_total += std::max(visible, 2u) - 1u;
+    if (node_total >= 0x7fffffffull) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_replace_meshes: scene too large for the BVH encoding");
+    // the unchanged meshes' records move in runs: consecutive meshes whose old ranges follow each other in every array
+    struct Run {
+        uint32_t last, old_v, new_v, vertices, old_t, new_t, old_s, triangles, old_n, new_n, nodes;
+    };
+    std::vector<Run> runs;
+    for (uint32_t m = 0; m < mesh_count; m++) {
+        if (entry[m] != ~0u) continue;
+        const lrk_mesh &o = ctx->meshes_host[m], &r = layout[m];
+        if (!runs.empty()) {
+            Run &p = runs.back();
+            if (p.last + 1u == m && p.old_v + p.vertices == o.vertex_offset && p.old_t + p.triangles == o.triangle_offset &&
+                p.old_s + p.triangles == o.tri_slot_offset && p.old_n + p.nodes == o.bvh_root) {
+                p.last = m;
+                p.vertices += o.vertex_count;
+                p.triangles += o.triangle_count;
+                p.nodes += node_count[m];
+                continue;
+            }
+        }
+        runs.push_back(Run{m, o.vertex_offset, r.vertex_offset, o.vertex_count, o.triangle_offset, r.triangle_offset, o.tri_slot_offset, o.triangle_count,
+                           o.bvh_root, r.bvh_root, node_count[m]});
+    }
+    std::vector<NodeRun> node_runs;
+    uint32_t moved_nodes = 0u;
+    for (const Run &p : runs) {
+        if (p.nodes == 0u) continue;
+        node_runs.push_back(NodeRun{p.old_n, p.new_n, p.new_t - p.old_s, moved_nodes});
+        moved_nodes += p.nodes;
+    }
+    // the emissive replaced meshes' area alias tables, from the caller's arrays (the other replaced meshes' tables are never read)
+    std::vector<std::vector<lrk_alias_entry>> tables(count);
+    std::vector<std::vector<float>> pdfs(count);
+    for (uint32_t k = 0; k < count; k++)
+        if (ctx->mesh_emissive[ids[k]]) mesh_area_alias_table(vertices + vertex_begin[k], triangles + triangle_begin[k], triangle_counts[k], tables[k], pdfs[k]);
+    // every allocation before anything changes: a refusal for memory leaves the scene as it was
+    LRK_CUDA(cudaSetDevice(ctx->device));
+    auto &a = ctx->arrays;
+    auto stream = ctx->stream;
+    DeviceBuffer nv, nt, nalias, npdf, ntv, nnodes, nmeshes;
+    {
+        const std::pair<DeviceBuffer *, uint64_t> sizes[] = {{&nv, vertex_total * sizeof(lrk_vertex)}, {&nt, triangle_total * sizeof(lrk_triangle)},
+                                                             {&nalias, triangle_total * sizeof(lrk_alias_entry)}, {&npdf, triangle_total * sizeof(float)},
+                                                             {&ntv, triangle_total * 48u}, {&nnodes, node_total * sizeof(lrk_bvh_node)},
+                                                             {&nmeshes, mesh_count * sizeof(lrk_mesh)}};
+        for (const auto &s : sizes) {
+            const cudaError_t e = s.first->reserve(std::max<uint64_t>(s.second, 16u));
+            if (e == cudaErrorMemoryAllocation) {
+                cudaGetLastError();
+                return fail(ctx, LRK_ERR_OUT_OF_MEMORY, "lrk_replace_meshes: out of device memory for the new geometry arrays (" +
+                                                            std::to_string(s.second) + " bytes); the scene is unchanged");
+            }
+            LRK_CUDA(e);
+        }
+    }
+    BuildScratch b;
+    int rc;
+    if ((rc = reserve_build_scratch(ctx, std::max<uint64_t>(max_n, std::max(visible, 2u)), b))) return rc;// the instance level's too
+    LRK_CUDA(a.mesh_bounds.reserve(std::max<size_t>(mesh_count, 1u) * sizeof(BuildBox)));
+    LRK_CUDA(a.node_runs.reserve(std::max<size_t>(node_runs.size() * sizeof(NodeRun), 16u)));
+    // the unchanged meshes: one copy per run and array, and their nodes in one launch
+    auto copy = [&](const DeviceBuffer &to, uint64_t to_off, const DeviceBuffer &from, uint64_t from_off, uint64_t bytes) {
+        return bytes ? cudaMemcpyAsync(to.get<char>() + to_off, from.get<const char>() + from_off, bytes, cudaMemcpyDeviceToDevice, stream) : cudaSuccess;
+    };
+    for (const Run &p : runs) {
+        LRK_CUDA(copy(nv, uint64_t{p.new_v} * sizeof(lrk_vertex), a.vertices, uint64_t{p.old_v} * sizeof(lrk_vertex), uint64_t{p.vertices} * sizeof(lrk_vertex)));
+        LRK_CUDA(copy(nt, uint64_t{p.new_t} * sizeof(lrk_triangle), a.triangles, uint64_t{p.old_t} * sizeof(lrk_triangle), uint64_t{p.triangles} * sizeof(lrk_triangle)));
+        LRK_CUDA(copy(nalias, uint64_t{p.new_t} * sizeof(lrk_alias_entry), a.alias, uint64_t{p.old_t} * sizeof(lrk_alias_entry),
+                      uint64_t{p.triangles} * sizeof(lrk_alias_entry)));
+        LRK_CUDA(copy(npdf, uint64_t{p.new_t} * sizeof(float), a.pdf, uint64_t{p.old_t} * sizeof(float), uint64_t{p.triangles} * sizeof(float)));
+        LRK_CUDA(copy(ntv, uint64_t{p.new_t} * 48u, a.tri_verts, uint64_t{p.old_s} * 48u, uint64_t{p.triangles} * 48u));
+    }
+    if (moved_nodes != 0u) {
+        LRK_CUDA(cudaMemcpyAsync(a.node_runs.get(), node_runs.data(), node_runs.size() * sizeof(NodeRun), cudaMemcpyHostToDevice, stream));
+        relayout_nodes_kernel<<<build_blocks(moved_nodes), 256, 0, stream>>>(a.node_runs.get<const NodeRun>(), static_cast<uint32_t>(node_runs.size()), moved_nodes,
+                                                                             a.bvh_nodes.get<const float4>(), nnodes.get<float4>());
+        LRK_CUDA(cudaGetLastError());
+    }
+    // the replaced meshes' records, and the new mesh table
+    for (uint32_t k = 0; k < count; k++) {
+        const lrk_mesh &r = layout[ids[k]];
+        LRK_CUDA(cudaMemcpyAsync(nv.get<lrk_vertex>() + r.vertex_offset, vertices + vertex_begin[k], uint64_t{r.vertex_count} * sizeof(lrk_vertex), cudaMemcpyHostToDevice, stream));
+        LRK_CUDA(cudaMemcpyAsync(nt.get<lrk_triangle>() + r.triangle_offset, triangles + triangle_begin[k], uint64_t{r.triangle_count} * sizeof(lrk_triangle),
+                                 cudaMemcpyHostToDevice, stream));
+        if (ctx->mesh_emissive[ids[k]]) {
+            LRK_CUDA(cudaMemcpyAsync(nalias.get<lrk_alias_entry>() + r.triangle_offset, tables[k].data(), tables[k].size() * sizeof(lrk_alias_entry), cudaMemcpyHostToDevice, stream));
+            LRK_CUDA(cudaMemcpyAsync(npdf.get<float>() + r.triangle_offset, pdfs[k].data(), pdfs[k].size() * sizeof(float), cudaMemcpyHostToDevice, stream));
+        } else {
+            LRK_CUDA(cudaMemsetAsync(nalias.get<lrk_alias_entry>() + r.triangle_offset, 0, uint64_t{r.triangle_count} * sizeof(lrk_alias_entry), stream));
+            LRK_CUDA(cudaMemsetAsync(npdf.get<float>() + r.triangle_offset, 0, uint64_t{r.triangle_count} * sizeof(float), stream));
+        }
+    }
+    LRK_CUDA(cudaMemcpyAsync(nmeshes.get(), layout.data(), layout.size() * sizeof(lrk_mesh), cudaMemcpyHostToDevice, stream));
+    // the new arrays become the scene's; the old ones are freed when this call returns, after finish_scene_update synchronises
+    a.vertices.swap(nv);
+    a.triangles.swap(nt);
+    a.alias.swap(nalias);
+    a.pdf.swap(npdf);
+    a.tri_verts.swap(ntv);
+    a.bvh_nodes.swap(nnodes);
+    a.meshes.swap(nmeshes);
+    for (uint32_t k = 0; k < count; k++) {
+        const lrk_mesh &r = layout[ids[k]];
+        if ((rc = build_mesh_hierarchy(ctx, b, ids[k], r, r.bvh_root, r.tri_slot_offset))) return rc;
+    }
+    if (ctx->scene.instance_count != 0u) {
+        rebase_instances_kernel<<<build_blocks(ctx->scene.instance_count), 256, 0, stream>>>(a.meshes.get<const lrk_mesh>(), ctx->scene.instance_count,
+                                                                                              a.inst_handles.get<uint4>(), a.inst_xform.get<float4>());
+        LRK_CUDA(cudaGetLastError());
+    }
+    // the host's copy of the layout: the refit starts of moved meshes move with their nodes, those of replaced meshes are derived again
+    std::vector<uint32_t> starts;
+    for (uint32_t m = 0; m < mesh_count; m++) {
+        auto &range = ctx->refit_start[m];
+        if (entry[m] != ~0u || range.second == 0u) {
+            range = {0u, 0u};
+            continue;
+        }
+        const uint32_t first = static_cast<uint32_t>(starts.size()), delta = layout[m].bvh_root - ctx->meshes_host[m].bvh_root;
+        for (uint32_t j = 0; j < range.second; j++) starts.push_back(ctx->refit_starts_host[range.first + j] + delta);
+        range.first = first;
+    }
+    ctx->refit_starts_host.swap(starts);
+    if (!ctx->refit_starts_host.empty())// a pageable copy, as lrk_update_meshes sends it; never larger than the buffer it had
+        LRK_CUDA(cudaMemcpyAsync(a.refit_starts.get(), ctx->refit_starts_host.data(), ctx->refit_starts_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+    ctx->meshes_host.swap(layout);
+    ctx->bvh_node_count = node_total;
+    auto &sc = ctx->scene;
+    sc.vertices = a.vertices.get<const lrk_vertex>();
+    sc.triangles = a.triangles.get<const lrk_triangle>();
+    sc.alias = a.alias.get<const lrk_alias_entry>();
+    sc.pdf = a.pdf.get<const float>();
+    sc.meshes = a.meshes.get<const lrk_mesh>();
+    sc.bvh_nodes = a.bvh_nodes.get<const float4>();
+    sc.tri_verts = a.tri_verts.get<const float4>();
+    sc.tlas_root = tlas_root;
+    // only the scene record: the light-tree record behind it (upload_light_sampling) stays
+    LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get(), &sc, sizeof(DeviceScene), cudaMemcpyHostToDevice, stream));
+    // the emissive replaced meshes' triangles, and their points in the light tree's source
+    bool lights_changed = false;
+    for (uint32_t k = 0; k < count; k++) {
+        const uint32_t id = ids[k];
+        if (!ctx->mesh_emissive[id]) continue;
+        const lrk_triangle *tris = triangles + triangle_begin[k];
+        ctx->emissive_triangles[id].assign(tris, tris + triangle_counts[k]);
+        if (!ctx->light_active.tree) continue;
+        const auto it = ctx->light_source.mesh_points.find(id);
+        if (it == ctx->light_source.mesh_points.end()) continue;
+        const lrk_vertex *v = vertices + vertex_begin[k];
+        auto &points = it->second;
+        points.clear();
+        for (uint32_t t = 0; t < triangle_counts[k]; t++)
+            for (uint32_t i : {tris[t].i0, tris[t].i1, tris[t].i2}) points.insert(points.end(), v[i].p, v[i].p + 3);
+        lights_changed = true;
     }
     return finish_scene_update(ctx, lights_changed);
 }
