@@ -81,7 +81,7 @@ struct TimedLaunch {
 };
 
 // What the light tree of the option "light_tree" and its bottom trees are built from, copied from the scene description by
-// lrk_upload_scene so that lrk_update_instances / lrk_update_meshes rebuild them with the same code: per instance that carries a light (in instance
+// lrk_upload_scene so that every scene update rebuilds them with the same code: per instance that carries a light (in instance
 // order) its mesh, object-to-world rows, power (luminance of the emission x the light's scale) and sidedness, and per such mesh
 // the object-space positions of its triangles' vertices (9 floats per triangle).
 struct LightTreeSource {
@@ -169,14 +169,14 @@ struct lrk_ctx {
     LightSampling light_requested, light_active;
     uint32_t *receiver_words{nullptr};// in path_allocs while light_active.receiver (alloc_paths)
     LightTreeSource light_source;// while light_active.tree
-    // scene updates (lrk_update_instances): the instance level of the hierarchy is rebuilt on the device from these
+    // every scene update (lrk_update_*, lrk_replace_meshes): the instance level of the hierarchy is rebuilt on the device from these
     std::vector<uint32_t> inst_mesh_host, visible_host;// per instance its mesh; the visible instances in order
     uint32_t mesh_count{0};
-    uint64_t bvh_node_count{0};// of the uploaded hierarchy, whose last max(visible, 2) - 1 nodes are the instance level
+    uint64_t bvh_node_count{0};// of the current hierarchy, whose last max(visible, 2) - 1 nodes are the instance level
     bool tlas_inputs{false};// a.inst_mesh, a.visible_ids and a.mesh_bounds hold the scene's (device_bvh, or since the first update)
-    // mesh updates (lrk_update_meshes): the uploaded mesh table and, per mesh, whether an instance with a light uses it; derived on a
-    // mesh's first update and kept until the next upload: its refit's start nodes (the reachable inner nodes of its hierarchy
-    // without inner children) at refit_start[m] in a.refit_starts, and an emissive mesh's triangles
+    // mesh updates and replacements: the current mesh table and, per mesh, whether an instance with a light uses it; derived on a
+    // mesh's first update and kept until the next upload or replacement: its refit's start nodes (the reachable inner nodes of its
+    // hierarchy without inner children) at refit_start[m] in a.refit_starts, and an emissive mesh's triangles
     std::vector<lrk_mesh> meshes_host;
     std::vector<uint8_t> mesh_emissive;
     std::vector<uint32_t> refit_starts_host;
@@ -727,9 +727,9 @@ struct MeshRefit {
     uint32_t start_first;// its start nodes in a.refit_starts
 };
 
-// The entry that owns item i of the call: the last entry whose `begin` is <= i (entry 0 begins at 0)
-template<uint32_t MeshRefit::*Begin>
-__device__ __forceinline__ uint32_t refit_entry(const MeshRefit *__restrict__ entries, uint32_t count, uint32_t i) {
+// The entry (MeshRefit, NodeRun) that owns item i of the call: the last entry whose `Begin` is <= i (entry 0 begins at 0)
+template<auto Begin, typename Entry>
+__device__ __forceinline__ uint32_t owning_entry(const Entry *__restrict__ entries, uint32_t count, uint32_t i) {
     uint32_t lo = 0u, hi = count;
     while (hi - lo > 1u) {
         const uint32_t mid = (lo + hi) / 2u;
@@ -744,7 +744,7 @@ __global__ void __launch_bounds__(256) update_vertices_kernel(const MeshRefit *_
                                                               uint32_t n, lrk_vertex *__restrict__ vertices) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const MeshRefit e = entries[refit_entry<&MeshRefit::vertex_begin>(entries, count, i)];
+    const MeshRefit e = entries[owning_entry<&MeshRefit::vertex_begin>(entries, count, i)];
     vertices[e.vertex_offset + (i - e.vertex_begin)] = staged[i];
 }
 
@@ -756,7 +756,7 @@ __global__ void __launch_bounds__(256) refit_triangles_kernel(const MeshRefit *_
                                                               float4 *__restrict__ tri_verts, BuildBox *__restrict__ slot_boxes, uint32_t *whole) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint32_t k = refit_entry<&MeshRefit::slot_begin>(entries, count, i);
+    const uint32_t k = owning_entry<&MeshRefit::slot_begin>(entries, count, i);
     const MeshRefit e = entries[k];
     float4 *dst = tri_verts + static_cast<size_t>(e.slot_offset + (i - e.slot_begin)) * 3u;
     const uint32_t prim = __float_as_uint(dst[0].w);
@@ -794,7 +794,7 @@ __global__ void __launch_bounds__(256) refit_nodes_kernel(const MeshRefit *__res
                                                           BuildBox *__restrict__ mesh_bounds) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint32_t k = refit_entry<&MeshRefit::start_begin>(entries, count, i);
+    const uint32_t k = owning_entry<&MeshRefit::start_begin>(entries, count, i);
     const MeshRefit e = entries[k];
     BuildBox bounds;
     for (int a = 0; a < 3; a++) { bounds.lo[a] = key_float(whole[6u * k + a]); bounds.hi[a] = key_float(whole[6u * k + 3u + a]); }
@@ -844,13 +844,7 @@ __global__ void __launch_bounds__(256) relayout_nodes_kernel(const NodeRun *__re
                                                              float4 *__restrict__ new_nodes) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    uint32_t lo = 0u, hi = count;// the last run whose begin is <= i
-    while (hi - lo > 1u) {
-        const uint32_t mid = (lo + hi) / 2u;
-        if (runs[mid].begin <= i) lo = mid;
-        else hi = mid;
-    }
-    const NodeRun r = runs[lo];
+    const NodeRun r = runs[owning_entry<&NodeRun::begin>(runs, count, i)];
     const float4 *src = old_nodes + static_cast<size_t>(r.old_first + (i - r.begin)) * 4u;
     float4 *dst = new_nodes + static_cast<size_t>(r.new_first + (i - r.begin)) * 4u;
     const float4 w = src[3];
@@ -1010,7 +1004,7 @@ int check_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
 }
 
 // The light sampling `want` of the uploaded scene, once the scene record is in a.scene_copy (lrk_upload_scene: the requested one,
-// lrk_update_instances: the active one): builds and uploads the light tree and its bottom trees from ctx->light_source where
+// the scene updates: the active one): builds and uploads the light tree and its bottom trees from ctx->light_source where
 // requested, writes the record the kernels find them through (scene.cuh: null arrays for what is off) after the scene record,
 // and latches `want` into ctx->light_active.
 int upload_light_sampling(lrk_ctx *ctx, const LightSampling want) {
@@ -1066,9 +1060,9 @@ int check_instance_level(lrk_ctx *ctx, const char *call) {
     return LRK_OK;
 }
 
-// The common end of lrk_update_instances and lrk_update_meshes, once the instances' rows or the meshes' vertices and hierarchies
-// are new: the first update's instance-level inputs (a host-built hierarchy: the per-instance meshes, the visible ids and the
-// meshes' bounds from their BLAS roots), the instance level, the light sampling when an emitter changed, and the film clear.
+// The common end of every scene update, once the instances' rows or the meshes' geometry and hierarchies are new: the first
+// update's instance-level inputs (a host-built hierarchy: the per-instance meshes, the visible ids and the meshes' bounds from
+// their BLAS roots), the instance level, the light sampling when an emitter changed, and the film clear.
 int finish_scene_update(lrk_ctx *ctx, bool lights_changed) {
     auto &a = ctx->arrays;
     auto stream = ctx->stream;
@@ -1126,6 +1120,73 @@ int derive_refit_starts(lrk_ctx *ctx, uint32_t mesh) {
     }
     ctx->refit_start[mesh] = {first, static_cast<uint32_t>(ctx->refit_starts_host.size()) - first};
     return LRK_OK;
+}
+
+// refit_starts_host to a.refit_starts: a pageable copy, not through upload(), which may page-lock the context's own vector
+int send_refit_starts(lrk_ctx *ctx) {
+    const auto &starts = ctx->refit_starts_host;
+    if (starts.empty()) return LRK_OK;
+    LRK_CUDA(ctx->arrays.refit_starts.reserve(starts.size() * sizeof(uint32_t)));
+    LRK_CUDA(cudaMemcpyAsync(ctx->arrays.refit_starts.get(), starts.data(), starts.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    return LRK_OK;
+}
+
+// The opening of every scene update `call`: a context with a scene, and no null array among those the call reads
+int open_scene_update(lrk_ctx *ctx, const char *call, bool null_array) {
+    if (!ctx) return LRK_ERR_INVALID_ARGUMENT;
+    if (!ctx->has_scene) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, std::string(call) + ": no scene");
+    if (null_array) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, std::string(call) + ": null array");
+    return LRK_OK;
+}
+
+// Id k of a scene update `call`: a `noun` (instance, mesh) below entry.size() and named once (entry[id] is ~0u until it is k)
+int claim_update_id(lrk_ctx *ctx, const char *call, const char *noun, uint32_t id, uint32_t k, std::vector<uint32_t> &entry) {
+    if (id >= entry.size() || entry[id] != ~0u)
+        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, std::string(call) + ": " + noun + " id " + std::to_string(id) + (id < entry.size() ? " repeated" : " out of range"));
+    entry[id] = k;
+    return LRK_OK;
+}
+
+// The n vertices a `call` gives mesh `id`, with finite positions
+int check_finite_positions(lrk_ctx *ctx, const char *call, uint32_t id, const lrk_vertex *v, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++)
+        for (int j = 0; j < 3; j++)
+            if (!std::isfinite(v[i].p[j])) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, std::string(call) + ": non-finite position in mesh " + std::to_string(id));
+    return LRK_OK;
+}
+
+// The light data of emissive mesh `id` from its new geometry (n triangles over vertices v): its area alias table, built on the host
+// as the flattening builds it into `table` / `pdf_table` (sent asynchronously: alive until finish_scene_update synchronises) and
+// sent to `alias` / `pdf`, and with the light tree its points in the tree's source, which sets lights_changed.
+int refresh_emissive_mesh(lrk_ctx *ctx, uint32_t id, const lrk_vertex *v, const lrk_triangle *tris, uint32_t n, lrk_alias_entry *alias, float *pdf,
+                          std::vector<lrk_alias_entry> &table, std::vector<float> &pdf_table, bool &lights_changed) {
+    mesh_area_alias_table(v, tris, n, table, pdf_table);
+    LRK_CUDA(cudaMemcpyAsync(alias, table.data(), table.size() * sizeof(lrk_alias_entry), cudaMemcpyHostToDevice, ctx->stream));
+    LRK_CUDA(cudaMemcpyAsync(pdf, pdf_table.data(), pdf_table.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    if (!ctx->light_active.tree) return LRK_OK;
+    const auto it = ctx->light_source.mesh_points.find(id);
+    if (it == ctx->light_source.mesh_points.end()) return LRK_OK;
+    auto &points = it->second;
+    points.clear();
+    for (uint32_t t = 0; t < n; t++)
+        for (uint32_t i : {tris[t].i0, tris[t].i1, tris[t].i2}) points.insert(points.end(), v[i].p, v[i].p + 3);
+    lights_changed = true;
+    return LRK_OK;
+}
+
+// The scene record's geometry: its pointers to the geometry arrays, which lrk_upload_scene fills and lrk_replace_meshes
+// reallocates, and the instance level's root
+void point_scene_at_geometry(lrk_ctx *ctx, uint32_t tlas_root) {
+    const auto &a = ctx->arrays;
+    auto &sc = ctx->scene;
+    sc.vertices = a.vertices.get<const lrk_vertex>();
+    sc.triangles = a.triangles.get<const lrk_triangle>();
+    sc.alias = a.alias.get<const lrk_alias_entry>();
+    sc.pdf = a.pdf.get<const float>();
+    sc.meshes = a.meshes.get<const lrk_mesh>();
+    sc.bvh_nodes = a.bvh_nodes.get<const float4>();
+    sc.tri_verts = a.tri_verts.get<const float4>();
+    sc.tlas_root = tlas_root;
 }
 
 }// namespace
@@ -1413,18 +1474,12 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
 
     auto &sc = ctx->scene;
-    sc.vertices = a.vertices.get<const lrk_vertex>();
-    sc.triangles = a.triangles.get<const lrk_triangle>();
-    sc.alias = a.alias.get<const lrk_alias_entry>();
-    sc.pdf = a.pdf.get<const float>();
-    sc.meshes = a.meshes.get<const lrk_mesh>();
+    point_scene_at_geometry(ctx, tlas_root);
     sc.inst_handles = a.inst_handles.get<const uint4>();
     sc.inst_kind = a.inst_kind.get<const uint32_t>();
     sc.inst_o2w = a.inst_o2w.get<const float4>();
     sc.inst_xform = a.inst_xform.get<const float4>();
-    sc.bvh_nodes = a.bvh_nodes.get<const float4>();
     sc.traversal_overflow = a.traversal_overflow.get<uint32_t>();
-    sc.tri_verts = a.tri_verts.get<const float4>();
     sc.surfaces = a.surfaces.get<const lrk_surface>();
     sc.textures = a.textures.get<const lrk_texture>();
     sc.env_alias = a.env_alias.get<const lrk_alias_entry>();
@@ -1441,7 +1496,6 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     sc.lights = a.lights.get<const lrk_light>();
     sc.light_handles = a.light_handles.get<const lrk_light_handle>();
     sc.camera = a.camera.get<const lrk_camera>();
-    sc.tlas_root = tlas_root;
     sc.light_count = s->light_count;
     sc.instance_count = s->instance_count;
     sc.surface_count = s->surface_count;
@@ -1509,18 +1563,13 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
 }
 
 int lrk_update_instances(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const float *object_to_world) {
-    if (!ctx) return LRK_ERR_INVALID_ARGUMENT;
-    if (!ctx->has_scene) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: no scene");
-    if (count != 0u && (!ids || !object_to_world)) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: null array");
+    if (const int rc = open_scene_update(ctx, "lrk_update_instances", count != 0u && (!ids || !object_to_world))) return rc;
     // everything is checked before anything changes
-    const uint32_t instances = ctx->scene.instance_count;
     std::vector<InstanceUpdate> updates(count);
-    std::vector<uint8_t> seen(instances, 0u);
+    std::vector<uint32_t> entry(ctx->scene.instance_count, ~0u);
     for (uint32_t k = 0; k < count; k++) {
         const uint32_t id = ids[k];
-        if (id >= instances) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: instance id " + std::to_string(id) + " out of range");
-        if (seen[id]) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: instance id " + std::to_string(id) + " repeated");
-        seen[id] = 1u;
+        if (const int rc = claim_update_id(ctx, "lrk_update_instances", "instance", id, k, entry)) return rc;
         const float *m = object_to_world + 12u * static_cast<size_t>(k);
         for (int j = 0; j < 12; j++)
             if (!std::isfinite(m[j])) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_instances: non-finite transform of instance " + std::to_string(id));
@@ -1554,18 +1603,14 @@ int lrk_update_instances(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, cons
 }
 
 int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const lrk_vertex *vertices, uint64_t vertex_count) {
-    if (!ctx) return LRK_ERR_INVALID_ARGUMENT;
-    if (!ctx->has_scene) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: no scene");
-    if (count != 0u && (!ids || !vertices)) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: null array");
+    if (const int rc = open_scene_update(ctx, "lrk_update_meshes", count != 0u && (!ids || !vertices))) return rc;
     // everything is checked before anything changes
     std::vector<MeshRefit> entries(count);
-    std::vector<uint8_t> seen(ctx->mesh_count, 0u);
+    std::vector<uint32_t> entry(ctx->mesh_count, ~0u);
     uint64_t total = 0u, slots = 0u;
     for (uint32_t k = 0; k < count; k++) {
         const uint32_t id = ids[k];
-        if (id >= ctx->mesh_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: mesh id " + std::to_string(id) + " out of range");
-        if (seen[id]) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: mesh id " + std::to_string(id) + " repeated");
-        seen[id] = 1u;
+        if (const int rc = claim_update_id(ctx, "lrk_update_meshes", "mesh", id, k, entry)) return rc;
         const lrk_mesh &m = ctx->meshes_host[id];
         entries[k] = MeshRefit{id, m.vertex_offset, m.triangle_offset, m.tri_slot_offset, static_cast<uint32_t>(total), static_cast<uint32_t>(slots), 0u, 0u};
         total += m.vertex_count;
@@ -1574,12 +1619,9 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
     if (vertex_count != total)
         return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: vertex_count is " + std::to_string(vertex_count) + ", the meshes have " +
                                                        std::to_string(total) + " vertices");
-    for (uint32_t k = 0; k < count; k++) {
-        const uint64_t end = k + 1u < count ? entries[k + 1u].vertex_begin : total;
-        for (uint64_t v = entries[k].vertex_begin; v < end; v++)
-            for (int j = 0; j < 3; j++)
-                if (!std::isfinite(vertices[v].p[j])) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: non-finite position in mesh " + std::to_string(ids[k]));
-    }
+    for (uint32_t k = 0; k < count; k++)
+        if (const int rc = check_finite_positions(ctx, "lrk_update_meshes", ids[k], vertices + entries[k].vertex_begin, ctx->meshes_host[ids[k]].vertex_count))
+            return rc;
     if (const int rc = check_instance_level(ctx, "lrk_update_meshes")) return rc;
     LRK_CUDA(cudaSetDevice(ctx->device));
     auto &a = ctx->arrays;
@@ -1601,10 +1643,7 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
             ctx->emissive_triangles.emplace(e.mesh, std::move(tris));
         }
     }
-    if (new_starts) {// a pageable copy (not through upload(), which may page-lock the context's own vector)
-        LRK_CUDA(a.refit_starts.reserve(ctx->refit_starts_host.size() * sizeof(uint32_t)));
-        LRK_CUDA(cudaMemcpyAsync(a.refit_starts.get(), ctx->refit_starts_host.data(), ctx->refit_starts_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-    }
+    if (new_starts && (rc = send_refit_starts(ctx))) return rc;
     bool lights_changed = false;
     std::vector<std::vector<lrk_alias_entry>> tables(count);// sent asynchronously: alive until finish_scene_update synchronises
     std::vector<std::vector<float>> pdfs(count);
@@ -1646,22 +1685,12 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
         LRK_CUDA(cudaGetLastError());
         // the emissive meshes' area alias tables, and their triangles in the light tree's source
         for (uint32_t k = 0; k < count; k++) {
-            const uint32_t id = entries[k].mesh;
-            if (!ctx->mesh_emissive[id]) continue;
-            const auto &tris = ctx->emissive_triangles.at(id);
-            const lrk_vertex *v = vertices + entries[k].vertex_begin;
-            mesh_area_alias_table(v, tris.data(), tris.size(), tables[k], pdfs[k]);
-            LRK_CUDA(cudaMemcpyAsync(a.alias.get<lrk_alias_entry>() + entries[k].triangle_offset, tables[k].data(), tables[k].size() * sizeof(lrk_alias_entry),
-                                     cudaMemcpyHostToDevice, stream));
-            LRK_CUDA(cudaMemcpyAsync(a.pdf.get<float>() + entries[k].triangle_offset, pdfs[k].data(), pdfs[k].size() * sizeof(float), cudaMemcpyHostToDevice, stream));
-            if (!ctx->light_active.tree) continue;
-            const auto it = ctx->light_source.mesh_points.find(id);
-            if (it == ctx->light_source.mesh_points.end()) continue;
-            auto &points = it->second;
-            points.clear();
-            for (const lrk_triangle &t : tris)
-                for (uint32_t i : {t.i0, t.i1, t.i2}) points.insert(points.end(), v[i].p, v[i].p + 3);
-            lights_changed = true;
+            const MeshRefit &e = entries[k];
+            if (!ctx->mesh_emissive[e.mesh]) continue;
+            const auto &tris = ctx->emissive_triangles.at(e.mesh);
+            if ((rc = refresh_emissive_mesh(ctx, e.mesh, vertices + e.vertex_begin, tris.data(), static_cast<uint32_t>(tris.size()),
+                                            a.alias.get<lrk_alias_entry>() + e.triangle_offset, a.pdf.get<float>() + e.triangle_offset, tables[k], pdfs[k], lights_changed)))
+                return rc;
         }
     }
     return finish_scene_update(ctx, lights_changed);
@@ -1669,28 +1698,22 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
 
 int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const uint32_t *vertex_counts, const lrk_vertex *vertices,
                        const uint32_t *triangle_counts, const lrk_triangle *triangles) {
-    if (!ctx) return LRK_ERR_INVALID_ARGUMENT;
-    if (!ctx->has_scene) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_replace_meshes: no scene");
-    if (count != 0u && (!ids || !vertex_counts || !vertices || !triangle_counts || !triangles))
-        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_replace_meshes: null array");
+    if (const int rc = open_scene_update(ctx, "lrk_replace_meshes", count != 0u && (!ids || !vertex_counts || !vertices || !triangle_counts || !triangles)))
+        return rc;
     // everything is checked before anything changes
     const uint32_t mesh_count = ctx->mesh_count;
     std::vector<uint32_t> entry(mesh_count, ~0u);// per mesh the index k of its id, ~0u for an unchanged mesh
     std::vector<uint64_t> vertex_begin(count + 1u, 0u), triangle_begin(count + 1u, 0u);// where id k's records start in the caller's arrays
     for (uint32_t k = 0; k < count; k++) {
         const uint32_t id = ids[k];
-        const std::string mesh = "lrk_replace_meshes: mesh id " + std::to_string(id);
-        if (id >= mesh_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, mesh + " out of range");
-        if (entry[id] != ~0u) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, mesh + " repeated");
-        if (vertex_counts[k] == 0u || triangle_counts[k] == 0u) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, mesh + " gets no vertices or no triangles");
-        entry[id] = k;
+        if (const int rc = claim_update_id(ctx, "lrk_replace_meshes", "mesh", id, k, entry)) return rc;
+        if (vertex_counts[k] == 0u || triangle_counts[k] == 0u)
+            return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_replace_meshes: mesh id " + std::to_string(id) + " gets no vertices or no triangles");
         vertex_begin[k + 1u] = vertex_begin[k] + vertex_counts[k];
         triangle_begin[k + 1u] = triangle_begin[k] + triangle_counts[k];
     }
     for (uint32_t k = 0; k < count; k++) {
-        for (uint64_t v = vertex_begin[k]; v < vertex_begin[k + 1u]; v++)
-            for (int j = 0; j < 3; j++)
-                if (!std::isfinite(vertices[v].p[j])) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_replace_meshes: non-finite position in mesh " + std::to_string(ids[k]));
+        if (const int rc = check_finite_positions(ctx, "lrk_replace_meshes", ids[k], vertices + vertex_begin[k], vertex_counts[k])) return rc;
         for (uint64_t t = triangle_begin[k]; t < triangle_begin[k + 1u]; t++)
             if (std::max({triangles[t].i0, triangles[t].i1, triangles[t].i2}) >= vertex_counts[k])
                 return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_replace_meshes: triangle index out of range in mesh " + std::to_string(ids[k]) + " (" +
@@ -1759,11 +1782,6 @@ int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const 
         node_runs.push_back(NodeRun{p.old_n, p.new_n, p.new_t - p.old_s, moved_nodes});
         moved_nodes += p.nodes;
     }
-    // the emissive replaced meshes' area alias tables, from the caller's arrays (the other replaced meshes' tables are never read)
-    std::vector<std::vector<lrk_alias_entry>> tables(count);
-    std::vector<std::vector<float>> pdfs(count);
-    for (uint32_t k = 0; k < count; k++)
-        if (ctx->mesh_emissive[ids[k]]) mesh_area_alias_table(vertices + vertex_begin[k], triangles + triangle_begin[k], triangle_counts[k], tables[k], pdfs[k]);
     // every allocation before anything changes: a refusal for memory leaves the scene as it was
     LRK_CUDA(cudaSetDevice(ctx->device));
     auto &a = ctx->arrays;
@@ -1807,15 +1825,22 @@ int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const 
                                                                              a.bvh_nodes.get<const float4>(), nnodes.get<float4>());
         LRK_CUDA(cudaGetLastError());
     }
-    // the replaced meshes' records, and the new mesh table
+    // the replaced meshes' records, the emissive ones' light data from the caller's arrays (the other replaced meshes' area tables
+    // are never read), and the new mesh table
+    bool lights_changed = false;
+    std::vector<std::vector<lrk_alias_entry>> tables(count);
+    std::vector<std::vector<float>> pdfs(count);
     for (uint32_t k = 0; k < count; k++) {
-        const lrk_mesh &r = layout[ids[k]];
+        const uint32_t id = ids[k];
+        const lrk_mesh &r = layout[id];
+        const lrk_triangle *tris = triangles + triangle_begin[k];
         LRK_CUDA(cudaMemcpyAsync(nv.get<lrk_vertex>() + r.vertex_offset, vertices + vertex_begin[k], uint64_t{r.vertex_count} * sizeof(lrk_vertex), cudaMemcpyHostToDevice, stream));
-        LRK_CUDA(cudaMemcpyAsync(nt.get<lrk_triangle>() + r.triangle_offset, triangles + triangle_begin[k], uint64_t{r.triangle_count} * sizeof(lrk_triangle),
-                                 cudaMemcpyHostToDevice, stream));
-        if (ctx->mesh_emissive[ids[k]]) {
-            LRK_CUDA(cudaMemcpyAsync(nalias.get<lrk_alias_entry>() + r.triangle_offset, tables[k].data(), tables[k].size() * sizeof(lrk_alias_entry), cudaMemcpyHostToDevice, stream));
-            LRK_CUDA(cudaMemcpyAsync(npdf.get<float>() + r.triangle_offset, pdfs[k].data(), pdfs[k].size() * sizeof(float), cudaMemcpyHostToDevice, stream));
+        LRK_CUDA(cudaMemcpyAsync(nt.get<lrk_triangle>() + r.triangle_offset, tris, uint64_t{r.triangle_count} * sizeof(lrk_triangle), cudaMemcpyHostToDevice, stream));
+        if (ctx->mesh_emissive[id]) {
+            if ((rc = refresh_emissive_mesh(ctx, id, vertices + vertex_begin[k], tris, r.triangle_count, nalias.get<lrk_alias_entry>() + r.triangle_offset,
+                                            npdf.get<float>() + r.triangle_offset, tables[k], pdfs[k], lights_changed)))
+                return rc;
+            ctx->emissive_triangles[id].assign(tris, tris + r.triangle_count);
         } else {
             LRK_CUDA(cudaMemsetAsync(nalias.get<lrk_alias_entry>() + r.triangle_offset, 0, uint64_t{r.triangle_count} * sizeof(lrk_alias_entry), stream));
             LRK_CUDA(cudaMemsetAsync(npdf.get<float>() + r.triangle_offset, 0, uint64_t{r.triangle_count} * sizeof(float), stream));
@@ -1852,38 +1877,12 @@ int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const 
         range.first = first;
     }
     ctx->refit_starts_host.swap(starts);
-    if (!ctx->refit_starts_host.empty())// a pageable copy, as lrk_update_meshes sends it; never larger than the buffer it had
-        LRK_CUDA(cudaMemcpyAsync(a.refit_starts.get(), ctx->refit_starts_host.data(), ctx->refit_starts_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+    if ((rc = send_refit_starts(ctx))) return rc;// never larger than the buffer it had
     ctx->meshes_host.swap(layout);
     ctx->bvh_node_count = node_total;
-    auto &sc = ctx->scene;
-    sc.vertices = a.vertices.get<const lrk_vertex>();
-    sc.triangles = a.triangles.get<const lrk_triangle>();
-    sc.alias = a.alias.get<const lrk_alias_entry>();
-    sc.pdf = a.pdf.get<const float>();
-    sc.meshes = a.meshes.get<const lrk_mesh>();
-    sc.bvh_nodes = a.bvh_nodes.get<const float4>();
-    sc.tri_verts = a.tri_verts.get<const float4>();
-    sc.tlas_root = tlas_root;
+    point_scene_at_geometry(ctx, tlas_root);
     // only the scene record: the light-tree record behind it (upload_light_sampling) stays
-    LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get(), &sc, sizeof(DeviceScene), cudaMemcpyHostToDevice, stream));
-    // the emissive replaced meshes' triangles, and their points in the light tree's source
-    bool lights_changed = false;
-    for (uint32_t k = 0; k < count; k++) {
-        const uint32_t id = ids[k];
-        if (!ctx->mesh_emissive[id]) continue;
-        const lrk_triangle *tris = triangles + triangle_begin[k];
-        ctx->emissive_triangles[id].assign(tris, tris + triangle_counts[k]);
-        if (!ctx->light_active.tree) continue;
-        const auto it = ctx->light_source.mesh_points.find(id);
-        if (it == ctx->light_source.mesh_points.end()) continue;
-        const lrk_vertex *v = vertices + vertex_begin[k];
-        auto &points = it->second;
-        points.clear();
-        for (uint32_t t = 0; t < triangle_counts[k]; t++)
-            for (uint32_t i : {tris[t].i0, tris[t].i1, tris[t].i2}) points.insert(points.end(), v[i].p, v[i].p + 3);
-        lights_changed = true;
-    }
+    LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get(), &ctx->scene, sizeof(DeviceScene), cudaMemcpyHostToDevice, stream));
     return finish_scene_update(ctx, lights_changed);
 }
 

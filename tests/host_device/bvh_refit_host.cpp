@@ -1,12 +1,15 @@
-// bvh_refit_host.cpp — the refit arithmetic of lrk_update_meshes (luisarender_b200/csrc/device/bvh_refit.h) and the shared area alias
-// tables (luisarender_b200/csrc/device/alias_table.h) compiled for the host, so that tests/test_mesh_update_cpu.py can refit
-// flattened hierarchies to deformed vertices and rebuild alias tables without a GPU.  The walk here is a recursive one over the
-// reachable nodes; the device kernel visits the same nodes bottom-up and computes every box with the same functions.
+// bvh_refit_host.cpp — the refit arithmetic of lrk_update_meshes and the node move of lrk_replace_meshes
+// (luisarender_b200/csrc/device/bvh_refit.h) and the shared area alias tables (luisarender_b200/csrc/device/alias_table.h) compiled
+// for the host, so that tests/test_mesh_update_cpu.py and tests/test_mesh_replace_cpu.py can refit flattened hierarchies to
+// deformed vertices, move them to a new layout and rebuild alias tables without a GPU.  The refit's walk here is a recursive one
+// over the reachable nodes; the device kernel visits the same nodes bottom-up and computes every box with the same functions.
+// The device's relayout_nodes_kernel moves every node of a run with the same function as relayout_nodes here.
 // TEST INFRASTRUCTURE: nothing here is part of the product.
 #include <cstdint>
 #include <cstring>
 #include <vector>
 
+#include "../../include/lrk.h"
 #include "../../luisarender_b200/csrc/device/alias_table.h"
 #include "../../luisarender_b200/csrc/device/bvh_refit.h"
 
@@ -69,4 +72,17 @@ extern "C" void mesh_alias_table(const lrk_vertex *vertices, const lrk_triangle 
     lrk::mesh_area_alias_table(vertices, triangles, triangle_count, table, pdf);
     std::memcpy(table_out, table.data(), table.size() * sizeof(lrk_alias_entry));
     std::memcpy(pdf_out, pdf.data(), pdf.size() * sizeof(float));
+}
+
+// dst[i] = src[i] moved by node_delta nodes and slot_delta triangle slots (both modulo 2^32), for i < count
+extern "C" void relayout_nodes(const lrk_bvh_node *src, lrk_bvh_node *dst, uint32_t count, uint32_t node_delta, uint32_t slot_delta) {
+    for (uint32_t i = 0; i < count; i++) {
+        lrk_bvh_node n = src[i];
+        uint32_t words[3] = {n.ref0, n.ref1, n.parent};
+        lrk::relayout_node_refs(words, node_delta, slot_delta);
+        n.ref0 = words[0];
+        n.ref1 = words[1];
+        n.parent = words[2];
+        dst[i] = n;
+    }
 }

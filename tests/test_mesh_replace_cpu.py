@@ -9,28 +9,26 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import mesh_replace_frames as R
-import mesh_update_frames as M
-from host_harness import DEVICE, REPO, load
+import scene_update_checks as U
+import scene_update_frames as S
 from luisarender_b200 import _ffi as F
-from luisarender_b200.api import Renderer
 from oracle import binding as O
-from test_scene_update import _random_rays
+from scene_update_checks import refit_host  # noqa: F401  (the host-compiled bvh_refit.h)
 
-ALL_FRAMES = {**R.FRAMES, **R.EMISSIVE_FRAMES}
+ALL_FRAMES = {**S.REPLACE_FRAMES, **S.REPLACE_EMISSIVE_FRAMES}
 
 
 def _pairs(name):
-    frames = [M.scene(t) for t in ALL_FRAMES[name]()]
+    frames = [S.scene(t) for t in ALL_FRAMES[name]()]
     return [(a, b) for a, b in zip(frames, frames[1:])]
 
 
 def _slices(d):
     """Per mesh its vertex, triangle, alias, pdf and tri_verts records as bytes."""
-    arrays = (M.vertices(d), R.triangles(d), M.array(d.alias, d.triangle_count, F.AliasEntry, np.uint32),
-              M.array(d.pdf, d.triangle_count, C.c_float, np.uint32, 1), M.array(d.tri_verts, d.tri_slot_count, C.c_float * 12, np.uint32))
+    arrays = (S.vertices(d), S.triangles(d), S.array(d.alias, d.triangle_count, F.AliasEntry, np.uint32),
+              S.array(d.pdf, d.triangle_count, C.c_float, np.uint32, 1), S.array(d.tri_verts, d.tri_slot_count, C.c_float * 12, np.uint32))
     out = []
-    for vo, vc, to, tc, _root, so, *_ in M.meshes(d):
+    for vo, vc, to, tc, _root, so, *_ in S.meshes(d):
         v, t, alias, pdf, tv = arrays
         out.append((v[vo:vo + vc].tobytes(), t[to:to + tc].tobytes(), alias[to:to + tc].tobytes(), pdf[to:to + tc].tobytes(), tv[so:so + tc].tobytes()))
     return out
@@ -40,13 +38,13 @@ def _slices(d):
 def test_frames_differ_only_in_the_replaced_meshes(name):
     for fa, fb in _pairs(name):
         a, b = fa.desc(), fb.desc()
-        ids, verts, tris = R.replaced_meshes(a, b)
+        ids, verts, tris = S.replaced_meshes(a, b)
         assert ids
         for ptr, count, cls in (("surfaces", "surface_count", F.Surface), ("lights", "light_count", F.Light), ("light_handles", "light_count", F.LightHandle)):
             assert getattr(b, count) == getattr(a, count)
-            assert M.array(getattr(b, ptr), getattr(b, count), cls, np.uint8).tobytes() == M.array(getattr(a, ptr), getattr(a, count), cls, np.uint8).tobytes()
+            assert S.array(getattr(b, ptr), getattr(b, count), cls, np.uint8).tobytes() == S.array(getattr(a, ptr), getattr(a, count), cls, np.uint8).tobytes()
         assert bytes(b.camera) == bytes(a.camera) and b.instance_count == a.instance_count and b.mesh_count == a.mesh_count
-        ma, mb = M.meshes(a), M.meshes(b)
+        ma, mb = S.meshes(a), S.meshes(b)
         # the layout: prefix sums over the new counts, in mesh order
         for col, count in ((0, 1), (2, 3), (5, 3)):
             assert np.array_equal(mb[:, col], np.concatenate([[0], np.cumsum(mb[:-1, count])]))
@@ -61,7 +59,7 @@ def test_frames_differ_only_in_the_replaced_meshes(name):
         for k in range(b.mesh_count):
             if k not in ids:
                 assert sb[k] == sa[k]  # an unchanged mesh's records move as they are
-        assert set(ids) & emissive or name not in R.EMISSIVE_FRAMES
+        assert set(ids) & emissive or name not in S.REPLACE_EMISSIVE_FRAMES
         # the instances: only handle[2] of the replaced meshes' instances, their new triangle count
         for i in range(b.instance_count):
             x, y = F.Instance.from_buffer_copy(bytes(a.instances[i])), b.instances[i]
@@ -71,35 +69,22 @@ def test_frames_differ_only_in_the_replaced_meshes(name):
             assert bytes(x) == bytes(y)
 
 
-@pytest.fixture(scope="module")
-def relayout():
-    lib = load("mesh_replace_host", [DEVICE / "bvh_refit.h", REPO / "include" / "lrk.h"], ["-O2", "-march=x86-64-v3", "-ffp-contract=off"])
-    lib.relayout_nodes.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]
-    return lib
-
-
-def _ranges(d):
-    """Per mesh its node range (first, end): from its root to the next mesh's root, or to the instance level."""
-    roots = M.meshes(d)[:, 4].astype(np.int64)
-    return [(int(r), int(roots[roots > r].min()) if (roots > r).any() else int(d.tlas_root)) for r in roots]
-
-
-def _move(relayout, nodes, node_delta, slot_delta):
+def _move(lib, nodes, node_delta, slot_delta):
     out = np.zeros_like(nodes)
-    relayout.relayout_nodes(nodes.ctypes.data, out.ctypes.data, len(nodes), node_delta % 2**32, slot_delta % 2**32)
+    lib.relayout_nodes(nodes.ctypes.data, out.ctypes.data, len(nodes), node_delta % 2**32, slot_delta % 2**32)
     return out
 
 
-def _relaid(a, b, relayout):
+def _relaid(a, b, lib):
     """The hierarchy lrk_replace_meshes leaves for frame a replaced by frame b's meshes, built on the host: in mesh order, every
     unchanged mesh's node range of a moved to its new place, every replaced mesh's range of max(n - 1, 1) nodes starting with b's
     own hierarchy of it (moved), and b's instance level behind them.  Returns the description (b's with these nodes and roots),
     the arrays it points into, and the new ranges."""
-    ids, _, _ = R.replaced_meshes(a, b)
-    nodes_a = M.array(a.bvh_nodes, a.bvh_node_count, F.BvhNode, np.uint32, 16)
-    nodes_b = M.array(b.bvh_nodes, b.bvh_node_count, F.BvhNode, np.uint32, 16)
-    ma, mb = M.meshes(a), M.meshes(b).copy()
-    ra, rb = _ranges(a), _ranges(b)
+    ids, _, _ = S.replaced_meshes(a, b)
+    nodes_a = S.array(a.bvh_nodes, a.bvh_node_count, F.BvhNode, np.uint32, 16)
+    nodes_b = S.array(b.bvh_nodes, b.bvh_node_count, F.BvhNode, np.uint32, 16)
+    ma, mb = S.meshes(a), S.meshes(b).copy()
+    ra, rb = U.node_ranges(a), U.node_ranges(b)
     parts, ranges, base = [], [], 0
     for k in range(b.mesh_count):
         if k in ids:
@@ -107,39 +92,28 @@ def _relaid(a, b, relayout):
             size = max(int(mb[k, 3]) - 1, 1)
             assert end - first <= size  # the host's hierarchy never has more nodes than the device builder's
             part = np.zeros((size, 16), np.uint32)
-            part[:end - first] = _move(relayout, nodes_b[first:end], base - first, 0)
+            part[:end - first] = _move(lib, nodes_b[first:end], base - first, 0)
         else:
             first, end = ra[k]
-            part = _move(relayout, nodes_a[first:end], base - first, int(mb[k, 5]) - int(ma[k, 5]))
+            part = _move(lib, nodes_a[first:end], base - first, int(mb[k, 5]) - int(ma[k, 5]))
             # the same mesh's hierarchy in b (the host build is deterministic), moved from b's place to the new one
-            assert np.array_equal(part, _move(relayout, nodes_b[rb[k][0]:rb[k][1]], base - rb[k][0], 0))
+            assert np.array_equal(part, _move(lib, nodes_b[rb[k][0]:rb[k][1]], base - rb[k][0], 0))
         mb[k, 4] = base
         ranges.append((base, base + len(part)))
         parts.append(part)
         base += len(part)
-    tlas = nodes_b[b.tlas_root:].copy()
-    for col in (12, 13, 14):  # inner references and parents move with the level
-        inner = (tlas[:, col] & np.uint32(0x80000000)) == 0
-        tlas[inner, col] = (tlas[inner, col].astype(np.int64) + (base - int(b.tlas_root))).astype(np.uint32)
-    nodes = np.ascontiguousarray(np.concatenate(parts + [tlas]))
-    h = F.SceneDesc()
-    C.memmove(C.byref(h), C.byref(b), C.sizeof(F.SceneDesc))
-    keep = [nodes, np.ascontiguousarray(mb)]
-    h.bvh_nodes = nodes.ctypes.data_as(C.POINTER(F.BvhNode))
-    h.bvh_node_count = len(nodes)
-    h.tlas_root = base
-    h.meshes = keep[1].ctypes.data_as(C.POINTER(F.Mesh))
+    h, keep = U.with_hierarchies(b, np.concatenate(parts), mb)
     return h, keep, ranges, ids
 
 
-def test_relayout_rules(relayout):
+def test_relayout_rules(refit_host):
     leaf = lambda count, slot: 0x80000000 | ((count - 1) << 28) | slot
     node = np.zeros((3, 16), np.uint32)
     node[:, :12] = np.arange(36).reshape(3, 12)
     node[:, 12:15] = [[5, leaf(3, 40), 0xFFFFFFFF], [0xFFFFFFFF, leaf(4, 0x0FFFFFF0), 9], [leaf(1, 7), 12, 2]]
     node[:, 15] = 77
     for nd, sd in ((7, 3), (-4, -7), (0, 0x10)):
-        out = _move(relayout, node, nd, sd)
+        out = _move(refit_host, node, nd, sd)
         assert np.array_equal(out[:, :12], node[:, :12]) and np.array_equal(out[:, 15], node[:, 15])  # boxes stay
         for got, ref in zip(out[:, 12:14].reshape(-1), node[:, 12:14].reshape(-1)):
             if ref == 0xFFFFFFFF:
@@ -153,11 +127,11 @@ def test_relayout_rules(relayout):
 
 
 @pytest.mark.parametrize("name", list(ALL_FRAMES))
-def test_relaid_hierarchies_trace_like_the_replaced_frame(name, relayout):
+def test_relaid_hierarchies_trace_like_the_replaced_frame(name, refit_host):
     for fa, fb in _pairs(name):
         a, b = fa.desc(), fb.desc()
-        h, keep, ranges, ids = _relaid(a, b, relayout)
-        rays = _random_rays(fb, 100_000, seed=5)
+        h, keep, ranges, ids = _relaid(a, b, refit_host)
+        rays = U.random_rays(fb, 100_000, seed=5)
         for any_hit in (False, True):
             want, _ = O.trace(b, rays, any_hit=any_hit)
             got, _ = O.trace(h, rays, any_hit=any_hit)
@@ -168,27 +142,15 @@ def test_relaid_hierarchies_trace_like_the_replaced_frame(name, relayout):
         del keep
 
 
-class _Lib:
-    """A stand-in for the device library that records what reached lrk_replace_meshes, read while the call's arrays are alive."""
-    def __init__(self):
-        self.calls = []
-
-    def lrk_replace_meshes(self, ctx, ids, count, vertex_counts, vertices, triangle_counts, triangles):
-        u32 = lambda ptr, n: list((C.c_uint32 * n).from_address(ptr))
-        vc, tc = u32(vertex_counts, count), u32(triangle_counts, count)
-        self.calls.append((u32(ids, count), vc, tc, list((C.c_float * (8 * sum(vc))).from_address(vertices)), u32(triangles, 3 * sum(tc))))
-        return 0
-
-
-def _renderer():
-    r = Renderer.__new__(Renderer)
-    r._lib, r._ctx = _Lib(), None
-    r._check = lambda rc, what: None
-    return r
+def _read_call(ctx, ids, count, vertex_counts, vertices, triangle_counts, triangles):
+    """What reached lrk_replace_meshes, read while the call's arrays are alive."""
+    u32 = lambda ptr, n: list((C.c_uint32 * n).from_address(ptr))
+    vc, tc = u32(vertex_counts, count), u32(triangle_counts, count)
+    return u32(ids, count), vc, tc, list((C.c_float * (8 * sum(vc))).from_address(vertices)), u32(triangles, 3 * sum(tc))
 
 
 def test_replace_meshes_argument_shapes():
-    r = _renderer()
+    r, calls = U.recording_renderer("lrk_replace_meshes", _read_call)
     v, t = np.zeros((4, 8), np.float32), np.array([[0, 1, 2], [0, 2, 3]])
     refusals = [(lambda: r.replace_meshes([0, 1], [v], [t]), "vertices must have one array per id"),
                 (lambda: r.replace_meshes([0], [v], [t, t]), "triangles must have one array per id"),
@@ -201,11 +163,11 @@ def test_replace_meshes_argument_shapes():
     for call, what in refusals:
         with pytest.raises(ValueError, match=what):
             call()
-    assert r._lib.calls == []  # refused before the library is reached
+    assert calls == []  # refused before the library is reached
     records = (F.Vertex * 3)()
     records[1].p[0] = 2.5
     r.replace_meshes(np.array([3, 1]), [v, np.ctypeslib.as_array(records)], [t.astype(np.int64), np.array([[0, 1, 2]], np.uint16)])
-    (ids, vc, tc, verts, tris), = r._lib.calls
+    (ids, vc, tc, verts, tris), = calls
     assert ids == [3, 1] and vc == [4, 3] and tc == [2, 1]
     assert tris == [0, 1, 2, 0, 2, 3, 0, 1, 2]
     assert verts[8 * 5] == 2.5 and sum(verts) == 2.5

@@ -10,14 +10,14 @@ import hashlib
 import numpy as np
 import pytest
 
-import mesh_update_frames as M
-from host_harness import DEVICE, load
+import scene_update_checks as U
+import scene_update_frames as S
 from luisarender_b200 import _ffi as F
 from luisarender_b200 import scenes
-from luisarender_b200.api import Renderer
 from oracle import binding as O
+from scene_update_checks import refit_host  # noqa: F401  (the host-compiled bvh_refit.h)
 
-ALL_FRAMES = {**M.FRAMES, **M.EMISSIVE_FRAMES}
+ALL_FRAMES = {**S.DEFORM_FRAMES, **S.DEFORM_EMISSIVE_FRAMES}
 
 
 def test_default_globe_text_is_unchanged():
@@ -34,28 +34,28 @@ def _emissive_meshes(d):
 
 @pytest.mark.parametrize("name", list(ALL_FRAMES))
 def test_frames_differ_only_in_the_deformed_vertices(name):
-    frames = [M.scene(t) for t in ALL_FRAMES[name]()]
+    frames = [S.scene(t) for t in ALL_FRAMES[name]()]
     d0 = frames[0].desc()
-    m0 = M.meshes(d0)
+    m0 = S.meshes(d0)
     for f in frames[1:]:
         d = f.desc()
         for ptr, count, cls in (("triangles", "triangle_count", F.Triangle), ("surfaces", "surface_count", F.Surface),
                                 ("lights", "light_count", F.Light), ("light_handles", "light_count", F.LightHandle)):
             assert getattr(d, count) == getattr(d0, count)
-            assert M.array(getattr(d, ptr), getattr(d, count), cls, np.uint8).tobytes() == \
-                M.array(getattr(d0, ptr), getattr(d0, count), cls, np.uint8).tobytes(), ptr
+            assert S.array(getattr(d, ptr), getattr(d, count), cls, np.uint8).tobytes() == \
+                S.array(getattr(d0, ptr), getattr(d0, count), cls, np.uint8).tobytes(), ptr
         assert d.vertex_count == d0.vertex_count and d.tri_slot_count == d0.tri_slot_count
-        m = M.meshes(d)
+        m = S.meshes(d)
         assert np.array_equal(np.delete(m, 4, axis=1), np.delete(m0, 4, axis=1))  # the layout; the hierarchy's roots may move
         assert bytes(d.camera) == bytes(d0.camera)
         for i in range(d.instance_count):
             a, b = d0.instances[i], d.instances[i]
             assert bytes(a) == bytes(b)
-        ids, _ = M.deformed_meshes(d0, d)
+        ids, _ = S.deformed_meshes(d0, d)
         assert ids
-        alias0, alias = M.array(d0.alias, d0.triangle_count, F.AliasEntry, np.uint32), M.array(d.alias, d.triangle_count, F.AliasEntry, np.uint32)
-        pdf0, pdf = M.array(d0.pdf, d0.triangle_count, C.c_float, np.uint32, 1), M.array(d.pdf, d.triangle_count, C.c_float, np.uint32, 1)
-        tv0, tv = M.array(d0.tri_verts, d0.tri_slot_count, C.c_float * 12), M.array(d.tri_verts, d.tri_slot_count, C.c_float * 12)
+        alias0, alias = S.array(d0.alias, d0.triangle_count, F.AliasEntry, np.uint32), S.array(d.alias, d.triangle_count, F.AliasEntry, np.uint32)
+        pdf0, pdf = S.array(d0.pdf, d0.triangle_count, C.c_float, np.uint32, 1), S.array(d.pdf, d.triangle_count, C.c_float, np.uint32, 1)
+        tv0, tv = S.array(d0.tri_verts, d0.tri_slot_count, C.c_float * 12), S.array(d.tri_verts, d.tri_slot_count, C.c_float * 12)
         for k, row in enumerate(m):
             t0, tn, s0 = row[2], row[3], row[5]
             same_tris = slice(t0, t0 + tn)
@@ -66,85 +66,55 @@ def test_frames_differ_only_in_the_deformed_vertices(name):
                 pos = np.delete(tv[s0:s0 + tn], [3, 7, 11], axis=1)
                 pos0 = np.delete(tv0[s0:s0 + tn], [3, 7, 11], axis=1)
                 assert not np.array_equal(np.sort(pos, axis=0), np.sort(pos0, axis=0))
-        if name in M.EMISSIVE_FRAMES:
+        if name in S.DEFORM_EMISSIVE_FRAMES:
             assert set(ids) <= _emissive_meshes(d)
 
 
-@pytest.fixture(scope="module")
-def refit():
-    lib = load("bvh_refit_host", [DEVICE / "bvh_refit.h", DEVICE / "alias_table.h"], ["-O2", "-march=x86-64-v3", "-ffp-contract=off"])
-    lib.refit_mesh.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_float)]
-    lib.mesh_alias_table.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
-    return lib
-
-
-@pytest.mark.parametrize("name", list(M.EMISSIVE_FRAMES))
-def test_shared_alias_tables_reproduce_the_flattened_ones(name, refit):
-    for f in [M.scene(t) for t in M.EMISSIVE_FRAMES[name]()]:
+@pytest.mark.parametrize("name", list(S.DEFORM_EMISSIVE_FRAMES))
+def test_shared_alias_tables_reproduce_the_flattened_ones(name, refit_host):
+    for f in [S.scene(t) for t in S.DEFORM_EMISSIVE_FRAMES[name]()]:
         d = f.desc()
-        v, tris = M.vertices(d), M.array(d.triangles, d.triangle_count, F.Triangle, np.uint32, 3)
-        alias = M.array(d.alias, d.triangle_count, F.AliasEntry, np.uint32)
-        pdf = M.array(d.pdf, d.triangle_count, C.c_float, np.uint32, 1)
+        v, tris = S.vertices(d), S.triangles(d)
+        alias = S.array(d.alias, d.triangle_count, F.AliasEntry, np.uint32)
+        pdf = S.array(d.pdf, d.triangle_count, C.c_float, np.uint32, 1)
         for k in _emissive_meshes(d):
-            vo, vc, to, tc = M.meshes(d)[k][:4]
+            vo, vc, to, tc = S.meshes(d)[k][:4]
             v_k, t_k = np.ascontiguousarray(v[vo:vo + vc]), np.ascontiguousarray(tris[to:to + tc])
             table, p = np.zeros((tc, 2), np.uint32), np.zeros(tc, np.uint32)
-            refit.mesh_alias_table(v_k.ctypes.data, t_k.ctypes.data, int(tc), table.ctypes.data, p.ctypes.data)
+            refit_host.mesh_alias_table(v_k.ctypes.data, t_k.ctypes.data, int(tc), table.ctypes.data, p.ctypes.data)
             assert np.array_equal(table, alias[to:to + tc]) and np.array_equal(p, pdf[to:to + tc, 0])
 
 
-def _node_ranges(d):
-    """Per mesh its hierarchy's node range: from its root to the next mesh's root or the instance level."""
-    roots = M.meshes(d)[:, 4]
-    ends = []
-    for r in roots:
-        later = roots[roots > r]
-        ends.append(int(later.min()) if len(later) else int(d.tlas_root))
-    return [(int(r), e) for r, e in zip(roots, ends)]
-
-
-def _hybrid(a, b, refit):
+def _hybrid(a, b, lib):
     """A description that renders frame b with frame a's mesh hierarchies refit to b's vertices (what lrk_update_meshes leaves on
     the device): a's refit BLAS nodes and mesh table, a's slot order with b's positions, b's vertices and instances, and b's
     instance level appended behind a's meshes.  Returns the description, the arrays it points into and the refit meshes' pads."""
-    nodes_a = M.array(a.bvh_nodes, a.bvh_node_count, F.BvhNode, np.uint32, 16)
-    nodes_b = M.array(b.bvh_nodes, b.bvh_node_count, F.BvhNode, np.uint32, 16)
+    nodes_a = S.array(a.bvh_nodes, a.bvh_node_count, F.BvhNode, np.uint32, 16)
     blas = np.ascontiguousarray(nodes_a[:a.tlas_root])
     # a's slot order, b's positions: every slot's primitive re-read through b's triangles and vertices
-    tv = M.array(a.tri_verts, a.tri_slot_count, C.c_float * 12).copy()
-    vb, tris = M.vertices(b), M.array(b.triangles, b.triangle_count, F.Triangle, np.uint32, 3)
-    m = M.meshes(a)
+    tv = S.array(a.tri_verts, a.tri_slot_count, C.c_float * 12).copy()
+    vb, tris = S.vertices(b), S.triangles(b)
+    m = S.meshes(a)
     for vo, vc, to, tc, _root, so, *_ in m:
         prim = tv[so:so + tc, 3].view(np.uint32)
         t = tris[to + prim]
         for c in range(3):
             tv[so:so + tc, 4 * c:4 * c + 3] = vb[vo + t[:, c], :3]
-    ids, _ = M.deformed_meshes(a, b)
+    ids, _ = S.deformed_meshes(a, b)
     pads = {}
     for k in ids:
-        root, end = _node_ranges(a)[k]
+        root, end = U.node_ranges(a)[k]
         pad = C.c_float()
-        assert refit.refit_mesh(blas.ctypes.data, root, end, tv.ctypes.data, int(m[k][5]), int(m[k][3]), C.byref(pad)) == 0
+        assert lib.refit_mesh(blas.ctypes.data, root, end, tv.ctypes.data, int(m[k][5]), int(m[k][3]), C.byref(pad)) == 0
         pads[k] = pad.value
-    tlas = nodes_b[b.tlas_root:].copy()
-    for col in (12, 13, 14):  # inner references and parents move with the level
-        inner = (tlas[:, col] & np.uint32(0x80000000)) == 0
-        tlas[inner, col] = (tlas[inner, col].astype(np.int64) + (int(a.tlas_root) - int(b.tlas_root))).astype(np.uint32)
-    nodes = np.ascontiguousarray(np.concatenate([blas, tlas]))
-    h = F.SceneDesc()
-    C.memmove(C.byref(h), C.byref(b), C.sizeof(F.SceneDesc))
-    keep = [nodes, tv, np.ascontiguousarray(m)]
-    h.bvh_nodes = nodes.ctypes.data_as(C.POINTER(F.BvhNode))
-    h.bvh_node_count = len(nodes)
-    h.tlas_root = a.tlas_root
+    h, keep = U.with_hierarchies(b, blas, m)
     h.tri_verts = tv.ctypes.data_as(C.POINTER(C.c_float))
-    h.meshes = keep[2].ctypes.data_as(C.POINTER(F.Mesh))
-    return h, keep, pads, blas, tv, ids
+    return h, keep + [tv], pads, blas, tv, ids
 
 
 def _check_refit_boxes(a, blas, tv, ids, pads):
     """Every reachable leaf child's stored box is its slots' triangle box padded by exactly 5e-7 x the deformed mesh's extent."""
-    m = M.meshes(a)
+    m = S.meshes(a)
     for k in ids:
         so, tc = int(m[k][5]), int(m[k][3])
         pos = tv[so:so + tc].reshape(-1, 3, 4)[:, :, :3]
@@ -171,14 +141,14 @@ def _check_refit_boxes(a, blas, tv, ids, pads):
 
 
 @pytest.mark.parametrize("name", list(ALL_FRAMES))
-def test_refit_hierarchies_trace_like_the_deformed_frame(name, refit):
-    frames = [M.scene(t) for t in ALL_FRAMES[name]()]
+def test_refit_hierarchies_trace_like_the_deformed_frame(name, refit_host):
+    frames = [S.scene(t) for t in ALL_FRAMES[name]()]
     a = frames[0].desc()
     for f in frames[1:]:
         b = f.desc()
-        h, keep, pads, blas, tv, ids = _hybrid(a, b, refit)
+        h, keep, pads, blas, tv, ids = _hybrid(a, b, refit_host)
         _check_refit_boxes(a, blas, tv, ids, pads)
-        rays = _random_rays(f, 100_000, seed=5)
+        rays = U.random_rays(f, 100_000, seed=5)
         for any_hit in (False, True):
             want, _ = O.trace(b, rays, any_hit=any_hit)
             got, _ = O.trace(h, rays, any_hit=any_hit)
@@ -189,38 +159,8 @@ def test_refit_hierarchies_trace_like_the_deformed_frame(name, refit):
         del keep
 
 
-def _random_rays(scene, n, seed):
-    rng = np.random.default_rng(seed)
-    info = scene.info()
-    lo, hi = np.array(info["world_min"]), np.array(info["world_max"])
-    o = rng.uniform(lo - 0.5, hi + 0.5, size=(n, 3))
-    d = rng.uniform(lo, hi, size=(n, 3)) - o
-    d /= np.linalg.norm(d, axis=1, keepdims=True)
-    rays = np.zeros((n, 8), np.float32)
-    rays[:, :3], rays[:, 4:7], rays[:, 7] = o, d, np.finfo(np.float32).max
-    rays[::3, 7] = rng.uniform(0.5, 6.0, size=len(rays[::3]))
-    return rays
-
-
-class _Lib:
-    """A stand-in for the device library that records whether lrk_update_meshes was reached."""
-    def __init__(self):
-        self.calls = []
-
-    def lrk_update_meshes(self, *args):
-        self.calls.append(args)
-        return 0
-
-
-def _renderer():
-    r = Renderer.__new__(Renderer)
-    r._lib, r._ctx = _Lib(), None
-    r._check = lambda rc, what: None
-    return r
-
-
 def test_update_meshes_argument_shapes():
-    r = _renderer()
+    r, calls = U.recording_renderer("lrk_update_meshes")
     v = np.zeros((4, 8), np.float32)
     with pytest.raises(ValueError, match="one array per id"):
         r.update_meshes([0, 1], [v])
@@ -228,9 +168,9 @@ def test_update_meshes_argument_shapes():
         r.update_meshes([0], [np.zeros((4, 7), np.float32)])
     with pytest.raises(ValueError, match=r"\[vertex_count, 8\] float32"):
         r.update_meshes([0], [np.zeros((4, 8), np.float64)])
-    assert r._lib.calls == []  # refused before the library is reached
+    assert calls == []  # refused before the library is reached
     records = (F.Vertex * 3)()
     records[1].p[0] = 2.5
     r.update_meshes(np.array([3, 1]), [v, np.ctypeslib.as_array(records)])
-    (ctx, ids_ptr, count, verts_ptr, total), = r._lib.calls
+    (ctx, ids_ptr, count, verts_ptr, total), = calls
     assert count == 2 and total == 7
