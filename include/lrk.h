@@ -500,6 +500,10 @@ int lrk_create(const lrk_device_cfg *cfg, lrk_ctx **out);
 void lrk_destroy(lrk_ctx *ctx);
 const char *lrk_last_error(const lrk_ctx *ctx);
 
+/* Copies the scene description to the device; the film is cleared.  The whole description and the options it reads are checked
+ * before anything changes: a refusal for either (LRK_ERR_INVALID_ARGUMENT, LRK_ERR_UNSUPPORTED) leaves the context, its scene and
+ * its film as they were.  A CUDA failure during the upload leaves the context without a scene (LRK_ERR_NO_SCENE from the calls that
+ * need one) until the next upload. */
 int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *scene);
 
 /* Scene updates (an extension: change an uploaded scene between renders without lrk_upload_scene; DESIGN.md §4 (Scene updates)).

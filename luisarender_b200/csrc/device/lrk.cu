@@ -24,9 +24,12 @@
 #include "denoise.cuh"
 #include "affine_inverse.h"
 #include "alias_table.h"
+#include "scene_check.h"
 #include <cub/device/device_scan.cuh>
 
 using namespace lrk;
+
+static_assert(kMaxDepth + 1u == kMaxDepthSlots, "check_scene_desc refuses the depths that have no counter slot");
 
 namespace {
 
@@ -80,17 +83,22 @@ struct TimedLaunch {
     cudaEvent_t start, stop;
 };
 
-// What the light tree of the option "light_tree" and its bottom trees are built from, copied from the scene description by
-// lrk_upload_scene so that every scene update rebuilds them with the same code: per instance that carries a light (in instance
-// order) its mesh, object-to-world rows, power (luminance of the emission x the light's scale) and sidedness, and per such mesh
-// the object-space positions of its triangles' vertices (9 floats per triangle).
-struct LightTreeSource {
-    uint32_t instance_count{0};
-    std::vector<uint32_t> inst, mesh;
-    std::vector<float> o2w;
-    std::vector<double> power;
-    std::vector<uint8_t> two_sided;
-    std::map<uint32_t, std::vector<float>> mesh_points;
+// The host state of the uploaded scene that the scene updates (lrk_update_*, lrk_replace_meshes) read and keep, set whole by
+// lrk_upload_scene.  Every update rebuilds the instance level of the hierarchy on the device from the per-instance meshes and the
+// visible instances.  Mesh updates and replacements keep the current mesh table and, per mesh, whether an instance with a light
+// uses it; derived on a mesh's first update and kept until the next upload or replacement: its refit's start nodes (the reachable
+// inner nodes of its hierarchy without inner children) at refit_start[m] in a.refit_starts, and an emissive mesh's triangles.
+struct SceneUpdateState {
+    std::vector<uint32_t> inst_mesh_host, visible_host;// per instance its mesh; the visible instances in order
+    uint32_t mesh_count{0};
+    uint64_t bvh_node_count{0};// of the current hierarchy, whose last max(visible, 2) - 1 nodes are the instance level
+    bool tlas_inputs{false};// a.inst_mesh, a.visible_ids and a.mesh_bounds hold the scene's (device_bvh, or since the first update)
+    std::vector<lrk_mesh> meshes_host;
+    std::vector<uint8_t> mesh_emissive;
+    std::vector<uint32_t> refit_starts_host;
+    std::vector<std::pair<uint32_t, uint32_t>> refit_start;// (first, count); count 0: not derived yet
+    std::map<uint32_t, std::vector<lrk_triangle>> emissive_triangles;
+    LightTreeSource light_source;// while light_active.tree
 };
 
 }// namespace
@@ -168,20 +176,7 @@ struct lrk_ctx {
     // instantiations (upload_light_sampling)
     LightSampling light_requested, light_active;
     uint32_t *receiver_words{nullptr};// in path_allocs while light_active.receiver (alloc_paths)
-    LightTreeSource light_source;// while light_active.tree
-    // every scene update (lrk_update_*, lrk_replace_meshes): the instance level of the hierarchy is rebuilt on the device from these
-    std::vector<uint32_t> inst_mesh_host, visible_host;// per instance its mesh; the visible instances in order
-    uint32_t mesh_count{0};
-    uint64_t bvh_node_count{0};// of the current hierarchy, whose last max(visible, 2) - 1 nodes are the instance level
-    bool tlas_inputs{false};// a.inst_mesh, a.visible_ids and a.mesh_bounds hold the scene's (device_bvh, or since the first update)
-    // mesh updates and replacements: the current mesh table and, per mesh, whether an instance with a light uses it; derived on a
-    // mesh's first update and kept until the next upload or replacement: its refit's start nodes (the reachable inner nodes of its
-    // hierarchy without inner children) at refit_start[m] in a.refit_starts, and an emissive mesh's triangles
-    std::vector<lrk_mesh> meshes_host;
-    std::vector<uint8_t> mesh_emissive;
-    std::vector<uint32_t> refit_starts_host;
-    std::vector<std::pair<uint32_t, uint32_t>> refit_start;// (first, count); count 0: not derived yet
-    std::map<uint32_t, std::vector<lrk_triangle>> emissive_triangles;
+    SceneUpdateState update;
 
     ~lrk_ctx();
 };
@@ -645,42 +640,29 @@ int build_mesh_hierarchy(lrk_ctx *ctx, const BuildScratch &b, uint32_t m, const 
     return LRK_OK;
 }
 
-// Hierarchy build on the device (bvh_build.cuh): fills a.bvh_nodes / a.tri_verts from the uploaded geometry, returns the root of
-// every mesh's BLAS and of the TLAS.  One round of kernels per unique mesh, one for the instances.
-int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, std::vector<uint32_t> &mesh_root, uint32_t &tlas_root) {
+// Hierarchy build on the device (bvh_build.cuh): fills a.bvh_nodes / a.tri_verts from the uploaded geometry in the node layout
+// that check_scene_desc derived (per mesh max(n - 1, 1) nodes from its root, then the TLAS).  One round of kernels per unique mesh,
+// one for the instances.
+int build_bvh_on_device(lrk_ctx *ctx, const lrk_scene_desc *s, const SceneCheck &layout) {
     auto &a = ctx->arrays;
-    const std::vector<uint32_t> &visible = ctx->visible_host, &inst_mesh = ctx->inst_mesh_host;
-    // node layout: per mesh max(n - 1, 1) nodes, then the TLAS
-    mesh_root.resize(s->mesh_count);
-    uint64_t nodes = 0u, max_n = std::max<uint64_t>(visible.size(), 2u);
-    for (uint32_t m = 0; m < s->mesh_count; m++) {
-        mesh_root[m] = static_cast<uint32_t>(nodes);
-        const uint64_t n = s->meshes[m].triangle_count;
-        if (n == 0u) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: mesh without triangles");
-        nodes += std::max<uint64_t>(n - 1u, 1u);
-        max_n = std::max(max_n, n);
-    }
-    tlas_root = static_cast<uint32_t>(nodes);
-    nodes += std::max<uint64_t>(visible.size(), 2u) - 1u;
-    if (nodes >= 0x7fffffffull || s->triangle_count >= (1ull << 28)) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: scene too large for the BVH encoding");
-    ctx->bvh_node_count = nodes;
+    const std::vector<uint32_t> &visible = ctx->update.visible_host, &inst_mesh = ctx->update.inst_mesh_host;
     int rc;
-    LRK_CUDA(a.bvh_nodes.reserve(nodes * 64u));
+    LRK_CUDA(a.bvh_nodes.reserve(layout.node_count * 64u));
     LRK_CUDA(a.tri_verts.reserve(std::max<uint64_t>(s->triangle_count, 1u) * 48u));
     LRK_CUDA(a.mesh_bounds.reserve(std::max<uint64_t>(s->mesh_count, 1u) * sizeof(BuildBox)));
     if ((rc = upload(ctx, a.inst_mesh, inst_mesh.data(), inst_mesh.size()))) return rc;
     if ((rc = upload(ctx, a.visible_ids, visible.data(), visible.size()))) return rc;
     BuildScratch b;
-    if ((rc = reserve_build_scratch(ctx, max_n, b))) return rc;
+    if ((rc = reserve_build_scratch(ctx, std::max<uint64_t>({visible.size(), 2u, layout.largest_mesh}), b))) return rc;
     uint32_t slot_base = 0u;
     for (uint32_t m = 0; m < s->mesh_count; m++) {
-        if ((rc = build_mesh_hierarchy(ctx, b, m, s->meshes[m], mesh_root[m], slot_base))) return rc;
+        if ((rc = build_mesh_hierarchy(ctx, b, m, s->meshes[m], layout.mesh_root[m], slot_base))) return rc;
         slot_base += s->meshes[m].triangle_count;
     }
-    if ((rc = build_instance_level(ctx, b, static_cast<uint32_t>(visible.size()), tlas_root))) return rc;
+    if ((rc = build_instance_level(ctx, b, static_cast<uint32_t>(visible.size()), layout.tlas_root))) return rc;
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));// the static init block is done with
     LRK_CUDA(cudaGetLastError());
-    ctx->tlas_inputs = true;
+    ctx->update.tlas_inputs = true;
     return LRK_OK;
 }
 
@@ -881,44 +863,6 @@ void gather_triangles(const std::vector<float> &points, const float *m, std::vec
     }
 }
 
-// The light tree's input from the scene's own arrays: every instance that carries a light - not only the first light_count
-// handles -, the emission (the mean of max(texel, 0) of an image emission), the sidedness and the emissive meshes' triangles.
-int capture_light_source(lrk_ctx *ctx, const lrk_scene_desc *s, LightTreeSource &src) {
-    src = LightTreeSource{};
-    src.instance_count = s->instance_count;
-    for (uint32_t i = 0; i < s->instance_count; i++) {
-        const auto &inst = s->instances[i];
-        if (!(inst.handle[0] & LRK_SHAPE_HAS_LIGHT)) continue;
-        const uint32_t tag = inst.handle[1] & 4095u;
-        if (tag >= s->light_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: light tag out of range");
-        const lrk_light &light = s->lights[tag];
-        double rgb[3] = {light.emission[0], light.emission[1], light.emission[2]};
-        if (light.emission_tex != 0u) {
-            const lrk_texture &t = s->textures[light.emission_tex - 1u];
-            const size_t texels = static_cast<size_t>(t.width) * t.height;
-            double sum[3] = {0.0, 0.0, 0.0};
-            for (size_t k = 0; k < texels; k++)
-                for (int c = 0; c < 3; c++) sum[c] += std::max(static_cast<double>(s->texels[(t.texel_offset + k) * 4u + c]), 0.0);
-            for (int c = 0; c < 3; c++) rgb[c] = sum[c] / static_cast<double>(texels);
-        }
-        for (double &c : rgb) c = std::max(c, 0.0);
-        const double lum = 0.2126 * rgb[0] + 0.7152 * rgb[1] + 0.0722 * rgb[2];
-        src.inst.push_back(i);
-        src.mesh.push_back(inst.mesh);
-        src.o2w.insert(src.o2w.end(), inst.object_to_world, inst.object_to_world + 12);
-        src.power.push_back(lum * light.scale);
-        src.two_sided.push_back(light.two_sided != 0u ? 1u : 0u);
-        auto &points = src.mesh_points[inst.mesh];
-        if (!points.empty()) continue;
-        const lrk_mesh &mesh = s->meshes[inst.mesh];
-        for (uint32_t t = 0; t < mesh.triangle_count; t++) {
-            const lrk_triangle &tri = s->triangles[mesh.triangle_offset + t];
-            for (uint32_t v : {tri.i0, tri.i1, tri.i2}) points.insert(points.end(), s->vertices[mesh.vertex_offset + v].p, s->vertices[mesh.vertex_offset + v].p + 3);
-        }
-    }
-    return LRK_OK;
-}
-
 // The light tree of the option "light_tree" (light_tree.h) over the emitters of `src`: world-space triangles, power and sidedness.
 // tree_inst: per tree light its instance; inst_light: per instance its tree light, kLightTreeNone for instances without a light or
 // without power.
@@ -977,34 +921,8 @@ bool LightSampling::*light_sampling_option(const std::string &name) {
     return nullptr;
 }
 
-// lrk_upload_scene's refusals of the requested light sampling
-int check_light_sampling(lrk_ctx *ctx, const lrk_scene_desc *s) {
-    const LightSampling &want = ctx->light_requested;
-    const bool volume = s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH;
-    if (want.tree && volume)
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: the light tree (option light_tree) serves the surface integrator only; the volume "
-                                              "integrator selects its lights uniformly");
-    if (want.triangles && !want.tree)
-        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: the triangle-level light trees (option light_tree_triangles) are the bottom "
-                                                   "level of the light tree: set the option light_tree too");
-    if (want.solid_angle && volume)
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: solid-angle light sampling (option light_solid_angle) serves the surface integrator "
-                                              "only; the volume integrator evaluates its light pdfs from the world origin");
-    if (want.candidates >= 2u && volume)
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: resampled next-event estimation (option light_candidates >= 2) serves the surface "
-                                              "integrator only; the volume integrator traces every light sample it draws, since the "
-                                              "occlusion of each advances its random stream");
-    if (want.receiver && volume)
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: receiver-aware light sampling (option light_receiver) serves the surface integrator "
-                                              "only; the volume integrator selects its lights uniformly by area");
-    if (want.receiver && !want.tree && !want.solid_angle)
-        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: receiver-aware light sampling (option light_receiver) refines the light tree "
-                                                   "and solid-angle sampling: set the option light_tree or light_solid_angle too");
-    return LRK_OK;
-}
-
 // The light sampling `want` of the uploaded scene, once the scene record is in a.scene_copy (lrk_upload_scene: the requested one,
-// the scene updates: the active one): builds and uploads the light tree and its bottom trees from ctx->light_source where
+// the scene updates: the active one): builds and uploads the light tree and its bottom trees from ctx->update.light_source where
 // requested, writes the record the kernels find them through (scene.cuh: null arrays for what is off) after the scene record,
 // and latches `want` into ctx->light_active.
 int upload_light_sampling(lrk_ctx *ctx, const LightSampling want) {
@@ -1014,7 +932,7 @@ int upload_light_sampling(lrk_ctx *ctx, const LightSampling want) {
     LightTreeBuild tree;
     std::vector<uint32_t> tree_inst, inst_light;
     if (want.tree) {
-        build_light_tree(ctx->light_source, tree, tree_inst, inst_light);
+        build_light_tree(ctx->update.light_source, tree, tree_inst, inst_light);
         if ((rc = upload(ctx, a.lt_nodes, tree.nodes.data(), tree.nodes.size()))) return rc;
         if ((rc = upload(ctx, a.lt_light_inst, tree_inst.data(), tree_inst.size()))) return rc;
         if ((rc = upload(ctx, a.lt_trail, tree.trail.data(), tree.trail.size()))) return rc;
@@ -1028,7 +946,7 @@ int upload_light_sampling(lrk_ctx *ctx, const LightSampling want) {
     std::vector<uint32_t> inst_bottom;
     std::vector<unsigned long long> bottom_trail;
     if (want.triangles) {
-        build_bottom_light_trees(ctx->light_source, inst_light, bottom_nodes, inst_bottom, bottom_trail);
+        build_bottom_light_trees(ctx->update.light_source, inst_light, bottom_nodes, inst_bottom, bottom_trail);
         if ((rc = upload(ctx, a.lt_bottom_nodes, bottom_nodes.data(), bottom_nodes.size()))) return rc;
         if ((rc = upload(ctx, a.lt_inst_bottom, inst_bottom.data(), inst_bottom.size()))) return rc;
         if ((rc = upload(ctx, a.lt_bottom_trail, bottom_trail.data(), bottom_trail.size()))) return rc;
@@ -1053,8 +971,8 @@ int upload_light_sampling(lrk_ctx *ctx, const LightSampling want) {
 // Scene updates rebuild the instance level in place: the host's SAH build with one instance per leaf and the device's LBVH both
 // emit max(visible, 2) - 1 nodes, behind every mesh's BLAS.  Checked before an update changes anything.
 int check_instance_level(lrk_ctx *ctx, const char *call) {
-    const uint32_t visible = static_cast<uint32_t>(ctx->visible_host.size());
-    if (static_cast<uint64_t>(ctx->scene.tlas_root) + std::max(visible, 2u) - 1u != ctx->bvh_node_count)
+    const uint32_t visible = static_cast<uint32_t>(ctx->update.visible_host.size());
+    if (static_cast<uint64_t>(ctx->scene.tlas_root) + std::max(visible, 2u) - 1u != ctx->update.bvh_node_count)
         return fail(ctx, LRK_ERR_UNSUPPORTED, std::string(call) + ": the uploaded hierarchy's instance level is not its last max(visible instances, 2) - 1 "
                                                                  "nodes, so it cannot be rebuilt in place");
     return LRK_OK;
@@ -1067,18 +985,18 @@ int finish_scene_update(lrk_ctx *ctx, bool lights_changed) {
     auto &a = ctx->arrays;
     auto stream = ctx->stream;
     int rc;
-    if (!ctx->tlas_inputs) {
-        LRK_CUDA(a.inst_mesh.reserve(std::max<size_t>(ctx->inst_mesh_host.size() * sizeof(uint32_t), 16u)));
-        LRK_CUDA(a.visible_ids.reserve(std::max<size_t>(ctx->visible_host.size() * sizeof(uint32_t), 16u)));
-        LRK_CUDA(a.mesh_bounds.reserve(std::max<size_t>(ctx->mesh_count, 1u) * sizeof(BuildBox)));
-        LRK_CUDA(cudaMemcpyAsync(a.inst_mesh.get(), ctx->inst_mesh_host.data(), ctx->inst_mesh_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-        LRK_CUDA(cudaMemcpyAsync(a.visible_ids.get(), ctx->visible_host.data(), ctx->visible_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-        blas_root_bounds_kernel<<<build_blocks(ctx->mesh_count), 256, 0, stream>>>(a.meshes.get<const lrk_mesh>(), a.bvh_nodes.get<const float4>(), ctx->mesh_count,
+    if (!ctx->update.tlas_inputs) {
+        LRK_CUDA(a.inst_mesh.reserve(std::max<size_t>(ctx->update.inst_mesh_host.size() * sizeof(uint32_t), 16u)));
+        LRK_CUDA(a.visible_ids.reserve(std::max<size_t>(ctx->update.visible_host.size() * sizeof(uint32_t), 16u)));
+        LRK_CUDA(a.mesh_bounds.reserve(std::max<size_t>(ctx->update.mesh_count, 1u) * sizeof(BuildBox)));
+        LRK_CUDA(cudaMemcpyAsync(a.inst_mesh.get(), ctx->update.inst_mesh_host.data(), ctx->update.inst_mesh_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        LRK_CUDA(cudaMemcpyAsync(a.visible_ids.get(), ctx->update.visible_host.data(), ctx->update.visible_host.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        blas_root_bounds_kernel<<<build_blocks(ctx->update.mesh_count), 256, 0, stream>>>(a.meshes.get<const lrk_mesh>(), a.bvh_nodes.get<const float4>(), ctx->update.mesh_count,
                                                                                   a.mesh_bounds.get<BuildBox>());
         LRK_CUDA(cudaGetLastError());
-        ctx->tlas_inputs = true;
+        ctx->update.tlas_inputs = true;
     }
-    const uint32_t visible = static_cast<uint32_t>(ctx->visible_host.size());
+    const uint32_t visible = static_cast<uint32_t>(ctx->update.visible_host.size());
     BuildScratch b;
     if ((rc = reserve_build_scratch(ctx, std::max(visible, 2u), b))) return rc;
     if ((rc = build_instance_level(ctx, b, visible, ctx->scene.tlas_root))) return rc;
@@ -1092,15 +1010,15 @@ int finish_scene_update(lrk_ctx *ctx, bool lights_changed) {
 // may be gone): the refit's start nodes, i.e. the inner nodes reachable from its root that have no inner child.  The range ends
 // at the next mesh's root or at the instance level: both builders lay the meshes' hierarchies out one after the other.
 int derive_refit_starts(lrk_ctx *ctx, uint32_t mesh) {
-    const uint32_t root = ctx->meshes_host[mesh].bvh_root;
+    const uint32_t root = ctx->update.meshes_host[mesh].bvh_root;
     uint32_t end = ctx->scene.tlas_root;
-    for (const auto &m : ctx->meshes_host)
+    for (const auto &m : ctx->update.meshes_host)
         if (m.bvh_root > root && m.bvh_root < end) end = m.bvh_root;
     std::vector<lrk_bvh_node> nodes(end - root);
     LRK_CUDA(cudaMemcpyAsync(nodes.data(), ctx->arrays.bvh_nodes.get<const lrk_bvh_node>() + root, nodes.size() * sizeof(lrk_bvh_node), cudaMemcpyDeviceToHost,
                              ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
-    const uint32_t first = static_cast<uint32_t>(ctx->refit_starts_host.size());
+    const uint32_t first = static_cast<uint32_t>(ctx->update.refit_starts_host.size());
     std::vector<uint32_t> stack{root};
     size_t walked = 0u;
     while (!stack.empty()) {
@@ -1116,15 +1034,15 @@ int derive_refit_starts(lrk_ctx *ctx, uint32_t mesh) {
             stack.push_back(ref);
             inner++;
         }
-        if (inner == 0u) ctx->refit_starts_host.push_back(n);
+        if (inner == 0u) ctx->update.refit_starts_host.push_back(n);
     }
-    ctx->refit_start[mesh] = {first, static_cast<uint32_t>(ctx->refit_starts_host.size()) - first};
+    ctx->update.refit_start[mesh] = {first, static_cast<uint32_t>(ctx->update.refit_starts_host.size()) - first};
     return LRK_OK;
 }
 
 // refit_starts_host to a.refit_starts: a pageable copy, not through upload(), which may page-lock the context's own vector
 int send_refit_starts(lrk_ctx *ctx) {
-    const auto &starts = ctx->refit_starts_host;
+    const auto &starts = ctx->update.refit_starts_host;
     if (starts.empty()) return LRK_OK;
     LRK_CUDA(ctx->arrays.refit_starts.reserve(starts.size() * sizeof(uint32_t)));
     LRK_CUDA(cudaMemcpyAsync(ctx->arrays.refit_starts.get(), starts.data(), starts.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
@@ -1164,8 +1082,8 @@ int refresh_emissive_mesh(lrk_ctx *ctx, uint32_t id, const lrk_vertex *v, const 
     LRK_CUDA(cudaMemcpyAsync(alias, table.data(), table.size() * sizeof(lrk_alias_entry), cudaMemcpyHostToDevice, ctx->stream));
     LRK_CUDA(cudaMemcpyAsync(pdf, pdf_table.data(), pdf_table.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     if (!ctx->light_active.tree) return LRK_OK;
-    const auto it = ctx->light_source.mesh_points.find(id);
-    if (it == ctx->light_source.mesh_points.end()) return LRK_OK;
+    const auto it = ctx->update.light_source.mesh_points.find(id);
+    if (it == ctx->update.light_source.mesh_points.end()) return LRK_OK;
     auto &points = it->second;
     points.clear();
     for (uint32_t t = 0; t < n; t++)
@@ -1187,6 +1105,13 @@ void point_scene_at_geometry(lrk_ctx *ctx, uint32_t tlas_root) {
     sc.bvh_nodes = a.bvh_nodes.get<const float4>();
     sc.tri_verts = a.tri_verts.get<const float4>();
     sc.tlas_root = tlas_root;
+}
+
+// The scene record's copy in device memory (DeviceScene::self), for the out-of-line device functions; the light-tree record behind
+// it (upload_light_sampling) stays.  Asynchronous: the caller synchronises before ctx->scene changes again.
+int write_scene_record(lrk_ctx *ctx) {
+    LRK_CUDA(cudaMemcpyAsync(ctx->arrays.scene_copy.get(), &ctx->scene, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
+    return LRK_OK;
 }
 
 }// namespace
@@ -1268,104 +1193,30 @@ const char *lrk_last_error(const lrk_ctx *ctx) { return ctx ? ctx->error.c_str()
 
 int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     if (!ctx || !s) return LRK_ERR_INVALID_ARGUMENT;
-    if (s->abi_version != LRK_ABI_VERSION) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: ABI version mismatch");
-    // The volume integrator has two implementations.  The wavefront kernels (kernels.cuh) cover config C4's shape: ONE homogeneous
-    // environment medium around opaque Matte / Disney closures, nothing else.  Everything beyond that - media bound to shapes,
-    // transmissive surfaces, no environment medium, an environment light - runs the per-thread kernel of volume_general.cuh.
-    bool volume_general = false;
-    if (s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH) {
-        if (s->medium_count > 256u || (s->medium_count != 0u && s->media == nullptr))
-            return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: invalid media table");
-        if (s->environment_medium_tag != LRK_MEDIUM_INVALID_TAG && s->environment_medium_tag >= s->medium_count)
-            return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: environment medium tag outside the media table");
-        for (uint32_t m = 0; m < s->medium_count; m++) {
-            if (s->media[m].present != LRK_MEDIUM_HOMOGENEOUS && s->media[m].present != LRK_MEDIUM_VACUUM)
-                return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: unknown medium kind");
-            if (s->media[m].present == LRK_MEDIUM_HOMOGENEOUS && s->media[m].eta != 1.f)
-                return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: media with eta != 1 are not supported");
-        }
-        volume_general = !s->environment_medium.present || s->medium_count != 1u || s->environment.present;
-        for (uint32_t i = 0; i < s->instance_count && !volume_general; i++)
-            if (s->instances[i].handle[0] & LRK_SHAPE_HAS_MEDIUM) volume_general = true;
-        for (uint32_t i = 0; i < s->surface_count && !volume_general; i++)
-            if (s->surfaces[i].type > LRK_SURFACE_DISNEY || (s->surfaces[i].flags & (LRK_SURFACE_DISNEY_TRANSMISSIVE | LRK_SURFACE_DISNEY_THIN))) volume_general = true;
-        for (uint32_t i = 0; i < s->instance_count; i++) {
-            const uint32_t flags = s->instances[i].handle[0] & 1023u, tag = (s->instances[i].handle[1] >> 24u) & 255u;
-            if ((flags & LRK_SHAPE_HAS_MEDIUM) && tag >= s->medium_count)
-                return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: a shape's medium tag is outside the media table");
-        }
-        if (volume_general && s->sampler.type != LRK_SAMPLER_INDEPENDENT)
-            return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: the volume path with shape media / transmissive surfaces takes the Independent sampler");
-        if (s->integrator.max_depth > 31u) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: volume path depth > 31");
-    } else if (s->integrator.type != LRK_INTEGRATOR_PATH) {
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: unknown integrator type");
-    } else if (s->environment_medium.present) {
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: an environment medium needs the volume path integrator (MegaVPTNaive)");
-    }
-    if (s->integrator.max_depth > kMaxDepthSlots - 1u) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: max depth > 63");
-    if (const int rc = check_light_sampling(ctx, s)) return rc;
-    if (s->camera.resolution[0] > 65535u || s->camera.resolution[1] > 65535u)
-        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: film larger than 65535 pixels per side");
-    if (s->light_count == 0u && !s->environment.present)// !pipeline().has_lighting(), wave_path.cpp:224-228
-        return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "No lights in scene. Rendering aborted.");
-    if (s->environment.present) {
-        const auto &e = s->environment;
-        if (e.emission_tex > s->texture_count || !(e.env_prob > 0.f && e.env_prob <= 1.f) ||
-            (e.emission_tex != 0u && (e.map_width == 0u || e.map_height == 0u || e.alias == nullptr || e.pdf == nullptr)))
-            return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: invalid environment record");
-        if (s->light_count == 0u && e.env_prob != 1.f) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: env_prob must be 1 without area lights");
-    }
-    for (uint32_t i = 0; i < s->surface_count; i++) {
-        if (s->surfaces[i].type >= LRK_SURFACE_TYPE_COUNT) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: unknown surface type");
-        if (s->surfaces[i].type == LRK_SURFACE_MIX && (s->surfaces[i].flags & LRK_SURFACE_HAS_TEXTURES) && s->surfaces[i].tex[0] != 0u)
-            return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: the ratio of a Mix is a constant");
-        if ((s->surfaces[i].flags & LRK_SURFACE_RAW_PARAMS) && (s->surfaces[i].type < LRK_SURFACE_MIRROR || s->surfaces[i].type > LRK_SURFACE_METAL))
-            return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: LRK_SURFACE_RAW_PARAMS is for Mirror / Glass / Plastic / Metal records");
-        if (s->surfaces[i].type == LRK_SURFACE_LAYERED) {
-            if (s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
-                return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: Layered surfaces are not supported by the volume path integrator");
-            if ((s->surfaces[i].lobes >> 16u) == 0u) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: a Layered surface needs samples >= 1");
-        }
-        if (s->surfaces[i].type == LRK_SURFACE_MIX || s->surfaces[i].type == LRK_SURFACE_LAYERED) {
-            for (uint32_t child : {s->surfaces[i].mix_a, s->surfaces[i].mix_b}) {
-                if (child >= s->surface_count || s->surfaces[child].type >= LRK_SURFACE_MIX || s->surfaces[child].type == LRK_SURFACE_DISNEY ||
-                    (s->surfaces[child].flags & (LRK_SURFACE_HAS_TEXTURES | LRK_SURFACE_HAS_NORMAL_MAP | LRK_SURFACE_MAYBE_NON_OPAQUE)))
-                    return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: a Mix / Layered surface combines two constant Matte / Mirror / Glass / Plastic / Metal records");
-            }
-        }
-        for (uint32_t k = 0; k < 16u; k++)
-            if (s->surfaces[i].tex[k] > s->texture_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: texture id out of range");
-        if (s->surfaces[i].opacity_tex > s->texture_count || s->surfaces[i].normal_tex > s->texture_count)
-            return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: texture id out of range");
-        if ((s->surfaces[i].flags & LRK_SURFACE_MAYBE_NON_OPAQUE) && s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
-            return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: non-opaque surfaces are not supported by the volume path integrator");
-    }
-    if (s->sampler.type > LRK_SAMPLER_ZSOBOL) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: unknown sampler type");
-    if (s->sampler.type != LRK_SAMPLER_INDEPENDENT) {
-        const auto &q = s->sampler;
-        if (s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH)
-            return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_upload_scene: the volume path integrator supports the Independent sampler only");
-        const bool ok = q.spp != 0u && q.sobol_matrices != nullptr &&
-                        (q.type != LRK_SAMPLER_PMJ02BN || (q.pmj_samples && q.blue_noise && q.pmj_pixel_samples && q.tile != 0u && q.spp <= 65536u &&
-                                                           q.pmj_pixel_sample_count == static_cast<uint64_t>(q.tile) * q.tile * q.spp)) &&
-                        (q.type != LRK_SAMPLER_SOBOL || (q.vdc && q.vdc_inv && q.scale != 0u && q.scale <= 0xffffu)) &&
-                        (q.type != LRK_SAMPLER_ZSOBOL || (q.zsobol_hash != nullptr && q.num_base4_digits <= 32u));
-        if (!ok) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: incomplete sampler record");
-    }
-    ctx->textured = false;
-    for (uint32_t i = 0; i < s->surface_count; i++)
-        if (s->surfaces[i].flags & (LRK_SURFACE_HAS_TEXTURES | LRK_SURFACE_HAS_NORMAL_MAP)) ctx->textured = true;
-    for (uint32_t i = 0; i < s->light_count; i++)
-        if (s->lights[i].emission_tex != 0u) ctx->textured = true;// image emission: looked up by the TEXTURED kernel variants only
-    for (uint32_t i = 0; i < s->texture_count; i++) {
-        const auto &t = s->textures[i];
-        if (t.width == 0u || t.height == 0u || t.texel_offset + static_cast<uint64_t>(t.width) * t.height > s->texel_count ||
-            t.address > LRK_TEX_ADDRESS_ZERO || t.filter > LRK_TEX_FILTER_LINEAR || t.encoding > LRK_TEX_ENCODING_GAMMA)
-            return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: invalid image texture record");
-    }
-    for (uint32_t i = 0; i < s->light_count; i++)
-        if (s->lights[i].emission_tex > s->texture_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: a light's emission texture id is out of range");
+    SceneCheck checked = check_scene_desc(*s, ctx->light_requested, ctx->device_bvh);
+    if (checked.status != LRK_OK) return fail(ctx, checked.status, checked.error);
     LRK_CUDA(cudaSetDevice(ctx->device));
+    // from here on the context has no scene until the scene record and its device copy are complete: a CUDA failure on the way
+    // leaves no record that points at half-written arrays
+    ctx->has_scene = false;
+    ctx->textured = checked.textured;
+    ctx->used_kinds = checked.used_kinds;
+    ctx->any_non_opaque = checked.any_non_opaque;
+    ctx->volume = checked.volume;
+    ctx->volume_general = checked.volume_general;
+    {
+        SceneUpdateState u;
+        u.inst_mesh_host = std::move(checked.inst_mesh);
+        u.visible_host = std::move(checked.visible);
+        u.mesh_count = s->mesh_count;
+        u.bvh_node_count = checked.node_count;
+        u.meshes_host.assign(s->meshes, s->meshes + s->mesh_count);
+        for (uint32_t m = 0; m < s->mesh_count; m++) u.meshes_host[m].bvh_root = checked.mesh_root[m];// the device builder's roots with device_bvh
+        u.mesh_emissive = std::move(checked.mesh_emissive);
+        u.refit_start.assign(s->mesh_count, {0u, 0u});
+        u.light_source = std::move(checked.light_source);
+        ctx->update = std::move(u);
+    }
     auto &a = ctx->arrays;
     int rc;
     if ((rc = upload(ctx, a.vertices, s->vertices, s->vertex_count))) return rc;
@@ -1419,62 +1270,30 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
         if (q.type == LRK_SAMPLER_ZSOBOL)
             if ((rc = upload(ctx, a.zsobol_hash, q.zsobol_hash, 2048u))) return rc;
     }
-    std::vector<uint32_t> handles(static_cast<size_t>(s->instance_count) * 4u), kinds(s->instance_count);
-    ctx->used_kinds = 1u;
-    ctx->any_non_opaque = false;
+    std::vector<uint32_t> handles(static_cast<size_t>(s->instance_count) * 4u);
     std::vector<float> o2w(static_cast<size_t>(s->instance_count) * 12u), xform(static_cast<size_t>(s->instance_count) * 16u);
-    ctx->tlas_inputs = false;
-    ctx->inst_mesh_host.resize(s->instance_count);
-    ctx->visible_host.clear();
-    ctx->mesh_emissive.assign(s->mesh_count, 0u);
     for (uint32_t i = 0; i < s->instance_count; i++) {
         const auto &inst = s->instances[i];
-        ctx->inst_mesh_host[i] = inst.mesh;
-        if (inst.visible) ctx->visible_host.push_back(i);
         std::memcpy(&handles[i * 4u], inst.handle, 16);
-        {// closure kind of the instance: the bucket key of the material sort
-            const uint32_t flags = inst.handle[0] & 1023u, surface_tag = (inst.handle[1] >> 12u) & 4095u;
-            uint32_t kind = kHitEmitter;
-            if (flags & LRK_SHAPE_HAS_SURFACE) {
-                if (surface_tag >= s->surface_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: surface tag out of range");
-                kind = hit_kind_of(s->surfaces[surface_tag]);
-            }
-            kinds[i] = kind;
-            ctx->used_kinds |= 1u << kind;
-            if ((flags & LRK_SHAPE_MAYBE_NON_OPAQUE) && (flags & LRK_SHAPE_HAS_SURFACE)) ctx->any_non_opaque = true;
-        }
-        if (inst.mesh >= s->mesh_count) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_upload_scene: mesh index out of range");
-        if (inst.handle[0] & LRK_SHAPE_HAS_LIGHT) ctx->mesh_emissive[inst.mesh] = 1u;
         std::memcpy(&o2w[i * 12u], inst.object_to_world, 48);
         std::memcpy(&xform[i * 16u], inst.world_to_object, 48);
         xform[i * 16u + 12u] = xform[i * 16u + 13u] = xform[i * 16u + 14u] = xform[i * 16u + 15u] = 0.f;
     }
     if ((rc = upload(ctx, a.inst_handles, handles.data(), handles.size()))) return rc;
-    if ((rc = upload(ctx, a.inst_kind, kinds.data(), kinds.size()))) return rc;
+    if ((rc = upload(ctx, a.inst_kind, checked.inst_kind.data(), checked.inst_kind.size()))) return rc;
     if ((rc = upload(ctx, a.inst_o2w, o2w.data(), o2w.size()))) return rc;
     // the hierarchy: the host's (the parity path: the oracle walks the same nodes) or one built here on the device
-    std::vector<uint32_t> mesh_root(s->mesh_count);
-    uint32_t tlas_root = s->tlas_root;
     if (ctx->device_bvh) {
         const auto t0 = std::chrono::steady_clock::now();
-        if ((rc = build_bvh_on_device(ctx, s, mesh_root, tlas_root))) return rc;
+        if ((rc = build_bvh_on_device(ctx, s, checked))) return rc;
         ctx->bvh_build_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    } else {
-        for (uint32_t m = 0; m < s->mesh_count; m++) mesh_root[m] = s->meshes[m].bvh_root;
-        ctx->bvh_node_count = s->bvh_node_count;
     }
-    ctx->mesh_count = s->mesh_count;
-    ctx->meshes_host.assign(s->meshes, s->meshes + s->mesh_count);
-    for (uint32_t m = 0; m < s->mesh_count; m++) ctx->meshes_host[m].bvh_root = mesh_root[m];// the device builder's roots with device_bvh
-    ctx->refit_starts_host.clear();
-    ctx->refit_start.assign(s->mesh_count, {0u, 0u});
-    ctx->emissive_triangles.clear();
-    for (uint32_t i = 0; i < s->instance_count; i++) std::memcpy(&xform[i * 16u + 12u], &mesh_root[s->instances[i].mesh], 4);
+    for (uint32_t i = 0; i < s->instance_count; i++) std::memcpy(&xform[i * 16u + 12u], &checked.mesh_root[s->instances[i].mesh], 4);
     if ((rc = upload(ctx, a.inst_xform, xform.data(), xform.size()))) return rc;
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));
 
     auto &sc = ctx->scene;
-    point_scene_at_geometry(ctx, tlas_root);
+    point_scene_at_geometry(ctx, checked.tlas_root);
     sc.inst_handles = a.inst_handles.get<const uint4>();
     sc.inst_kind = a.inst_kind.get<const uint32_t>();
     sc.inst_o2w = a.inst_o2w.get<const float4>();
@@ -1525,14 +1344,12 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     ctx->sampler_spp = s->sampler.spp;
     if (sc.refill_below == 0u) sc.refill_below = static_cast<uint32_t>(kRefillBelow);
     if (sc.inner_min == 0u) sc.inner_min = static_cast<uint32_t>(kInnerMin);
-    ctx->volume = s->integrator.type == LRK_INTEGRATOR_VOLUME_PATH;
     for (int i = 0; i < 3; i++) {
         sc.sigma_a[i] = s->environment_medium.sigma_a[i];
         sc.sigma_s[i] = s->environment_medium.sigma_s[i];
     }
     sc.medium_g = s->environment_medium.g;
     sc.medium_priority = s->environment_medium.priority;
-    ctx->volume_general = volume_general;
     if ((rc = upload(ctx, a.media, s->media, s->medium_count))) return rc;
     sc.media = a.media.get<const lrk_medium>();
     sc.medium_count = s->medium_count;
@@ -1546,9 +1363,7 @@ int lrk_upload_scene(lrk_ctx *ctx, const lrk_scene_desc *s) {
     {// the scene record itself in device memory, for the out-of-line device functions (DeviceScene::self), and the light tree's after it
         LRK_CUDA(a.scene_copy.reserve(sizeof(DeviceScene) + sizeof(DeviceLightTree)));
         sc.self = a.scene_copy.get<const DeviceScene>();
-        LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get(), &sc, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
-        ctx->light_source = LightTreeSource{};
-        if (ctx->light_requested.tree && (rc = capture_light_source(ctx, s, ctx->light_source))) return rc;
+        if ((rc = write_scene_record(ctx))) return rc;
         if ((rc = upload_light_sampling(ctx, ctx->light_requested))) return rc;
     }
     ctx->has_scene = true;
@@ -1584,7 +1399,7 @@ int lrk_update_instances(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, cons
     auto stream = ctx->stream;
     bool emitter_moved = false;
     if (ctx->light_active.tree) {
-        auto &src = ctx->light_source;
+        auto &src = ctx->update.light_source;
         for (const auto &u : updates) {
             const auto it = std::lower_bound(src.inst.begin(), src.inst.end(), u.id);
             if (it == src.inst.end() || *it != u.id) continue;
@@ -1606,12 +1421,12 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
     if (const int rc = open_scene_update(ctx, "lrk_update_meshes", count != 0u && (!ids || !vertices))) return rc;
     // everything is checked before anything changes
     std::vector<MeshRefit> entries(count);
-    std::vector<uint32_t> entry(ctx->mesh_count, ~0u);
+    std::vector<uint32_t> entry(ctx->update.mesh_count, ~0u);
     uint64_t total = 0u, slots = 0u;
     for (uint32_t k = 0; k < count; k++) {
         const uint32_t id = ids[k];
         if (const int rc = claim_update_id(ctx, "lrk_update_meshes", "mesh", id, k, entry)) return rc;
-        const lrk_mesh &m = ctx->meshes_host[id];
+        const lrk_mesh &m = ctx->update.meshes_host[id];
         entries[k] = MeshRefit{id, m.vertex_offset, m.triangle_offset, m.tri_slot_offset, static_cast<uint32_t>(total), static_cast<uint32_t>(slots), 0u, 0u};
         total += m.vertex_count;
         slots += m.triangle_count;
@@ -1620,7 +1435,7 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
         return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_update_meshes: vertex_count is " + std::to_string(vertex_count) + ", the meshes have " +
                                                        std::to_string(total) + " vertices");
     for (uint32_t k = 0; k < count; k++)
-        if (const int rc = check_finite_positions(ctx, "lrk_update_meshes", ids[k], vertices + entries[k].vertex_begin, ctx->meshes_host[ids[k]].vertex_count))
+        if (const int rc = check_finite_positions(ctx, "lrk_update_meshes", ids[k], vertices + entries[k].vertex_begin, ctx->update.meshes_host[ids[k]].vertex_count))
             return rc;
     if (const int rc = check_instance_level(ctx, "lrk_update_meshes")) return rc;
     LRK_CUDA(cudaSetDevice(ctx->device));
@@ -1630,17 +1445,17 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
     // a mesh's first update derives its refit's start nodes and, for an emissive mesh, downloads its triangles: nothing changes yet
     bool new_starts = false;
     for (const auto &e : entries) {
-        if (ctx->refit_start[e.mesh].second == 0u) {
+        if (ctx->update.refit_start[e.mesh].second == 0u) {
             if ((rc = derive_refit_starts(ctx, e.mesh))) return rc;
             new_starts = true;
         }
-        if (ctx->mesh_emissive[e.mesh] && ctx->emissive_triangles.count(e.mesh) == 0u) {
-            const lrk_mesh &m = ctx->meshes_host[e.mesh];
+        if (ctx->update.mesh_emissive[e.mesh] && ctx->update.emissive_triangles.count(e.mesh) == 0u) {
+            const lrk_mesh &m = ctx->update.meshes_host[e.mesh];
             std::vector<lrk_triangle> tris(m.triangle_count);
             LRK_CUDA(cudaMemcpyAsync(tris.data(), a.triangles.get<const lrk_triangle>() + m.triangle_offset, tris.size() * sizeof(lrk_triangle),
                                      cudaMemcpyDeviceToHost, stream));
             LRK_CUDA(cudaStreamSynchronize(stream));
-            ctx->emissive_triangles.emplace(e.mesh, std::move(tris));
+            ctx->update.emissive_triangles.emplace(e.mesh, std::move(tris));
         }
     }
     if (new_starts && (rc = send_refit_starts(ctx))) return rc;
@@ -1651,8 +1466,8 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
         uint32_t starts = 0u;
         for (auto &e : entries) {
             e.start_begin = starts;
-            e.start_first = ctx->refit_start[e.mesh].first;
-            starts += ctx->refit_start[e.mesh].second;
+            e.start_first = ctx->update.refit_start[e.mesh].first;
+            starts += ctx->update.refit_start[e.mesh].second;
         }
         std::vector<uint32_t> whole(6u * static_cast<size_t>(count));
         for (uint32_t k = 0; k < count; k++) std::memcpy(&whole[6u * k], kWholeInit, sizeof(kWholeInit));
@@ -1678,7 +1493,7 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
                                                                                static_cast<uint32_t>(vertex_count), a.vertices.get<lrk_vertex>());
         refit_triangles_kernel<<<build_blocks(slots), 256, 0, stream>>>(d_entries, count, static_cast<uint32_t>(slots), a.vertices.get<const lrk_vertex>(),
                                                                         a.triangles.get<const lrk_triangle>(), a.tri_verts.get<float4>(), slot_boxes, d_whole);
-        LRK_CUDA(a.mesh_bounds.reserve(std::max<size_t>(ctx->mesh_count, 1u) * sizeof(BuildBox)));
+        LRK_CUDA(a.mesh_bounds.reserve(std::max<size_t>(ctx->update.mesh_count, 1u) * sizeof(BuildBox)));
         refit_nodes_kernel<<<build_blocks(starts), 256, 0, stream>>>(d_entries, count, starts, a.refit_starts.get<const uint32_t>(), d_whole, slot_boxes,
                                                                      node_boxes, a.refit_visits.get<uint32_t>(), a.bvh_nodes.get<float4>(),
                                                                      a.mesh_bounds.get<BuildBox>());
@@ -1686,8 +1501,8 @@ int lrk_update_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const l
         // the emissive meshes' area alias tables, and their triangles in the light tree's source
         for (uint32_t k = 0; k < count; k++) {
             const MeshRefit &e = entries[k];
-            if (!ctx->mesh_emissive[e.mesh]) continue;
-            const auto &tris = ctx->emissive_triangles.at(e.mesh);
+            if (!ctx->update.mesh_emissive[e.mesh]) continue;
+            const auto &tris = ctx->update.emissive_triangles.at(e.mesh);
             if ((rc = refresh_emissive_mesh(ctx, e.mesh, vertices + e.vertex_begin, tris.data(), static_cast<uint32_t>(tris.size()),
                                             a.alias.get<lrk_alias_entry>() + e.triangle_offset, a.pdf.get<float>() + e.triangle_offset, tables[k], pdfs[k], lights_changed)))
                 return rc;
@@ -1701,7 +1516,7 @@ int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const 
     if (const int rc = open_scene_update(ctx, "lrk_replace_meshes", count != 0u && (!ids || !vertex_counts || !vertices || !triangle_counts || !triangles)))
         return rc;
     // everything is checked before anything changes
-    const uint32_t mesh_count = ctx->mesh_count;
+    const uint32_t mesh_count = ctx->update.mesh_count;
     std::vector<uint32_t> entry(mesh_count, ~0u);// per mesh the index k of its id, ~0u for an unchanged mesh
     std::vector<uint64_t> vertex_begin(count + 1u, 0u), triangle_begin(count + 1u, 0u);// where id k's records start in the caller's arrays
     for (uint32_t k = 0; k < count; k++) {
@@ -1724,9 +1539,9 @@ int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const 
     // instance level), a replaced one gets the device builder's max(n - 1, 1) nodes; the instance level goes last
     const uint32_t old_tlas = ctx->scene.tlas_root;
     std::vector<uint32_t> roots(mesh_count);
-    for (uint32_t m = 0; m < mesh_count; m++) roots[m] = ctx->meshes_host[m].bvh_root;
+    for (uint32_t m = 0; m < mesh_count; m++) roots[m] = ctx->update.meshes_host[m].bvh_root;
     std::sort(roots.begin(), roots.end());
-    std::vector<lrk_mesh> layout(ctx->meshes_host);
+    std::vector<lrk_mesh> layout(ctx->update.meshes_host);
     std::vector<uint32_t> node_count(mesh_count);
     uint64_t vertex_total = 0u, triangle_total = 0u, node_total = 0u, max_n = 0u;
     for (uint32_t m = 0; m < mesh_count; m++) {
@@ -1746,13 +1561,14 @@ int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const 
         vertex_total += r.vertex_count;
         triangle_total += r.triangle_count;
         node_total += node_count[m];
-        if (vertex_total > 0xffffffffull || triangle_total >= (1ull << 28) || node_total >= 0x7fffffffull)
+        if (!fits_bvh_encoding(node_total, triangle_total, vertex_total))
             return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_replace_meshes: scene too large for the BVH encoding");
     }
-    const uint32_t visible = static_cast<uint32_t>(ctx->visible_host.size());
+    const uint32_t visible = static_cast<uint32_t>(ctx->update.visible_host.size());
     const uint32_t tlas_root = static_cast<uint32_t>(node_total);
     node_total += std::max(visible, 2u) - 1u;
-    if (node_total >= 0x7fffffffull) return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_replace_meshes: scene too large for the BVH encoding");
+    if (!fits_bvh_encoding(node_total, triangle_total, vertex_total))
+        return fail(ctx, LRK_ERR_UNSUPPORTED, "lrk_replace_meshes: scene too large for the BVH encoding");
     // the unchanged meshes' records move in runs: consecutive meshes whose old ranges follow each other in every array
     struct Run {
         uint32_t last, old_v, new_v, vertices, old_t, new_t, old_s, triangles, old_n, new_n, nodes;
@@ -1760,7 +1576,7 @@ int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const 
     std::vector<Run> runs;
     for (uint32_t m = 0; m < mesh_count; m++) {
         if (entry[m] != ~0u) continue;
-        const lrk_mesh &o = ctx->meshes_host[m], &r = layout[m];
+        const lrk_mesh &o = ctx->update.meshes_host[m], &r = layout[m];
         if (!runs.empty()) {
             Run &p = runs.back();
             if (p.last + 1u == m && p.old_v + p.vertices == o.vertex_offset && p.old_t + p.triangles == o.triangle_offset &&
@@ -1836,11 +1652,11 @@ int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const 
         const lrk_triangle *tris = triangles + triangle_begin[k];
         LRK_CUDA(cudaMemcpyAsync(nv.get<lrk_vertex>() + r.vertex_offset, vertices + vertex_begin[k], uint64_t{r.vertex_count} * sizeof(lrk_vertex), cudaMemcpyHostToDevice, stream));
         LRK_CUDA(cudaMemcpyAsync(nt.get<lrk_triangle>() + r.triangle_offset, tris, uint64_t{r.triangle_count} * sizeof(lrk_triangle), cudaMemcpyHostToDevice, stream));
-        if (ctx->mesh_emissive[id]) {
+        if (ctx->update.mesh_emissive[id]) {
             if ((rc = refresh_emissive_mesh(ctx, id, vertices + vertex_begin[k], tris, r.triangle_count, nalias.get<lrk_alias_entry>() + r.triangle_offset,
                                             npdf.get<float>() + r.triangle_offset, tables[k], pdfs[k], lights_changed)))
                 return rc;
-            ctx->emissive_triangles[id].assign(tris, tris + r.triangle_count);
+            ctx->update.emissive_triangles[id].assign(tris, tris + r.triangle_count);
         } else {
             LRK_CUDA(cudaMemsetAsync(nalias.get<lrk_alias_entry>() + r.triangle_offset, 0, uint64_t{r.triangle_count} * sizeof(lrk_alias_entry), stream));
             LRK_CUDA(cudaMemsetAsync(npdf.get<float>() + r.triangle_offset, 0, uint64_t{r.triangle_count} * sizeof(float), stream));
@@ -1867,22 +1683,21 @@ int lrk_replace_meshes(lrk_ctx *ctx, const uint32_t *ids, uint32_t count, const 
     // the host's copy of the layout: the refit starts of moved meshes move with their nodes, those of replaced meshes are derived again
     std::vector<uint32_t> starts;
     for (uint32_t m = 0; m < mesh_count; m++) {
-        auto &range = ctx->refit_start[m];
+        auto &range = ctx->update.refit_start[m];
         if (entry[m] != ~0u || range.second == 0u) {
             range = {0u, 0u};
             continue;
         }
-        const uint32_t first = static_cast<uint32_t>(starts.size()), delta = layout[m].bvh_root - ctx->meshes_host[m].bvh_root;
-        for (uint32_t j = 0; j < range.second; j++) starts.push_back(ctx->refit_starts_host[range.first + j] + delta);
+        const uint32_t first = static_cast<uint32_t>(starts.size()), delta = layout[m].bvh_root - ctx->update.meshes_host[m].bvh_root;
+        for (uint32_t j = 0; j < range.second; j++) starts.push_back(ctx->update.refit_starts_host[range.first + j] + delta);
         range.first = first;
     }
-    ctx->refit_starts_host.swap(starts);
+    ctx->update.refit_starts_host.swap(starts);
     if ((rc = send_refit_starts(ctx))) return rc;// never larger than the buffer it had
-    ctx->meshes_host.swap(layout);
-    ctx->bvh_node_count = node_total;
+    ctx->update.meshes_host.swap(layout);
+    ctx->update.bvh_node_count = node_total;
     point_scene_at_geometry(ctx, tlas_root);
-    // only the scene record: the light-tree record behind it (upload_light_sampling) stays
-    LRK_CUDA(cudaMemcpyAsync(a.scene_copy.get(), &ctx->scene, sizeof(DeviceScene), cudaMemcpyHostToDevice, stream));
+    if ((rc = write_scene_record(ctx))) return rc;
     return finish_scene_update(ctx, lights_changed);
 }
 
@@ -1994,7 +1809,7 @@ int lrk_set_option(lrk_ctx *ctx, const char *name, int64_t value) {
     else if (n == "refill_below" || n == "inner_min") {
         (n == "refill_below" ? ctx->scene.refill_below : ctx->scene.inner_min) = static_cast<uint32_t>(std::min<int64_t>(std::max<int64_t>(value, 1), 32));
         if (ctx->has_scene && ctx->arrays.scene_copy.get() != nullptr) {// keep DeviceScene::self in step
-            LRK_CUDA(cudaMemcpyAsync(ctx->arrays.scene_copy.get(), &ctx->scene, sizeof(DeviceScene), cudaMemcpyHostToDevice, ctx->stream));
+            if (const int rc = write_scene_record(ctx)) return rc;
             LRK_CUDA(cudaStreamSynchronize(ctx->stream));
         }
     }

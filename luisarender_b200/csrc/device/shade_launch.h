@@ -5,17 +5,9 @@
 #include <cuda_runtime.h>
 
 #include "pathstate.cuh"
+#include "scene_check.h"// LightSampling
 
 namespace lrk {
-
-// How next-event estimation picks a light and a point on it: the options "light_tree", "light_tree_triangles" (the light tree's
-// bottom level: set with tree only), "light_solid_angle", "light_candidates" (M: 0 .. 32, resampling from M candidates for
-// M >= 2) and "light_receiver" (the receiver's normal in the tree and the solid-angle sampler: set with tree or solid angle only; no
-// instantiation of its own).  Not part of the ABI.
-struct LightSampling {
-    bool tree{false}, triangles{false}, solid_angle{false}, receiver{false};
-    uint32_t candidates{0u};
-};
 
 #define LRK_DECLARE_SHADE_VARIANT(NS)                                                                                                        \
     namespace NS {                                                                                                                           \

@@ -306,6 +306,76 @@ def test_error_paths(cornell_small, gpu_renderer):
     assert C.sizeof(F.Stats) > 0
 
 
+def test_refused_uploads_leave_the_scene_and_the_film(textured_wrappers_small, gpu_renderer):
+    """A refused lrk_upload_scene leaves the context as it was: the film and the stats of the uploaded scene, and every later
+    render, trace and instance update, whatever the refused description would have replaced, and however large it is."""
+    from luisarender_b200 import _ffi as F
+    import ctypes as C
+    r = gpu_renderer
+    d = textured_wrappers_small.desc()
+    big = Scene.from_source(scenes.instanced_spheres(resolution=(64, 36), spp=4, big_subdivision=5, small_subdivision=2, small_count=12), REPO)
+    keep = []
+
+    def corrupted(desc, field=None, ctype=None, count=0, edit=None, **fields):
+        bad = F.SceneDesc.from_buffer_copy(bytes(desc))
+        for k, v in fields.items():
+            setattr(bad, k, v)
+        if field is not None:
+            arr = (ctype * max(count, 1))()
+            C.memmove(arr, getattr(desc, field), C.sizeof(ctype) * count)
+            edit(arr)
+            setattr(bad, field, C.cast(arr, C.POINTER(ctype)))
+            keep.append(arr)
+        return bad
+
+    b = big.desc()
+    light = next(i for i in range(b.instance_count) if b.instances[i].handle[0] & F.SHAPE_HAS_LIGHT)
+    shaded = next(i for i in range(b.instance_count) if b.instances[i].handle[0] & F.SHAPE_HAS_SURFACE)
+
+    def set_handle(i, word, value):
+        return lambda insts: insts[i].handle.__setitem__(word, value)
+
+    no_texture = F.Texture()  # width 0
+    keep.append(no_texture)
+    refused = [  # (description, device_bvh, message)
+        (corrupted(b, abi_version=99), False, "ABI version mismatch"),
+        (corrupted(b, texture_count=1, textures=C.pointer(no_texture)), False, "invalid image texture record"),
+        (corrupted(b, "instances", F.Instance, b.instance_count, set_handle(shaded, 1, b.instances[shaded].handle[1] | (4095 << 12))), False,
+         "surface tag out of range"),
+        (corrupted(b, "instances", F.Instance, b.instance_count, lambda insts: setattr(insts[b.instance_count - 1], "mesh", b.mesh_count)), False,
+         "mesh index out of range"),
+        (corrupted(b, "instances", F.Instance, b.instance_count, set_handle(light, 1, b.instances[light].handle[1] | 4095)), False,
+         "light tag out of range"),
+        (corrupted(b, "light_handles", F.LightHandle, b.light_count, lambda h: setattr(h[0], "instance_id", b.instance_count)), False,
+         "light handle instance id out of range"),
+        (corrupted(b, "meshes", F.Mesh, b.mesh_count, lambda m: setattr(m[b.mesh_count - 1], "triangle_count", 0)), True, "mesh without triangles"),
+        (corrupted(d, "light_handles", F.LightHandle, d.light_count, lambda h: setattr(h[0], "instance_id", d.instance_count)), False,
+         "light handle instance id out of range"),
+    ]
+    r.upload(d)
+    r.render(0, 4)
+    film, stats = r.film(raw=True), r.stats()
+    rays = _random_rays(textured_wrappers_small, 20_000, seed=23)
+    hits = r.trace(rays)
+    try:
+        for bad, device_bvh, message in refused:
+            r.set_option("device_bvh", int(device_bvh))
+            with pytest.raises(RuntimeError, match=message):
+                r.upload(bad)
+            assert np.array_equal(r.film(raw=True), film) and r.stats() == stats, message
+    finally:
+        r.set_option("device_bvh", 0)
+    r.clear()
+    r.render(0, 4)
+    assert np.array_equal(r.film(raw=True), film)
+    got = r.trace(rays)
+    assert all(np.array_equal(got[k], hits[k]) for k in hits.dtype.names)
+    rows = np.array([d.instances[i].object_to_world[:] for i in range(d.instance_count)], np.float32).reshape(-1, 3, 4)
+    r.update_instances(np.arange(d.instance_count), rows)
+    r.render(0, 4)
+    assert np.array_equal(r.film(raw=True), film)
+
+
 def test_full_size_properties_c2_cornell(gpu_renderer):
     """Config C2 geometry/resolution (1024x1024 Cornell) at a bounded spp: size-independent properties."""
     scene = Scene.from_source(scenes.cornell_box(resolution=(1024, 1024), spp=4096), REPO)
