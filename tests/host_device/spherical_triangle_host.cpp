@@ -1,5 +1,6 @@
 // spherical_triangle_host.cpp — the solid-angle triangle sampler (luisarender_b200/csrc/device/spherical_triangle.h, the header the
-// shade kernels include) compiled for the host, so that tests/test_light_solid_angle_cpu.py can check it without a GPU.
+// shade kernels include) compiled for the host, so that tests/test_light_solid_angle_cpu.py can check it, and
+// tests/test_light_receiver_cpu.py its receiver-cosine warp (option "light_receiver"), without a GPU.
 // TEST INFRASTRUCTURE: nothing here is part of the product.
 #include <cmath>
 #include <cstdint>
@@ -76,4 +77,31 @@ extern "C" void st_sample(int64_t n, const float *p, const float *v, const float
 // the pdf an emitter hit at point x evaluates, and the rule's choice there
 extern "C" void st_pdf(int64_t n, const float *p, const float *v, const float *x, float *pdf, int32_t *spherical) {
     for (int64_t i = 0; i < n; i++) pdf[i] = point_pdf(at(p, i), at(v, 3 * i), at(v, 3 * i + 1), at(v, 3 * i + 2), at(x, i), spherical + i);
+}
+
+// n samples: point p (3), receiver normal (3), triangle (9), (u0, u1) -> the unit direction, the point's barycentrics, the warp's pdf
+// factor evaluated at the point made (spherical_warp_pdf), the solid angle; warp 0 samples without the warp (factor 1)
+extern "C" void st_warp_sample(int64_t n, const float *p, const float *nr, const float *v, const float *u, float *dir, float *bary, float *factor,
+                               float *omega_out, int warp) {
+    for (int64_t i = 0; i < n; i++) {
+        const SphVec P = at(p, i), N = at(nr, i), A = at(v, 3 * i), B = at(v, 3 * i + 1), Cc = at(v, 3 * i + 2);
+        const float omega = lrk::solid_angle(P, A, B, Cc);
+        float u0 = u[2 * i], u1 = u[2 * i + 1];
+        if (warp) lrk::sample_bilinear(lrk::spherical_warp_weights(P, N, A, B, Cc), u0, u1);
+        const SphVec w = lrk::sample_spherical_direction(P, A, B, Cc, omega, u0, u1);
+        const SphVec b = lrk::spherical_barycentrics(P, A, B, Cc, w);
+        const SphVec x = point_of(A, B, Cc, b);
+        dir[3 * i] = w.x, dir[3 * i + 1] = w.y, dir[3 * i + 2] = w.z;
+        bary[3 * i] = b.x, bary[3 * i + 1] = b.y, bary[3 * i + 2] = b.z;
+        factor[i] = warp ? lrk::spherical_warp_pdf(P, N, A, B, Cc, omega, x) : 1.f;
+        omega_out[i] = omega;
+    }
+}
+
+// (u0, u1) of unit directions w (unwarped: the inverse of sample_spherical_direction)
+extern "C" void st_invert(int64_t n, const float *p, const float *v, const float *w, float *u) {
+    for (int64_t i = 0; i < n; i++) {
+        const SphVec P = at(p, i), A = at(v, 3 * i), B = at(v, 3 * i + 1), Cc = at(v, 3 * i + 2);
+        lrk::invert_spherical_triangle_sample(P, A, B, Cc, lrk::solid_angle(P, A, B, Cc), at(w, i), u[2 * i], u[2 * i + 1]);
+    }
 }

@@ -1,63 +1,21 @@
 """Receiver-aware light sampling (option "light_receiver") without a GPU: csrc/device/receiver.h (the receiver word), the receiver term
 of light_tree.h and the receiver-cosine warp of spherical_triangle.h, compiled for the host and checked on seeded normals, the light
-sets of test_light_tree_cpu.py and random triangles.  Also the one-sided bit of each closure kind and the option's surface in Python
-and on the command line."""
+sets and meshes of light_sampling_checks.py and random triangles.  Also the one-sided bit of each closure kind and the option's
+surface in Python and on the command line."""
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 
 import numpy as np
 import pytest
+from scipy import stats
 
 import host_harness
-from light_sampling_checks import check_cli_lists_and_parses_flag, check_python_option_rejects_bad_values
-from test_light_tree_cpu import LightSet
+from light_sampling_checks import (NONE, Bottom, LightSet, check_cli_flag, check_python_option, decode, encode, f32, icosphere,  # noqa: F401
+                                   lambert_irradiance, lib, spherical, unit)
 
-NONE = 0xFFFFFFFF
-f32 = np.float32
 ONE_SIDED_KINDS = {1, 2, 3, 5, 6}  # Matte, Disney, Mirror, Plastic, Metal (hit_kinds.h)
-
-
-@pytest.fixture(scope="module")
-def lib():
-    deps = [host_harness.DEVICE / n for n in ("receiver.h", "light_tree.h", "spherical_triangle.h")]
-    h = host_harness.load("light_receiver_host", deps, ["-O2", "-ffp-contract=off"])
-    h.lr_encode.argtypes = [C.c_int64] + [C.c_void_p] * 3
-    h.lr_decode.argtypes = [C.c_int64] + [C.c_void_p] * 3
-    h.lr_build.restype = C.c_void_p
-    h.lr_build.argtypes = [C.c_int] + [C.c_void_p] * 4
-    h.lr_free.argtypes = [C.c_void_p]
-    h.lr_pmf.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    h.lr_sample.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 5
-    h.lr_dead_mass.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 3
-    h.lrt_build.restype = C.c_void_p
-    h.lrt_build.argtypes = [C.c_int64, C.c_void_p, C.c_int]
-    h.lrt_free.argtypes = [C.c_void_p]
-    h.lrt_pmf.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 4 + [C.c_int, C.c_void_p]
-    h.lrt_sample.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 7
-    h.lrt_dead_mass.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 5
-    h.lr_warp_sample.argtypes = [C.c_int64] + [C.c_void_p] * 8 + [C.c_int]
-    h.lr_invert.argtypes = [C.c_int64] + [C.c_void_p] * 4
-    return h
-
-
-def unit(x):
-    return x / np.linalg.norm(x, axis=-1, keepdims=True)
-
-
-def encode(lib, normals, one_sided):
-    normals = np.ascontiguousarray(normals, f32)
-    flags = np.ascontiguousarray(np.broadcast_to(np.asarray(one_sided, np.int32), (len(normals),)))
-    words = np.zeros(len(normals), np.uint32)
-    lib.lr_encode(len(normals), normals.ctypes.data, flags.ctypes.data, words.ctypes.data)
-    return words
-
-
-def decode(lib, words):
-    words = np.ascontiguousarray(words, np.uint32)
-    n, k = np.zeros((len(words), 3), f32), np.zeros(len(words), np.uint32)
-    lib.lr_decode(len(words), words.ctypes.data, n.ctypes.data, k.ctypes.data)
-    return n, k
 
 
 # ---- the word ---------------------------------------------------------------------------------------------------------------------
@@ -79,27 +37,6 @@ def test_encoding_round_trip(lib):
 
 
 # ---- the tree -----------------------------------------------------------------------------------------------------------------------
-def tree_of(lib, ls):
-    counts = np.array([len(t) for t in ls.tris], np.int32)
-    tris = np.ascontiguousarray(np.concatenate([t.reshape(-1) for t in ls.tris]), np.float64)
-    power, two = np.array(ls.power, np.float64), np.array(ls.two_sided, np.int32)
-    return lib.lr_build(ls.n, counts.ctypes.data, tris.ctypes.data, power.ctypes.data, two.ctypes.data)
-
-
-def pmfs(lib, h, n_emitters, pts, words):
-    out = np.zeros((n_emitters, len(pts)), f32)
-    for e in range(n_emitters):
-        lib.lr_pmf(h, len(pts), pts.ctypes.data, words.ctypes.data, e, out[e].ctypes.data)
-    return out
-
-
-def sample(lib, h, pts, words, u):
-    light, pmf = np.zeros(len(pts), np.uint32), np.zeros(len(pts), f32)
-    u = np.ascontiguousarray(u, f32)
-    lib.lr_sample(h, len(pts), pts.ctypes.data, words.ctypes.data, u.ctypes.data, light.ctypes.data, pmf.ctypes.data)
-    return light, pmf
-
-
 SETS = [(2, 11), (7, 12), (1000, 13)]
 
 
@@ -108,32 +45,27 @@ def test_tree_pmfs_with_receivers(lib, n, seed):
     """For one-sided, two-sided and no receivers: sum of pmfs + P(no light) = 1, sampled pmf = evaluated pmf bit for bit, a
     two-sided receiver culls nothing the tree without a receiver keeps, and the word 0 gives the pmfs of the tree without a receiver."""
     ls = LightSet(n, seed)
-    h = tree_of(lib, ls)
-    try:
-        m = 64 if n == 1000 else 400
-        pts = ls.points(m, seed + 100)
-        rng = np.random.default_rng(seed)
-        normals = unit(rng.normal(size=(m, 3)))
-        base = pmfs(lib, h, n, pts, np.zeros(m, np.uint32))
-        for one_sided in (False, True):
-            words = encode(lib, normals, one_sided)
-            p = pmfs(lib, h, n, pts, words)
-            dead = np.zeros(m)
-            lib.lr_dead_mass(h, m, pts.ctypes.data, words.ctypes.data, dead.ctypes.data)
-            assert np.abs(p.astype(np.float64).sum(0) + dead - 1.0).max() < 1e-5
-            if not one_sided:
-                assert ((base > 0) <= (p > 0)).all()
-            for u in rng.random((8, m)):
-                light, pmf = sample(lib, h, pts, words, u)
-                ok = light != NONE
-                assert (pmf[~ok] == 0).all()
-                assert (pmf[ok].view(np.uint32) == p[light[ok], np.nonzero(ok)[0]].view(np.uint32)).all()
-        # the word 0 is the tree without a receiver, which is what test_light_tree_cpu.py checks
-        light, pmf = sample(lib, h, pts, np.zeros(m, np.uint32), rng.random(m))
-        ok = light != NONE
-        assert (pmf[ok].view(np.uint32) == base[light[ok], np.nonzero(ok)[0]].view(np.uint32)).all()
-    finally:
-        lib.lr_free(h)
+    tree = ls.build(lib)
+    m = 64 if n == 1000 else 400
+    pts = ls.points(m, seed + 100)
+    rng = np.random.default_rng(seed)
+    normals = unit(rng.normal(size=(m, 3)))
+    base = tree.pmfs(pts, np.zeros(m, np.uint32))
+    for one_sided in (False, True):
+        words = encode(lib, normals, one_sided)
+        p = tree.pmfs(pts, words)
+        assert np.abs(p.astype(np.float64).sum(0) + tree.dead_mass(pts, words) - 1.0).max() < 1e-5
+        if not one_sided:
+            assert ((base > 0) <= (p > 0)).all()
+        for u in rng.random((8, m)):
+            light, pmf = tree.sample(pts, u, words)
+            ok = light != NONE
+            assert (pmf[~ok] == 0).all()
+            assert (pmf[ok].view(np.uint32) == p[light[ok], np.nonzero(ok)[0]].view(np.uint32)).all()
+    # the word 0 is the tree without a receiver, which is what test_light_tree_cpu.py checks
+    light, pmf = tree.sample(pts, rng.random(m), np.zeros(m, np.uint32))
+    ok = light != NONE
+    assert (pmf[ok].view(np.uint32) == base[light[ok], np.nonzero(ok)[0]].view(np.uint32)).all()
 
 
 def test_tree_culls_only_lights_behind_a_one_sided_receiver(lib):
@@ -150,25 +82,21 @@ def test_tree_culls_only_lights_behind_a_one_sided_receiver(lib):
         ls.power.append(1.0)
         ls.two_sided.append(1)
     ls.n = n
-    h = tree_of(lib, ls)
-    try:
-        pts = np.zeros((1, 3), f32)
-        words = encode(lib, [[0.0, 0.0, 1.0]], True)
-        p = pmfs(lib, h, n, pts, words)[:, 0]
-        elev = np.arcsin(centres[:, 2] / np.linalg.norm(centres, axis=1))
-        radius = 0.1 / np.linalg.norm(centres, axis=1)  # angular radius of each emitter's bounds, padded
-        assert (p[elev > radius + 0.05] > 0).all()
-        assert (p[elev < -0.2] == 0).all()
-        assert (elev < -0.2).sum() > 50
-        two = pmfs(lib, h, n, pts, encode(lib, [[0.0, 0.0, 1.0]], False))[:, 0]
-        assert (two > 0).all()
-    finally:
-        lib.lr_free(h)
+    tree = ls.build(lib)
+    pts = np.zeros((1, 3), f32)
+    p = tree.pmfs(pts, encode(lib, [[0.0, 0.0, 1.0]], True))[:, 0]
+    elev = np.arcsin(centres[:, 2] / np.linalg.norm(centres, axis=1))
+    radius = 0.1 / np.linalg.norm(centres, axis=1)  # angular radius of each emitter's bounds, padded
+    assert (p[elev > radius + 0.05] > 0).all()
+    assert (p[elev < -0.2] == 0).all()
+    assert (elev < -0.2).sum() > 50
+    two = tree.pmfs(pts, encode(lib, [[0.0, 0.0, 1.0]], False))[:, 0]
+    assert (two > 0).all()
 
 
 # SHA-256 of the float32 pmfs [emitter, point] of LightSet(n, seed=n) at LightSet.points(64, n + 7), and of the bottom trees of the
 # level-3 icosphere at 32 seeded points per transform, computed with the parent commit's light_tree.h (through light_tree_host.cpp):
-# the word 0 must give these bytes.
+# the queries without words (a null word array) must give these bytes, and the word 0 the same.
 PARENT_TOP_PMF_SHA256 = {2: "255860b266726efb54cfcedd5005e73890959970698710666b3f3ead5a14dd2d",
                          7: "c41d047eb665814970fa5826533174017f71b898715a007410c63698243f5f77",
                          1000: "23bf362820d626ff9a5ef35d6d3c69c94b38df7cceb975df786d618784aa9c37"}
@@ -179,73 +107,27 @@ PARENT_BOTTOM_PMF_SHA256 = {"identity": "49d5574e5678e16b72914cd98eaf1460a6ab913
 
 @pytest.mark.parametrize("n", sorted(PARENT_TOP_PMF_SHA256))
 def test_zero_word_gives_the_parents_pmfs(lib, n):
-    import hashlib
-
     ls = LightSet(n, n)
-    h = tree_of(lib, ls)
-    try:
-        out = pmfs(lib, h, n, ls.points(64, n + 7), np.zeros(64, np.uint32))
-    finally:
-        lib.lr_free(h)
+    tree = ls.build(lib)
+    pts = ls.points(64, n + 7)
+    out = tree.pmfs(pts)
     assert hashlib.sha256(out.tobytes()).hexdigest() == PARENT_TOP_PMF_SHA256[n]
+    assert np.array_equal(tree.pmfs(pts, np.zeros(64, np.uint32)).view(np.uint32), out.view(np.uint32))
 
 
 def test_tree_draws_follow_the_pmf_with_a_receiver(lib):
     """10^6 draws at one point with a one-sided receiver: chi-square of the emitter counts against the evaluated pmfs."""
-    from scipy import stats
-
     ls = LightSet(7, 12)
-    h = tree_of(lib, ls)
-    try:
-        pts = np.repeat(ls.points(1, 3)[:1], 1_000_000, axis=0)
-        words = np.repeat(encode(lib, [[0.3, -0.5, 0.8]], True), len(pts))
-        p = pmfs(lib, h, 7, pts[:1], words[:1])[:, 0].astype(np.float64)
-        light, _ = sample(lib, h, pts, words, np.random.default_rng(9).random(len(pts)))
-    finally:
-        lib.lr_free(h)
+    tree = ls.build(lib)
+    pts = np.repeat(ls.points(1, 3)[:1], 1_000_000, axis=0)
+    words = np.repeat(encode(lib, [[0.3, -0.5, 0.8]], True), len(pts))
+    p = tree.pmfs(pts[:1], words[:1])[:, 0].astype(np.float64)
+    light, _ = tree.sample(pts, np.random.default_rng(9).random(len(pts)), words)
     counts = np.bincount(light[light != NONE], minlength=7)
     keep = p > 0
     assert counts[~keep].sum() == 0 and p.sum() > 0.5
     chi = stats.chisquare(counts[keep], p[keep] / p[keep].sum() * counts.sum())
     assert chi.pvalue > 1e-4, chi
-
-
-class BottomReceiver:
-    """A bottom tree of test_light_tree_triangles_cpu.py's meshes under one of its transforms, queried with receiver words."""
-
-    def __init__(self, lib, kind, side):
-        import test_light_tree_triangles_cpu as T
-
-        tris = T.icosphere(3) if side != 1 else T.icosphere(3)[:, ::-1]
-        self.lib, self.n = lib, len(tris)
-        flat = np.ascontiguousarray(np.asarray(tris, np.float64).reshape(-1))
-        self.h = lib.lrt_build(self.n, flat.ctypes.data, side)
-        o2w = T.xform(kind)
-        self.w2o = T.world_to_object(o2w)
-        self.o2w = np.ascontiguousarray(o2w[:, :3].reshape(-1), f32)
-        self.world = np.asarray(tris) @ o2w[:, :3].T + o2w[:, 3]
-
-    def free(self):
-        self.lib.lrt_free(self.h)
-
-    def pmfs(self, pts, words):
-        out = np.zeros((self.n, len(pts)), f32)
-        for k in range(self.n):
-            self.lib.lrt_pmf(self.h, len(pts), pts.ctypes.data, words.ctypes.data, self.w2o.ctypes.data, self.o2w.ctypes.data, k,
-                             out[k].ctypes.data)
-        return out
-
-    def sample(self, pts, words, u):
-        tri, pmf = np.zeros(len(pts), np.uint32), np.zeros(len(pts), f32)
-        u = np.ascontiguousarray(u, f32)
-        self.lib.lrt_sample(self.h, len(pts), pts.ctypes.data, words.ctypes.data, self.w2o.ctypes.data, self.o2w.ctypes.data, u.ctypes.data,
-                            tri.ctypes.data, pmf.ctypes.data)
-        return tri, pmf
-
-    def dead(self, pts, words):
-        out = np.zeros(len(pts))
-        self.lib.lrt_dead_mass(self.h, len(pts), pts.ctypes.data, words.ctypes.data, self.w2o.ctypes.data, self.o2w.ctypes.data, out.ctypes.data)
-        return out
 
 
 @pytest.mark.parametrize("kind,side", [("identity", 0), ("stretched", 0), ("mirrored", 1), ("stretched", 2)])
@@ -254,39 +136,35 @@ def test_bottom_trees_with_receivers(lib, kind, side):
     two-sided receivers, sum of pmfs + P(no light) = 1, sampled = evaluated bit for bit, a two-sided receiver culls nothing, and a
     one-sided receiver keeps every triangle that has a vertex in front of its WORLD-space plane by a margin (which a wrong
     object-space map of the normal would cull) and culls some that lie wholly behind it."""
-    import hashlib
-
-    b = BottomReceiver(lib, kind, side)
-    try:
-        rng = np.random.default_rng(3)
-        lo, hi = b.world.reshape(-1, 3).min(0), b.world.reshape(-1, 3).max(0)
-        pts = np.ascontiguousarray(rng.uniform(lo - 1, hi + 1, (32, 3)), f32)
-        base = b.pmfs(pts, np.zeros(32, np.uint32))
-        if side != 2:
-            assert hashlib.sha256(base.tobytes()).hexdigest() == PARENT_BOTTOM_PMF_SHA256[kind]
-        normals = unit(rng.normal(size=(32, 3)))
-        size = float(np.ptp(b.world.reshape(-1, 3), axis=0).max())
-        culled = 0
-        for one_sided in (False, True):
-            words = encode(lib, normals, one_sided)
-            p = b.pmfs(pts, words)
-            assert np.abs(p.astype(np.float64).sum(0) + b.dead(pts, words) - 1.0).max() < 1e-5
-            for u in rng.random((4, 32)):
-                tri, pmf = b.sample(pts, words, u)
-                ok = tri != NONE
-                assert (pmf[ok].view(np.uint32) == p[tri[ok], np.nonzero(ok)[0]].view(np.uint32)).all()
-            if not one_sided:
-                assert ((base > 0) <= (p > 0)).all()
-                continue
-            # [tri, point]: signed distance of each world vertex to the receiver's world plane
-            d = np.einsum("pc,tkpc->tkp", normals, b.world[:, :, None, :] - pts.astype(np.float64)[None, None])
-            front = (d > 0.05 * size).any(axis=1)
-            assert (p[front & (base > 0)] > 0).all()
-            behind = (d < -0.05 * size).all(axis=1)
-            culled += int(((p == 0) & behind & (base > 0)).sum())
-        assert culled > 0
-    finally:
-        b.free()
+    b = Bottom(lib, icosphere(3) if side != 1 else icosphere(3)[:, ::-1], side, kind)
+    rng = np.random.default_rng(3)
+    lo, hi = b.world.reshape(-1, 3).min(0), b.world.reshape(-1, 3).max(0)
+    pts = np.ascontiguousarray(rng.uniform(lo - 1, hi + 1, (32, 3)), f32)
+    base = b.pmfs(pts, np.zeros(32, np.uint32))
+    assert np.array_equal(b.pmfs(pts).view(np.uint32), base.view(np.uint32))
+    if side != 2:
+        assert hashlib.sha256(base.tobytes()).hexdigest() == PARENT_BOTTOM_PMF_SHA256[kind]
+    normals = unit(rng.normal(size=(32, 3)))
+    size = float(np.ptp(b.world.reshape(-1, 3), axis=0).max())
+    culled = 0
+    for one_sided in (False, True):
+        words = encode(lib, normals, one_sided)
+        p = b.pmfs(pts, words)
+        assert np.abs(p.astype(np.float64).sum(0) + b.dead_mass(pts, words) - 1.0).max() < 1e-5
+        for u in rng.random((4, 32)):
+            tri, pmf = b.sample(pts, u, words)
+            ok = tri != NONE
+            assert (pmf[ok].view(np.uint32) == p[tri[ok], np.nonzero(ok)[0]].view(np.uint32)).all()
+        if not one_sided:
+            assert ((base > 0) <= (p > 0)).all()
+            continue
+        # [tri, point]: signed distance of each world vertex to the receiver's world plane
+        d = np.einsum("pc,tkpc->tkp", normals, b.world[:, :, None, :] - pts.astype(np.float64)[None, None])
+        front = (d > 0.05 * size).any(axis=1)
+        assert (p[front & (base > 0)] > 0).all()
+        behind = (d < -0.05 * size).all(axis=1)
+        culled += int(((p == 0) & behind & (base > 0)).sum())
+    assert culled > 0
 
 
 # ---- the warp -----------------------------------------------------------------------------------------------------------------------
@@ -300,27 +178,31 @@ def warp_case(n, seed, close=False):
     return np.ascontiguousarray(p, f32), np.ascontiguousarray(nr, f32), np.ascontiguousarray(v, f32)
 
 
-def warp_sample(lib, p, nr, v, u, warp=True):
+def warp_sample(spherical, p, nr, v, u, warp=True):
     n = len(p)
     u = np.ascontiguousarray(u, f32)
     d, b = np.zeros((n, 3), f32), np.zeros((n, 3), f32)
     fac, om = np.zeros(n, f32), np.zeros(n, f32)
-    lib.lr_warp_sample(n, p.ctypes.data, nr.ctypes.data, v.ctypes.data, u.ctypes.data, d.ctypes.data, b.ctypes.data, fac.ctypes.data,
-                       om.ctypes.data, int(warp))
+    spherical.st_warp_sample(n, p.ctypes.data, nr.ctypes.data, v.ctypes.data, u.ctypes.data, d.ctypes.data, b.ctypes.data, fac.ctypes.data,
+                             om.ctypes.data, int(warp))
     return d, b, fac, om
 
 
-def test_invert_returns_the_sample_numbers(lib):
+def invert(spherical, p, v, d):
+    back = np.zeros((len(p), 2), f32)
+    spherical.st_invert(len(p), p.ctypes.data, v.ctypes.data, np.ascontiguousarray(d).ctypes.data, back.ctypes.data)
+    return back
+
+
+def test_invert_returns_the_sample_numbers(spherical):
     """Inverting sample_spherical_direction's direction gives (u0, u1) back.  Where the spherical triangle is not small (omega >= 0.05
     sr): median error below 1e-5, 99 % below 1e-4, all below 3e-3 (measured 8e-7, 4e-5, 1.4e-3).  Small spherical triangles
     (3e-4 to 0.05 sr), where fp32 loses the angles, separately: 99 % below 5e-2."""
     p, _, v = warp_case(100_000, 3)
     rng = np.random.default_rng(4)
     u = rng.uniform(0.02, 0.98, (len(p), 2)).astype(f32)
-    d, _, _, om = warp_sample(lib, p, np.zeros_like(p), v, u, warp=False)
-    back = np.zeros((len(p), 2), f32)
-    lib.lr_invert(len(p), p.ctypes.data, v.ctypes.data, np.ascontiguousarray(d).ctypes.data, back.ctypes.data)
-    err = np.abs(back - u).max(axis=1)
+    d, _, _, om = warp_sample(spherical, p, np.zeros_like(p), v, u, warp=False)
+    err = np.abs(invert(spherical, p, v, d) - u).max(axis=1)
     good = (om >= 0.05) & (om <= 6.22)
     small = (om >= 3e-4) & (om < 0.05)
     assert good.sum() > 50_000
@@ -329,27 +211,16 @@ def test_invert_returns_the_sample_numbers(lib):
         assert np.quantile(err[small], 0.99) < 5e-2
 
 
-def irradiance_estimates(lib, p, nr, v, u, warp):
+def irradiance_estimates(spherical, p, nr, v, u, warp):
     """L cos / pdf for L = 1 of a light sample on each triangle (pdf = factor / omega)."""
-    d, _, fac, om = warp_sample(lib, p, nr, v, u, warp)
+    d, _, fac, om = warp_sample(spherical, p, nr, v, u, warp)
     cos = np.einsum("ij,ij->i", d.astype(np.float64), nr.astype(np.float64))
     pdf = fac.astype(np.float64) / om
     return np.where(pdf > 0, np.maximum(cos, 0.0) / pdf, 0.0)
 
 
-def lambert(p, nr, v):
-    """Lambert's irradiance of a unit-radiance polygon: 1/2 sum over the edges of the angle times n . the edge normal."""
-    a = unit(v.astype(np.float64) - p.astype(np.float64)[:, None, :])
-    e = 0.0
-    for k in range(3):
-        b, c = a[:, k], a[:, (k + 1) % 3]
-        g = unit(np.cross(b, c))
-        e = e + np.arccos(np.clip(np.einsum("ij,ij->i", b, c), -1, 1)) * np.einsum("ij,ij->i", g, nr.astype(np.float64))
-    return 0.5 * np.abs(e)
-
-
 @pytest.mark.parametrize("close", [False, True])
-def test_warped_estimator_matches_lambert(lib, close):
+def test_warped_estimator_matches_lambert(spherical, close):
     """One receiver and one triangle wholly above it: the mean of L cos / pdf over 10^6 warped draws equals Lambert's polygon
     irradiance within 4 sigma; for a large, close triangle its variance is below the unwarped estimator's."""
     p, nr, v = warp_case(1, 21 if close else 22, close)
@@ -361,26 +232,23 @@ def test_warped_estimator_matches_lambert(lib, close):
     n = 1_000_000
     P, N, V = np.repeat(p, n, 0), np.repeat(nr, n, 0), np.repeat(v, n, 0)
     u = np.random.default_rng(7).random((n, 2)).astype(f32)
-    est = irradiance_estimates(lib, P, N, V, u, True)
-    want = lambert(p, nr, v)[0]
+    est = irradiance_estimates(spherical, P, N, V, u, True)
+    want = lambert_irradiance(p, nr, v)[0]
     assert abs(est.mean() - want) < 4 * est.std() / np.sqrt(n) + 1e-6 * want, (est.mean(), want)
     if close:
-        plain = irradiance_estimates(lib, P, N, V, u, False)
+        plain = irradiance_estimates(spherical, P, N, V, u, False)
         assert est.var() < 0.5 * plain.var(), (est.var(), plain.var())
 
 
-def test_warped_draws_follow_their_density(lib):
+def test_warped_draws_follow_their_density(spherical):
     """10^6 warped draws on one triangle, binned by their unwarped (u0, u1) on an 8 x 8 grid: chi-square against the bilinear
     density's cell masses (float64 integration of pbrt-v4's bilinear density)."""
-    from scipy import stats
-
     p, nr, v = warp_case(1, 31)
     n = 1_000_000
     P, N, V = np.repeat(p, n, 0), np.repeat(nr, n, 0), np.repeat(v, n, 0)
     u = np.random.default_rng(8).random((n, 2)).astype(f32)
-    d, _, _, om = warp_sample(lib, P, N, V, u, True)
-    back = np.zeros((n, 2), f32)
-    lib.lr_invert(n, P.ctypes.data, V.ctypes.data, np.ascontiguousarray(d).ctypes.data, back.ctypes.data)
+    d, _, _, om = warp_sample(spherical, P, N, V, u, True)
+    back = invert(spherical, P, V, d)
     a = unit(v[0].astype(np.float64) - p[0].astype(np.float64))
     w = np.maximum(0.01, np.abs(a @ nr[0].astype(np.float64)))
     w4 = np.array([w[1], w[1], w[0], w[2]])
@@ -465,14 +333,10 @@ def test_one_sided_table_is_the_checked_kinds():
                                                                                          kinds["Plastic"], kinds["Metal"]}
 
 
-# ---- Python and CLI ------------------------------------------------------------------------------------------------------------------
+# ---- Python and CLI ---------------------------------------------------------------------------------------------------------------
 def test_python_option_rejects_bad_values():
-    check_python_option_rejects_bad_values("light_receiver", light_tree=True)
-    from luisarender_b200.api import Renderer
-
-    with pytest.raises(ValueError):
-        Renderer(light_receiver=True)
+    check_python_option("light_receiver")
 
 
 def test_cli_lists_and_parses_flag(tmp_path):
-    check_cli_lists_and_parses_flag("--light-receiver", tmp_path)
+    check_cli_flag("light_receiver", tmp_path)

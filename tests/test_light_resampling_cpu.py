@@ -1,16 +1,17 @@
 """Resampled next-event estimation (option "light_candidates") without a GPU: csrc/device/light_resampling.h, the header the shade
 kernels include, compiled for the host - the reservoir's choice, the candidates' numbers, the estimator's mean and variance on a
-synthetic discrete problem, and the single-candidate weight.  Also the option's surface in Python and on the command line."""
+synthetic discrete problem, and the single-candidate weight.  Also the option's surface in Python and on the command
+line, and the glossy-desk scene generator."""
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 
 import numpy as np
 import pytest
 from scipy import stats
 
 import host_harness
+from light_sampling_checks import check_cli_flag, check_python_option
 
 f32 = np.float32
 
@@ -149,30 +150,14 @@ def test_single_candidate_weight_is_c_over_p(lib):
 
 # ---- the option's surface ---------------------------------------------------------------------------------------------------------
 def test_python_option_accepts_counts_and_rejects_other_values():
-    from luisarender_b200.api import Renderer
-
-    for bad in (-1, 33, 2.0, 4.5, True, False, "4", None):
-        with pytest.raises(ValueError):
-            Renderer(device_index=-1, light_candidates=bad)
+    check_python_option("light_candidates")
 
 
 def test_cli_lists_and_parses_light_candidates(tmp_path):
-    from luisarender_b200 import _ffi as F
-
-    cli = F.LIB_DIR / "luisa-render-cli"
-    r = subprocess.run([str(cli), "--help"], capture_output=True, text=True, timeout=60)
-    assert r.returncode == 0 and "--light-candidates <n>" in r.stdout
-    # valid counts parse: the run gets as far as reading the scene, which does not exist
-    for args in (["--light-candidates", "0"], ["--light-candidates", "8"], ["--light-candidates=32"]):
-        r = subprocess.run([str(cli), "-b", "cuda", *args, str(tmp_path / "missing.luisa")], capture_output=True, text=True, timeout=60)
-        assert r.returncode != 0 and "Unrecognized options" not in r.stderr and "missing.luisa" in r.stderr, r.stderr
-    # bad counts are refused before the scene is read
-    for bad in ("-1", "33", "4x"):
-        r = subprocess.run([str(cli), "-b", "cuda", f"--light-candidates={bad}", str(tmp_path / "missing.luisa")], capture_output=True,
-                           text=True, timeout=60)
-        assert r.returncode != 0 and "--light-candidates takes a count from 0 to 32" in r.stderr, r.stderr
+    check_cli_flag("light_candidates", tmp_path)
 
 
+# ---- the scene generator ----------------------------------------------------------------------------------------------------------
 def test_glossy_desk_scene_generator():
     from luisarender_b200 import scenes
 

@@ -1,34 +1,17 @@
 """Solid-angle light sampling (option "light_solid_angle") without a GPU: csrc/device/spherical_triangle.h, the header the shade kernels
 include, compiled for the host and checked on seeded random triangles and points - general, grazing, near a vertex, very close
 (solid angle near 2 pi) and far (below the 3e-4 sr threshold, area sampling).  Also the option's surface in Python and on the
-command line."""
+command line, and the near-light scene generators."""
 from __future__ import annotations
-
-import ctypes as C
 
 import numpy as np
 import pytest
 from scipy import stats
 
-import host_harness
-from light_sampling_checks import check_cli_lists_and_parses_flag, check_python_option_rejects_bad_values
+from light_sampling_checks import (check_cli_flag, check_python_option, f32, lambert_irradiance, spherical,  # noqa: F401 (a fixture)
+                                   unit)
 
-f32 = np.float32
 EPS = float(np.finfo(f32).eps)
-
-
-@pytest.fixture(scope="module")
-def lib():
-    h = host_harness.load("spherical_triangle_host", [host_harness.DEVICE / "spherical_triangle.h"], ["-O2", "-ffp-contract=off"])
-    h.st_solid_angle.argtypes = [C.c_int64] + [C.c_void_p] * 3
-    h.st_use_spherical.argtypes = [C.c_int64] + [C.c_void_p] * 2
-    h.st_sample.argtypes = [C.c_int64] + [C.c_void_p] * 8
-    h.st_pdf.argtypes = [C.c_int64] + [C.c_void_p] * 5
-    return h
-
-
-def unit(x):
-    return x / np.linalg.norm(x, axis=-1, keepdims=True)
 
 
 def omega64(p, v):
@@ -80,35 +63,35 @@ def case(name: str, n: int, seed: int):
     return np.ascontiguousarray(p, f32), np.ascontiguousarray(v, f32)
 
 
-def solid_angle(lib, p, v):
+def solid_angle(spherical, p, v):
     out = np.zeros(len(p), f32)
-    lib.st_solid_angle(len(p), p.ctypes.data, v.ctypes.data, out.ctypes.data)
+    spherical.st_solid_angle(len(p), p.ctypes.data, v.ctypes.data, out.ctypes.data)
     return out
 
 
-def sample(lib, p, v, u):
+def sample(spherical, p, v, u):
     n = len(p)
     u = np.ascontiguousarray(u, f32)
     b, x, w = (np.zeros((n, 3), f32) for _ in range(3))
     pdf, sph = np.zeros(n, f32), np.zeros(n, np.int32)
-    lib.st_sample(n, p.ctypes.data, v.ctypes.data, u.ctypes.data, b.ctypes.data, x.ctypes.data, w.ctypes.data, pdf.ctypes.data, sph.ctypes.data)
+    spherical.st_sample(n, p.ctypes.data, v.ctypes.data, u.ctypes.data, b.ctypes.data, x.ctypes.data, w.ctypes.data, pdf.ctypes.data, sph.ctypes.data)
     return b, x, w, pdf, sph.astype(bool)
 
 
-def evaluated_pdf(lib, p, v, x):
+def evaluated_pdf(spherical, p, v, x):
     pdf, sph = np.zeros(len(p), f32), np.zeros(len(p), np.int32)
     x = np.ascontiguousarray(x, f32)
-    lib.st_pdf(len(p), p.ctypes.data, v.ctypes.data, x.ctypes.data, pdf.ctypes.data, sph.ctypes.data)
+    spherical.st_pdf(len(p), p.ctypes.data, v.ctypes.data, x.ctypes.data, pdf.ctypes.data, sph.ctypes.data)
     return pdf, sph.astype(bool)
 
 
 # ---- the solid angle --------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name", CASES)
-def test_solid_angle_matches_float64(lib, name):
+def test_solid_angle_matches_float64(spherical, name):
     """|omega - omega64| / omega64 <= 32 eps (1 + kappa), kappa = |v0 - p| |N| / |(v0 - p).N| the condition number of the triple
     product (1 / sin of p's elevation over the plane seen from v0).  Measured: at most a third of that bound."""
     p, v = case(name, 200_000, seed=CASES.index(name) + 1)
-    got = solid_angle(lib, p, v).astype(np.float64)
+    got = solid_angle(spherical, p, v).astype(np.float64)
     want = omega64(p, v)
     P, V = p.astype(np.float64), v.astype(np.float64)
     n = np.cross(V[:, 1] - V[:, 0], V[:, 2] - V[:, 0])
@@ -116,17 +99,17 @@ def test_solid_angle_matches_float64(lib, name):
     kappa = np.linalg.norm(d0, axis=1) * np.linalg.norm(n, axis=1) / np.abs(np.einsum("ij,ij->i", d0, n))
     rel = np.abs(got - want) / want
     assert (rel <= 32 * EPS * (1.0 + kappa)).all(), rel.max()
-    spherical = (want >= 3e-4) & (want <= 6.22)
+    in_rule = (want >= 3e-4) & (want <= 6.22)
     if name == "far":
-        assert not spherical.any()
+        assert not in_rule.any()
     else:
-        assert spherical.mean() > 0.5
+        assert in_rule.mean() > 0.5
 
 
-def test_rule_bounds(lib):
+def test_rule_bounds(spherical):
     omega = np.array([0.0, 2.9e-4, 3e-4, 1.0, 6.22, 6.2201, 2 * np.pi, np.nan], f32)
     out = np.zeros(len(omega), np.int32)
-    lib.st_use_spherical(len(omega), omega.ctypes.data, out.ctypes.data)
+    spherical.st_use_spherical(len(omega), omega.ctypes.data, out.ctypes.data)
     assert out.tolist() == [0, 0, 1, 1, 1, 0, 0, 0]
 
 
@@ -138,9 +121,9 @@ DIRECTION_BOUND = {"general": 1e-4, "grazing": 1e-4, "near_vertex": 2e-3, "very_
 
 
 @pytest.mark.parametrize("name", CASES)
-def test_samples_are_points_of_the_triangle_in_the_sampled_direction(lib, name):
+def test_samples_are_points_of_the_triangle_in_the_sampled_direction(spherical, name):
     p, v = case(name, 200_000, seed=10 + CASES.index(name))
-    b, x, w, _, sph = sample(lib, p, v, np.random.default_rng(20).random((len(p), 2)))
+    b, x, w, _, sph = sample(spherical, p, v, np.random.default_rng(20).random((len(p), 2)))
     assert not np.isnan(b).any()
     assert (b >= 0).all() and (b <= 1).all()
     assert np.abs(b.astype(np.float64).sum(axis=1) - 1.0).max() <= 2 * EPS
@@ -156,14 +139,14 @@ def test_samples_are_points_of_the_triangle_in_the_sampled_direction(lib, name):
 
 
 @pytest.mark.parametrize("name", CASES)
-def test_sampled_pdf_is_the_evaluated_pdf(lib, name):
+def test_sampled_pdf_is_the_evaluated_pdf(spherical, name):
     """The pdf a sample returns and the pdf an emitter hit at the same point evaluates, bit for bit, with the same rule."""
     p, v = case(name, 100_000, seed=30 + CASES.index(name))
-    _, x, _, pdf, sph = sample(lib, p, v, np.random.default_rng(31).random((len(p), 2)))
-    ev_pdf, ev_sph = evaluated_pdf(lib, p, v, x)
+    _, x, _, pdf, sph = sample(spherical, p, v, np.random.default_rng(31).random((len(p), 2)))
+    ev_pdf, ev_sph = evaluated_pdf(spherical, p, v, x)
     assert np.array_equal(sph, ev_sph)
     assert np.array_equal(pdf.view(np.uint32), ev_pdf.view(np.uint32))
-    omega = solid_angle(lib, p, v)
+    omega = solid_angle(spherical, p, v)
     assert np.array_equal(pdf[sph], (f32(1.0) / omega[sph]))
 
 
@@ -201,13 +184,13 @@ CHI_CASES = [  # (point, triangle): the spherical sampler at its two ends and be
 
 
 @pytest.mark.parametrize("name, p0, tri", CHI_CASES, ids=[c[0] for c in CHI_CASES])
-def test_samples_are_uniform_in_solid_angle(lib, name, p0, tri):
+def test_samples_are_uniform_in_solid_angle(spherical, name, p0, tri):
     """Chi-square of 10^6 draws over the 64 cells of the triangle's regular subdivision, expected counts in proportion to the cells'
     float64 solid angles; fails at p < 1e-4."""
     draws, n = 1_000_000, 8
     p = np.ascontiguousarray(np.repeat(np.array([p0], f32), draws, axis=0))
     v = np.ascontiguousarray(np.repeat(np.array([tri], f32), draws, axis=0))
-    b, _, _, _, sph = sample(lib, p, v, np.random.default_rng(40).random((draws, 2)))
+    b, _, _, _, sph = sample(spherical, p, v, np.random.default_rng(40).random((draws, 2)))
     assert sph.all()
     sub, index = cells(np.array(tri, f32).astype(np.float64), n)
     expected = omega64(np.repeat(np.array([p0], f32).astype(np.float64), len(sub), axis=0), sub)
@@ -221,18 +204,6 @@ def test_samples_are_uniform_in_solid_angle(lib, name, p0, tri):
     assert stats.chisquare(obs[keep], exp[keep]).pvalue > 1e-4
 
 
-def lambert_irradiance(p, n, v):
-    """Lambert's formula for a polygon of unit radiance wholly above the receiver's plane: E = 1/2 sum_i theta_i (n . g_i), g_i the
-    unit normal of the plane through p and edge i, pointed so that every term is positive for a polygon facing the receiver."""
-    a = unit(np.asarray(v, np.float64) - p)
-    e = 0.0
-    for i in range(3):
-        g = np.cross(a[i], a[(i + 1) % 3])
-        theta = np.arctan2(np.linalg.norm(g), np.dot(a[i], a[(i + 1) % 3]))
-        e += theta * np.dot(n, g / np.linalg.norm(g))
-    return 0.5 * abs(e)
-
-
 IRRADIANCE_CASES = [  # receiver point and normal under a triangle: close and large, moderate, tilted, far (area sampling)
     ((0.1, 0.0, 0.0), (0.0, 0.0, 1.0), ((-1.0, -1.0, 0.3), (1.2, -0.8, 0.3), (0.1, 1.1, 0.3))),
     ((0.0, 0.0, 0.0), (0.0, 0.0, 1.0), ((-1.0, -1.0, 2.0), (1.2, -0.8, 2.0), (0.1, 1.1, 2.0))),
@@ -242,29 +213,29 @@ IRRADIANCE_CASES = [  # receiver point and normal under a triangle: close and la
 
 
 @pytest.mark.parametrize("p0, n0, tri", IRRADIANCE_CASES)
-def test_irradiance_estimate_matches_lambert(lib, p0, n0, tri):
+def test_irradiance_estimate_matches_lambert(spherical, p0, n0, tri):
     """The mean of L cos(theta) / pdf over 10^6 samples against Lambert's polygon irradiance, within 4 sigma."""
     draws = 1_000_000
     p = np.ascontiguousarray(np.repeat(np.array([p0], f32), draws, axis=0))
     v = np.ascontiguousarray(np.repeat(np.array([tri], f32), draws, axis=0))
-    _, x, _, pdf, sph = sample(lib, p, v, np.random.default_rng(50).random((draws, 2)))
+    _, x, _, pdf, sph = sample(spherical, p, v, np.random.default_rng(50).random((draws, 2)))
     wi = unit(x.astype(np.float64) - np.array(p0, np.float64))
     f = np.maximum(wi @ np.array(n0, np.float64), 0.0) / pdf.astype(np.float64)
-    want = lambert_irradiance(np.array(p0, np.float64), np.array(n0, np.float64), np.array(tri, np.float64))
+    want = lambert_irradiance(p0, n0, tri)
     se = f.std(ddof=1) / np.sqrt(draws)
     assert abs(f.mean() - want) <= 4.0 * se + 1e-6 * want, (f.mean(), want, se, sph.mean())
 
 
-def test_spherical_sampling_is_quieter_close_to_a_large_light(lib):
+def test_spherical_sampling_is_quieter_close_to_a_large_light(spherical):
     p0, n0, tri = IRRADIANCE_CASES[0]
     draws = 100_000
     p = np.ascontiguousarray(np.repeat(np.array([p0], f32), draws, axis=0))
     v = np.ascontiguousarray(np.repeat(np.array([tri], f32), draws, axis=0))
     u = np.random.default_rng(51).random((draws, 2))
-    _, x, _, pdf, sph = sample(lib, p, v, u)
+    _, x, _, pdf, sph = sample(spherical, p, v, u)
     assert sph.all()
     wi = unit(x.astype(np.float64) - np.array(p0, np.float64))
-    spherical = np.maximum(wi @ np.array(n0, np.float64), 0.0) / pdf
+    solid = np.maximum(wi @ np.array(n0, np.float64), 0.0) / pdf
     # area sampling of the same triangle from the same point: the pdf d^2 / (A cos_l)
     b = np.empty((draws, 3))
     lo = u[:, 0] < u[:, 1]
@@ -278,18 +249,19 @@ def test_spherical_sampling_is_quieter_close_to_a_large_light(lib):
     area = 0.5 * np.linalg.norm(nl)
     cos_l = np.abs(unit(d) @ (nl / np.linalg.norm(nl)))
     area_est = np.maximum(unit(d) @ np.array(n0), 0.0) * area * cos_l / (d * d).sum(axis=1)
-    assert spherical.var() < 0.5 * area_est.var()
+    assert solid.var() < 0.5 * area_est.var()
 
 
 # ---- the option's surface ---------------------------------------------------------------------------------------------------------
 def test_python_option_rejects_unknown_values():
-    check_python_option_rejects_bad_values("light_solid_angle")
+    check_python_option("light_solid_angle")
 
 
 def test_cli_lists_and_parses_light_solid_angle(tmp_path):
-    check_cli_lists_and_parses_flag("--light-solid-angle", tmp_path)
+    check_cli_flag("light_solid_angle", tmp_path)
 
 
+# ---- the scene generators ---------------------------------------------------------------------------------------------------------
 def test_near_light_scene_generators():
     from luisarender_b200 import scenes
 

@@ -1,155 +1,14 @@
 """The light tree (option "light_tree") without a GPU: csrc/device/light_tree.h, the header the shade kernels and lrk_upload_scene
 include, compiled for the host and checked on synthetic light sets of 1, 2, 7 and 1000 emitters that mix one-sided, two-sided,
 coincident and zero-power lights, at points inside and outside their bounds.  Also the option's surface in Python and on the
-command line."""
+command line, and the many-light scene generator."""
 from __future__ import annotations
-
-import ctypes as C
 
 import numpy as np
 import pytest
 from scipy import stats
 
-import host_harness
-from light_sampling_checks import check_cli_lists_and_parses_flag, check_python_option_rejects_bad_values
-
-NONE = 0xFFFFFFFF
-f32 = np.float32
-
-
-@pytest.fixture(scope="module")
-def lib():
-    """The harness of light_tree.h: the instance-level trees (lt_*) and the triangle-level ones (ltt_*, test_light_tree_triangles_cpu.py)."""
-    h = host_harness.load("light_tree_host", [host_harness.DEVICE / "light_tree.h"], ["-O2", "-ffp-contract=off"])
-    h.lt_build.restype = C.c_void_p
-    h.lt_build.argtypes = [C.c_int] + [C.c_void_p] * 4
-    h.lt_free.argtypes = [C.c_void_p]
-    h.lt_node_count.restype = C.c_int64
-    h.lt_node_count.argtypes = [C.c_void_p]
-    h.lt_copy.argtypes = [C.c_void_p] * 3
-    h.lt_pmf.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]
-    h.lt_sample.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 4
-    h.lt_dead_mass.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
-    h.ltt_build.restype = C.c_void_p
-    h.ltt_build.argtypes = [C.c_int64, C.c_void_p, C.c_int]
-    h.ltt_free.argtypes = [C.c_void_p]
-    h.ltt_node_count.restype = C.c_int64
-    h.ltt_node_count.argtypes = [C.c_void_p]
-    h.ltt_copy.argtypes = [C.c_void_p] * 3
-    h.ltt_pmf.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    h.ltt_sample.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 5
-    h.ltt_sample_u_left.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 4
-    h.ltt_dead_mass.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 3
-    return h
-
-
-class LightSet:
-    """Emitters as world-space triangles: one-sided quads facing random directions, two-sided quads, small one-sided boxes (normals
-    over the whole sphere), exact duplicates of earlier emitters and emitters of zero power."""
-
-    def __init__(self, n: int, seed: int):
-        rng = np.random.default_rng(seed)
-        self.tris, self.power, self.two_sided = [], [], []
-        for i in range(n):
-            kind = rng.integers(0, 5) if i else 0
-            if kind == 3 and i >= 1:  # coincident with an earlier emitter
-                j = int(rng.integers(0, i))
-                self.tris.append(self.tris[j].copy())
-                self.power.append(self.power[j])
-                self.two_sided.append(self.two_sided[j])
-                continue
-            c = rng.uniform(-5.0, 5.0, 3)
-            size = rng.uniform(0.05, 1.0)
-            if kind == 2:
-                t = box(c, size)
-            else:
-                n_ = rng.normal(size=3)
-                t = quad(c, n_ / np.linalg.norm(n_), size)
-            self.tris.append(t)
-            self.power.append(0.0 if kind == 4 else float(10.0 ** rng.uniform(-1.0, 1.0)))
-            self.two_sided.append(int(kind == 1))
-        self.n = n
-
-    def build(self, lib):
-        counts = np.array([len(t) for t in self.tris], np.int32)
-        tris = np.ascontiguousarray(np.concatenate([t.reshape(-1) for t in self.tris]), np.float64)
-        power = np.array(self.power, np.float64)
-        two = np.array(self.two_sided, np.int32)
-        return Tree(lib, lib.lt_build(self.n, counts.ctypes.data, tris.ctypes.data, power.ctypes.data, two.ctypes.data), self.n)
-
-    def points(self, count: int, seed: int) -> np.ndarray:
-        """Half of them inside an emitter's bounds, half around the whole set."""
-        rng = np.random.default_rng(seed)
-        inside = []
-        for _ in range(count // 2):
-            t = self.tris[rng.integers(0, self.n)].reshape(-1, 3)
-            lo, hi = t.min(0), t.max(0)
-            inside.append(rng.uniform(lo, hi))
-        outside = rng.uniform(-8.0, 8.0, (count - count // 2, 3))
-        return np.ascontiguousarray(np.concatenate([np.array(inside).reshape(-1, 3), outside]), f32)
-
-    def can_illuminate(self, e: int, p: np.ndarray, rng, samples: int = 64) -> np.ndarray:
-        """Whether some sampled point of emitter e emits towards each of the points p: facing its triangle's geometric normal, or
-        two-sided; never with zero power."""
-        if self.power[e] == 0.0:
-            return np.zeros(len(p), bool)
-        if self.two_sided[e]:
-            return np.ones(len(p), bool)
-        t = self.tris[e].reshape(-1, 3, 3)
-        k = rng.integers(0, len(t), samples)
-        b = rng.dirichlet([1, 1, 1], samples)
-        x = np.einsum("sj,sjc->sc", b, t[k])
-        nrm = np.cross(t[k, 1] - t[k, 0], t[k, 2] - t[k, 0])
-        facing = np.einsum("sc,psc->ps", nrm, p.astype(np.float64)[:, None, :] - x[None]) > 1e-6 * np.linalg.norm(nrm, axis=1)
-        return facing.any(axis=1)
-
-
-def quad(c, n, size):
-    a = np.cross(n, [1.0, 0.0, 0.0] if abs(n[0]) < 0.9 else [0.0, 1.0, 0.0])
-    a /= np.linalg.norm(a)
-    b = np.cross(n, a)  # (a, b, n) right-handed: the triangles' normal is +n
-    v = [c + size * (sa * a + sb * b) for sa, sb in ((-1, -1), (1, -1), (1, 1), (-1, 1))]
-    return np.array([[v[0], v[1], v[2]], [v[0], v[2], v[3]]], np.float64)
-
-
-def box(c, size):
-    faces = []
-    for axis in range(3):
-        for sign in (-1.0, 1.0):
-            n = np.zeros(3)
-            n[axis] = sign
-            faces.append(quad(c + size * n, n, size))
-    return np.concatenate(faces)
-
-
-class Tree:
-    def __init__(self, lib, handle, n):
-        self.lib, self.h, self.n = lib, handle, n
-
-    def __del__(self):
-        self.lib.lt_free(self.h)
-
-    def pmf(self, p, e):
-        out = np.zeros(len(p), f32)
-        self.lib.lt_pmf(self.h, len(p), p.ctypes.data, e, out.ctypes.data)
-        return out
-
-    def sample(self, p, u):
-        light, pmf = np.zeros(len(p), np.uint32), np.zeros(len(p), f32)
-        u = np.ascontiguousarray(u, f32)
-        self.lib.lt_sample(self.h, len(p), p.ctypes.data, u.ctypes.data, light.ctypes.data, pmf.ctypes.data)
-        return light, pmf
-
-    def dead_mass(self, p):
-        out = np.zeros(len(p), np.float64)
-        self.lib.lt_dead_mass(self.h, len(p), p.ctypes.data, out.ctypes.data)
-        return out
-
-    def bytes(self):
-        nodes = np.zeros(self.lib.lt_node_count(self.h) * 48, np.uint8)
-        trails = np.zeros(self.n, np.uint64)
-        self.lib.lt_copy(self.h, nodes.ctypes.data, trails.ctypes.data)
-        return nodes.tobytes() + trails.tobytes()
+from light_sampling_checks import NONE, LightSet, check_cli_flag, check_python_option, f32, lib  # noqa: F401 (lib: the harness's fixture)
 
 
 SETS = [1, 2, 7, 1000]
@@ -242,11 +101,11 @@ def test_single_light_pmf_is_exactly_one(lib):
 
 
 def test_python_option_rejects_unknown_values():
-    check_python_option_rejects_bad_values("light_tree")
+    check_python_option("light_tree")
 
 
 def test_cli_lists_and_parses_light_tree(tmp_path):
-    check_cli_lists_and_parses_flag("--light-tree", tmp_path)
+    check_cli_flag("light_tree", tmp_path)
 
 
 def test_many_light_scene_generator():

@@ -1,8 +1,8 @@
 """The triangle-level light trees (option "light_tree_triangles") without a GPU: the bottom trees of csrc/device/light_tree.h, built
 in object space over a level-3 icosphere (one-sided, mirrored and two-sided), a quad, a single triangle, a soup with degenerate
 triangles and a 20 480-triangle icosphere, and queried at world points mapped through identity, non-uniform and mirrored 3x4
-transforms with the expressions the shade kernels use.  Also the top-level trees' bytes against the parent's, and the option's
-surface in Python and on the command line."""
+transforms with the expressions the shade kernels use.  Also the top-level trees' bytes against the parent's, the option's surface
+in Python and on the command line, and the emissive globe's generator."""
 from __future__ import annotations
 
 import hashlib
@@ -11,122 +11,8 @@ import numpy as np
 import pytest
 from scipy import stats
 
-from light_sampling_checks import check_cli_lists_and_parses_flag, check_python_option_rejects_bad_values
-from luisarender_b200.scenes import _icosphere
-from test_light_tree_cpu import LightSet, lib  # noqa: F401 (lib: the fixture of light_tree.h's harness)
-
-NONE = 0xFFFFFFFF
-ONE_SIDED, MIRRORED, TWO_SIDED = 0, 1, 2
-f32 = np.float32
-
-
-# ---- meshes (object space, [n, 3, 3]) and transforms (object-to-world 3x4) -------------------------------------------------------
-def icosphere(level):
-    v, f = _icosphere(level)
-    return v[f]
-
-
-def quad():
-    v = np.array([(-1.0, 0.0, -1.0), (1.0, 0.0, -1.0), (1.0, 0.0, 1.0), (-1.0, 0.0, 1.0)])
-    return np.array([[v[0], v[2], v[1]], [v[0], v[3], v[2]]])  # normal +y
-
-
-def single():
-    return np.array([[(0.1, 0.2, 0.0), (1.3, -0.1, 0.2), (0.4, 0.9, -0.3)]])
-
-
-def soup():
-    """Random triangles, every fourth degenerate (two coincident vertices or three collinear ones)."""
-    rng = np.random.default_rng(5)
-    t = rng.uniform(-1.0, 1.0, (40, 3, 3))
-    t[::8, 1] = t[::8, 0]
-    t[4::8, 2] = 0.5 * (t[4::8, 0] + t[4::8, 1])
-    return t
-
-
-def xform(kind):
-    if kind == "identity":
-        return np.hstack([np.eye(3), np.zeros((3, 1))])
-    if kind == "stretched":  # rotation times non-uniform scale
-        a, b = np.radians(35.0), np.radians(20.0)
-        rz = np.array([[np.cos(a), -np.sin(a), 0.0], [np.sin(a), np.cos(a), 0.0], [0.0, 0.0, 1.0]])
-        ry = np.array([[np.cos(b), 0.0, np.sin(b)], [0.0, 1.0, 0.0], [-np.sin(b), 0.0, np.cos(b)]])
-        return np.hstack([ry @ rz @ np.diag([1.3, 0.4, 0.8]), [[0.3], [1.1], [-0.4]]])
-    if kind == "mirrored":  # negative determinant
-        return np.hstack([np.diag([-0.7, 1.1, 0.9]) @ np.array([[0.0, 1.0, 0.0], [1.0, 0.0, 0.0], [0.0, 0.0, 1.0]]) @ np.diag([1, 1, -1]),
-                          [[-0.2], [0.5], [0.1]]])
-    raise ValueError(kind)
-
-
-def world_to_object(o2w):
-    """The 12 floats of the instance's world-to-object rows, as lrk_upload_scene stores them (rows of the inverse, in float)."""
-    m = np.vstack([o2w, [0.0, 0.0, 0.0, 1.0]])
-    return np.ascontiguousarray(np.linalg.inv(m)[:3].reshape(-1), f32)
-
-
-class Bottom:
-    def __init__(self, lib, tris, side, kind):
-        self.lib, self.tris, self.side, self.kind = lib, np.asarray(tris, np.float64), side, kind
-        flat = np.ascontiguousarray(self.tris.reshape(-1), np.float64)
-        self.h = lib.ltt_build(len(self.tris), flat.ctypes.data, side)
-        self.o2w = xform(kind)
-        self.w2o = world_to_object(self.o2w)
-        self.world = self.tris @ self.o2w[:, :3].T + self.o2w[:, 3]
-        self.n = len(self.tris)
-
-    def __del__(self):
-        self.lib.ltt_free(self.h)
-
-    def pmf(self, p, prim):
-        out = np.zeros(len(p), f32)
-        self.lib.ltt_pmf(self.h, len(p), p.ctypes.data, self.w2o.ctypes.data, prim, out.ctypes.data)
-        return out
-
-    def sample(self, p, u):
-        tri, pmf = np.zeros(len(p), np.uint32), np.zeros(len(p), f32)
-        u = np.ascontiguousarray(u, f32)
-        self.lib.ltt_sample(self.h, len(p), p.ctypes.data, self.w2o.ctypes.data, u.ctypes.data, tri.ctypes.data, pmf.ctypes.data)
-        return tri, pmf
-
-    def dead_mass(self, p):
-        out = np.zeros(len(p), np.float64)
-        self.lib.ltt_dead_mass(self.h, len(p), p.ctypes.data, self.w2o.ctypes.data, out.ctypes.data)
-        return out
-
-    def nodes_and_trails(self):
-        nodes = np.zeros(self.lib.ltt_node_count(self.h) * 48, np.uint8)
-        trails = np.zeros(self.n, np.uint64)
-        self.lib.ltt_copy(self.h, nodes.ctypes.data, trails.ctypes.data)
-        return nodes, trails
-
-    def bytes(self):
-        nodes, trails = self.nodes_and_trails()
-        return nodes.tobytes() + trails.tobytes()
-
-    def points(self, count, seed):
-        """World points: half inside the mesh's world bounds, half in a box three times their size around them."""
-        rng = np.random.default_rng(seed)
-        lo, hi = self.world.reshape(-1, 3).min(0), self.world.reshape(-1, 3).max(0)
-        c, e = 0.5 * (lo + hi), 0.5 * (hi - lo) + 1e-3
-        inside = rng.uniform(lo, hi, (count // 2, 3))
-        outside = rng.uniform(c - 3 * e, c + 3 * e, (count - count // 2, 3))
-        return np.ascontiguousarray(np.concatenate([inside, outside]), f32)
-
-    def facing(self, p, margin=1e-3):
-        """[points, triangles]: the world point lies in front of the triangle's emitting side by more than `margin` (relative to the
-        mesh's size), judged at the triangle's three vertices and centroid; always for two-sided, never for a degenerate triangle.
-        World-space normals are cross(p1 - p0, p2 - p0) of the world vertices, as the shade kernels take them."""
-        w = self.world
-        n = np.cross(w[:, 1] - w[:, 0], w[:, 2] - w[:, 0])
-        nl = np.linalg.norm(n, axis=1)
-        ok = nl > 1e-12 * max(1.0, float(np.abs(w).max())) ** 2
-        if self.side == TWO_SIDED:
-            return np.repeat(ok[None], len(p), axis=0)
-        n = n / np.where(ok, nl, 1.0)[:, None]
-        size = float(np.ptp(w.reshape(-1, 3), axis=0).max())
-        pts = np.concatenate([w, w.mean(axis=1, keepdims=True)], axis=1)  # [tri, 4, 3]
-        d = np.einsum("tc,ptkc->ptk", n, p.astype(np.float64)[:, None, None, :] - pts[None])
-        return (d > margin * size).any(axis=2) & ok[None]
+from light_sampling_checks import (MIRRORED, NONE, ONE_SIDED, TWO_SIDED, Bottom, LightSet, check_cli_flag, check_python_option,  # noqa: F401
+                                   f32, icosphere, lib, quad, single, soup)
 
 
 def cases():
@@ -146,7 +32,7 @@ def big(lib):
 
 
 def all_pmfs(b, p):
-    return np.stack([b.pmf(p, k) for k in range(b.n)], axis=1).astype(np.float64)  # [points, triangles]
+    return b.pmfs(p).T.astype(np.float64)  # [points, triangles]
 
 
 # ---- 1. the pmf is a distribution, and sampling returns it bit for bit ------------------------------------------------------------
@@ -303,7 +189,7 @@ def test_mirrored_cones_are_the_negated_one_sided_ones(lib):
 
 
 # ---- 5. the instance-level trees keep their bytes -------------------------------------------------------------------------------
-# SHA-256 of the nodes and trails of test_light_tree_cpu.LightSet(n, seed=n), taken at the commit before the triangle-level trees
+# SHA-256 of the nodes and trails of LightSet(n, seed=n), taken at the commit before the triangle-level trees
 PARENT_TOP_TREE_SHA256 = {
     1: "c1db4f2f46bd727f2872d1741e2a1e4f841f00e4754ccdce09be1869d1e88339",
     2: "eee2820fb4a1e8201741ebf6f54c7c49ce97a8393cdb54c2757a769564c343ce",
@@ -317,19 +203,16 @@ def test_instance_level_trees_keep_their_bytes(lib, n):
     assert hashlib.sha256(LightSet(n, seed=n).build(lib).bytes()).hexdigest() == PARENT_TOP_TREE_SHA256[n]
 
 
-# ---- 6. the option's surface ----------------------------------------------------------------------------------------------------
+# ---- 6. the option's surface ------------------------------------------------------------------------------------------------------
 def test_python_option_rejects_bad_values():
-    from luisarender_b200.api import Renderer
-
-    check_python_option_rejects_bad_values("light_tree_triangles", light_tree=True)
-    with pytest.raises(ValueError, match="light_tree=True"):
-        Renderer(light_tree_triangles=True)
+    check_python_option("light_tree_triangles")
 
 
 def test_cli_lists_and_parses_light_tree_triangles(tmp_path):
-    check_cli_lists_and_parses_flag("--light-tree-triangles", tmp_path)
+    check_cli_flag("light_tree_triangles", tmp_path)
 
 
+# ---- 7. the scene generator -------------------------------------------------------------------------------------------------------
 def test_emissive_globe_generator():
     from luisarender_b200 import scenes
 
