@@ -37,6 +37,13 @@ int grid_of(Kernel kernel, int block, int sm_count) {
     return (per_sm > 0 ? per_sm : 1) * sm_count;
 }
 
+// calls f(std::bool_constant<b>{}): the run-time flag as a compile-time one
+template<typename F>
+void with_flag(bool b, F &&f) {
+    if (b) f(std::true_type{});
+    else f(std::false_type{});
+}
+
 // calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection, light point sampling), or with the
 // kind's resampling instantiation (RESAMPLE; none for emitter-only hits).  The fast variant has none for the kinds that always run
 // in strict arithmetic (hit_kind_always_strict): render_pass never launches them there.
@@ -48,13 +55,6 @@ void with_shade_kernel(uint32_t kind, bool textured, F &&f) {
             textured ? f(shade_kernel<K, true, SEL, PT, RESAMPLE, RECEIVER>) : f(shade_kernel<K, false, SEL, PT, RESAMPLE, RECEIVER>);
     });
 }
-// the light sampling <SEL, PT> with or without the option "light_receiver"
-template<uint32_t SEL, uint32_t PT, typename F>
-void with_light_kernel(uint32_t kind, bool textured, bool receiver, F &&f) {
-    if (receiver) with_shade_kernel<SEL, PT, false, true>(kind, textured, f);
-    else with_shade_kernel<SEL, PT>(kind, textured, f);
-}
-
 // the volume integrator's surface step exists for the kinds of config C4's closures: emitter-only, Matte and Disney
 template<typename F>
 void with_volume_surface_kernel(uint32_t kind, bool textured, F &&f) {
@@ -80,22 +80,21 @@ int volume_surface_grid(uint32_t kind, int sm_count) {
     return g;
 }
 
-// the light sampling as the kernels' <SEL, PT>; the triangle-level trees need no instantiation of their own: the kernels find them
-// through light_tree_of(sc).bottom_nodes.  Resampling (candidates >= 2) has one instantiation per kind, which reads the selection,
-// the point sampling and the candidate count from light_tree_of(sc); emitter-only hits sample no light and keep theirs.
+// The light sampling as the kernels' <SEL, PT, RESAMPLE, RECEIVER>.  The triangle-level trees need no instantiation of their own: the
+// kernels find them through light_tree_of(sc).bottom_nodes.  Resampling (candidates >= 2) has one instantiation per kind, which reads
+// the selection, the point sampling and the candidate count from light_tree_of(sc); emitter-only hits sample no light and keep
+// theirs.  The receiver refines the tree, the solid-angle sampler and the resampling only: uniform area sampling keeps its kernel.
 void launch_shade(uint32_t kind, bool textured, const LightSampling &light, int blocks, cudaStream_t stream, const DeviceScene &sc,
                   const PathBuffers &pb, uint32_t depth) {
-    const auto launch = [&](auto kernel) { kernel<<<blocks, kShadeBlock, 0, stream>>>(sc, pb, depth); };
-    if (light.candidates >= 2u && kind != kHitEmitter) {
-        if (light.receiver) with_shade_kernel<kLightSelectUniform, kLightPointArea, true, true>(kind, textured, launch);
-        else with_shade_kernel<kLightSelectUniform, kLightPointArea, true>(kind, textured, launch);
-    } else if (light.solid_angle) {
-        if (light.tree) with_light_kernel<kLightSelectTree, kLightPointSolidAngle>(kind, textured, light.receiver, launch);
-        else with_light_kernel<kLightSelectUniform, kLightPointSolidAngle>(kind, textured, light.receiver, launch);
-    } else {
-        if (light.tree) with_light_kernel<kLightSelectTree, kLightPointArea>(kind, textured, light.receiver, launch);
-        else with_shade_kernel<kLightSelectUniform, kLightPointArea>(kind, textured, launch);
-    }
+    const bool resample = light.candidates >= 2u && kind != kHitEmitter;
+    const bool tree = light.tree && !resample, solid_angle = light.solid_angle && !resample;
+    const bool receiver = light.receiver && (resample || tree || solid_angle);
+    with_flag(resample, [&](auto r) { with_flag(tree, [&](auto t) { with_flag(solid_angle, [&](auto s) { with_flag(receiver, [&](auto v) {
+        constexpr bool RESAMPLE = decltype(r)::value, TREE = decltype(t)::value, SOLID_ANGLE = decltype(s)::value, RECEIVER = decltype(v)::value;
+        if constexpr (!(RESAMPLE && (TREE || SOLID_ANGLE)) && (!RECEIVER || RESAMPLE || TREE || SOLID_ANGLE))// the flags' combinations above
+            with_shade_kernel<TREE ? kLightSelectTree : kLightSelectUniform, SOLID_ANGLE ? kLightPointSolidAngle : kLightPointArea, RESAMPLE, RECEIVER>(
+                    kind, textured, [&](auto kernel) { kernel<<<blocks, kShadeBlock, 0, stream>>>(sc, pb, depth); });
+    }); }); }); });
 }
 
 void launch_volume_medium(int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth) {

@@ -39,63 +39,29 @@ __device__ __noinline__ inline BounceDraws draw_bounce_from_tables(SamplerRef sc
     return d;
 }
 
-// The light sampling of the resampling shade kernels, chosen at run time from light_tree_of(sc): one instantiation per TEXTURED
-// serves every (selection, point) pair, out of line so that the kernels hold one call site each.  `sc`: *DeviceScene::self.
-template<bool TEXTURED>
-__device__ __noinline__ LightSample sample_light_configured(const DeviceScene &sc, const Interaction &it, float u_sel, float u0, float u1) {
-    if (sc.light_count == 0u && sc.env_prob == 0.f) {
-        LightSample ls;
-        ls.eval.L = v3(0.f);
-        ls.eval.pdf = 0.f;
-        ls.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
-        ls.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
-        return ls;
-    }
+// The light sampling of the resampling shade kernels, chosen at run time from light_tree_of(sc): one instantiation per (TEXTURED,
+// RCV) serves every (selection, point) pair, out of line so that the kernels hold one call site each.  `sc`: *DeviceScene::self.
+// RCV: the kernels of the option "light_receiver", with `path`, the path's generation slot, where receiver_store left the vertex's
+// receiver word.
+template<bool TEXTURED, bool RCV>
+__device__ __noinline__ LightSample sample_light_configured(const DeviceScene &sc, const Interaction &it, float u_sel, float u0, float u1,
+                                                            uint32_t path) {
+    if (sc.light_count == 0u && sc.env_prob == 0.f) return no_light_sample();
     const DeviceLightTree &lt = light_tree_of(sc);
     if (lt.select == kLightSelectTree)
-        return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectTree, kLightPointSolidAngle>(sc, it, u_sel, u0, u1)
-                                                 : sample_light<TEXTURED, kLightSelectTree, kLightPointArea>(sc, it, u_sel, u0, u1);
-    return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectUniform, kLightPointSolidAngle>(sc, it, u_sel, u0, u1)
-                                             : sample_light<TEXTURED, kLightSelectUniform, kLightPointArea>(sc, it, u_sel, u0, u1);
+        return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectTree, kLightPointSolidAngle, RCV>(sc, it, u_sel, u0, u1, path)
+                                                 : sample_light<TEXTURED, kLightSelectTree, kLightPointArea, RCV>(sc, it, u_sel, u0, u1, path);
+    return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectUniform, kLightPointSolidAngle, RCV>(sc, it, u_sel, u0, u1, path)
+                                             : sample_light<TEXTURED, kLightSelectUniform, kLightPointArea, RCV>(sc, it, u_sel, u0, u1, path);
 }
-template<bool TEXTURED>
-__device__ __noinline__ LightEval evaluate_hit_configured(const DeviceScene &sc, const Interaction &it, V3 p_from, uint32_t inst) {
+template<bool TEXTURED, bool RCV>
+__device__ __noinline__ LightEval evaluate_hit_configured(const DeviceScene &sc, const Interaction &it, V3 p_from, uint32_t inst, uint32_t path) {
     const DeviceLightTree &lt = light_tree_of(sc);
     if (lt.select == kLightSelectTree)
-        return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectTree, kLightPointSolidAngle>(sc, it, p_from, inst)
-                                                 : evaluate_hit<TEXTURED, kLightSelectTree, kLightPointArea>(sc, it, p_from, inst);
-    return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointSolidAngle>(sc, it, p_from, inst)
-                                             : evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointArea>(sc, it, p_from, inst);
-}
-
-// The same for the resampling kernels of the option "light_receiver": `path`, the path's generation slot, where receiver_store left
-// the vertex's receiver word.
-template<bool TEXTURED>
-__device__ __noinline__ LightSample sample_light_configured_receiver(const DeviceScene &sc, const Interaction &it, float u_sel, float u0, float u1,
-                                                                     uint32_t path) {
-    if (sc.light_count == 0u && sc.env_prob == 0.f) {
-        LightSample ls;
-        ls.eval.L = v3(0.f);
-        ls.eval.pdf = 0.f;
-        ls.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
-        ls.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
-        return ls;
-    }
-    const DeviceLightTree &lt = light_tree_of(sc);
-    if (lt.select == kLightSelectTree)
-        return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectTree, kLightPointSolidAngle, true>(sc, it, u_sel, u0, u1, path)
-                                                 : sample_light<TEXTURED, kLightSelectTree, kLightPointArea, true>(sc, it, u_sel, u0, u1, path);
-    return lt.point == kLightPointSolidAngle ? sample_light<TEXTURED, kLightSelectUniform, kLightPointSolidAngle, true>(sc, it, u_sel, u0, u1, path)
-                                             : sample_light<TEXTURED, kLightSelectUniform, kLightPointArea>(sc, it, u_sel, u0, u1);
-}
-template<bool TEXTURED>
-__device__ __noinline__ LightEval evaluate_hit_configured_receiver(const DeviceScene &sc, const Interaction &it, V3 p_from, uint32_t inst, uint32_t path) {
-    const DeviceLightTree &lt = light_tree_of(sc);
-    if (lt.select == kLightSelectTree)
-        return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectTree, kLightPointSolidAngle, true>(sc, it, p_from, inst, path)
-                                                 : evaluate_hit<TEXTURED, kLightSelectTree, kLightPointArea, true>(sc, it, p_from, inst, path);
-    return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointSolidAngle, true>(sc, it, p_from, inst, path)
-                                             : evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointArea>(sc, it, p_from, inst);
+        return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectTree, kLightPointSolidAngle, RCV>(sc, it, p_from, inst, path)
+                                                 : evaluate_hit<TEXTURED, kLightSelectTree, kLightPointArea, RCV>(sc, it, p_from, inst, path);
+    return lt.point == kLightPointSolidAngle ? evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointSolidAngle, RCV>(sc, it, p_from, inst, path)
+                                             : evaluate_hit<TEXTURED, kLightSelectUniform, kLightPointArea, RCV>(sc, it, p_from, inst, path);
 }
 
 // The receiver word of a surface vertex (option "light_receiver", receiver.h): its geometric normal on the side wo leaves from, with
@@ -117,7 +83,6 @@ template<uint32_t KIND, bool TEXTURED = false, uint32_t SEL = kLightSelectUnifor
 __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kernel(DeviceScene sc, PathBuffers pb, uint32_t depth) {
     static_assert(!RESAMPLE || (KIND != kHitEmitter && SEL == kLightSelectUniform && PT == kLightPointArea), "one resampling kernel per kind");
     static_assert(!RECEIVER || RESAMPLE || SEL == kLightSelectTree || PT == kLightPointSolidAngle, "the receiver refines the tree or solid angle");
-    constexpr bool kReceiver = RECEIVER;
     // the compaction is written out here rather than through block_append, which raises registers or spills of most instantiations
     __shared__ uint32_t s_warp_next[kShadeBlock / 32], s_warp_shadow[kShadeBlock / 32];
     __shared__ uint32_t s_base_next, s_base_shadow;
@@ -147,10 +112,8 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                 if (sc.light_count != 0u && it.shape.has_light()) {
                     LightEval e;
                     const uint32_t path = depth != 0u ? ir.x : kNoReceiverPath;// the receiver word of the vertex the ray left
-                    if constexpr (RESAMPLE && kReceiver) e = evaluate_hit_configured_receiver<TEXTURED>(*sc.self, it, v3(ro.x, ro.y, ro.z), hit.x, path);
-                    else if constexpr (RESAMPLE) e = evaluate_hit_configured<TEXTURED>(*sc.self, it, v3(ro.x, ro.y, ro.z), hit.x);
-                    else if constexpr (kReceiver) e = evaluate_hit<TEXTURED, SEL, PT, true>(sc, it, v3(ro.x, ro.y, ro.z), hit.x, path);
-                    else e = evaluate_hit<TEXTURED, SEL, PT>(sc, it, v3(ro.x, ro.y, ro.z), hit.x);
+                    if constexpr (RESAMPLE) e = evaluate_hit_configured<TEXTURED, RECEIVER>(*sc.self, it, v3(ro.x, ro.y, ro.z), hit.x, path);
+                    else e = evaluate_hit<TEXTURED, SEL, PT, RECEIVER>(sc, it, v3(ro.x, ro.y, ro.z), hit.x, path);
                     V3 add = beta * e.L * balance_heuristic(pdf_bsdf, e.pdf);
                     float4 li = pb.li[ir.x];
                     li.x += add.x;
@@ -175,18 +138,11 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                         u_sel = dr.u_sel; ul0 = dr.ul0; ul1 = dr.ul1; u_lobe = dr.u_lobe; ub0 = dr.ub0; ub1 = dr.ub1; u_rr = dr.u_rr;
                         state = dr.state;
                     }
-                    LightSample ls;// with RESAMPLE: the kept candidate's shadow ray only
-                    ls.eval.L = v3(0.f);
-                    ls.eval.pdf = 0.f;
-                    ls.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
-                    ls.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
-                    if constexpr (kReceiver) {// the word goes to memory here; the light sampling reads it back through the path's slot
+                    LightSample ls = no_light_sample();// with RESAMPLE: the kept candidate's shadow ray only
+                    if constexpr (RECEIVER)// the word goes to memory here; the light sampling reads it back through the path's slot
                         if (light_tree_of(sc).receiver != nullptr) receiver_store(*sc.self, ir.x, it.ng, wo, hit_kind_one_sided(KIND));
-                        if constexpr (!RESAMPLE)
-                            if (sc.light_count != 0u || sc.env_prob != 0.f) ls = sample_light<TEXTURED, SEL, PT, true>(sc, it, u_sel, ul0, ul1, ir.x);
-                    } else if constexpr (!RESAMPLE) {
-                        if (sc.light_count != 0u || sc.env_prob != 0.f) ls = sample_light<TEXTURED, SEL, PT>(sc, it, u_sel, ul0, ul1);
-                    }
+                    if constexpr (!RESAMPLE)
+                        if (sc.light_count != 0u || sc.env_prob != 0.f) ls = sample_light<TEXTURED, SEL, PT, RECEIVER>(sc, it, u_sel, ul0, ul1, ir.x);
                     const lrk_surface *surf = sc.surfaces + it.shape.surface_tag;
                     V3 contrib, wi, f;
                     float pdf;
@@ -194,8 +150,7 @@ __global__ void __launch_bounds__(kShadeBlock, LRK_SHADE_MIN_BLOCKS) shade_kerne
                                                                            [&](auto &cl, const Frame &fr) {
                         if constexpr (RESAMPLE) {
                             const auto draw_light = [&](float us, float u0, float u1) {
-                                if constexpr (kReceiver) return sample_light_configured_receiver<TEXTURED>(*sc.self, it, us, u0, u1, ir.x);
-                                else return sample_light_configured<TEXTURED>(*sc.self, it, us, u0, u1);
+                                return sample_light_configured<TEXTURED, RECEIVER>(*sc.self, it, us, u0, u1, ir.x);
                             };
                             shade_surface_resampled(cl, it, fr, wo, draw_light, light_tree_of(sc).candidates, depth, u_sel, ul0, ul1, beta, u_lobe, ub0, ub1,
                                                     contrib, ls.ray_o_tmin, ls.ray_d_tmax, wi, f, pdf);

@@ -246,39 +246,32 @@ __device__ __forceinline__ LightEval diffuse_light_evaluate(const DeviceScene &s
 // of the option "light_tree" over the emissive instances (light_tree.h)
 enum LightSelect : uint32_t { kLightSelectUniform = 0u, kLightSelectTree = 1u };
 
-__device__ __noinline__ inline uint32_t light_tree_sample(const LightTreeNode *nodes, V3 p, float u, float &pmf, float &u_left) {
-    return light_tree_walk<true>(nodes, p.x, p.y, p.z, u, 0ull, pmf, &u_left);
-}
-__device__ __noinline__ inline float light_tree_pmf(const LightTreeNode *nodes, const uint32_t *inst_light, const unsigned long long *trail, V3 p,
-                                                    uint32_t inst) {
-    const uint32_t l = __ldg(inst_light + inst);
-    if (l == kLightTreeNone) return 0.f;// an emitter without power
-    float pmf;
-    light_tree_walk<false>(nodes, p.x, p.y, p.z, 0.f, __ldg(trail + l), pmf);
-    return pmf;
-}
-
 // The receiver word (option "light_receiver", receiver.h) of the vertex that path `path` (its generation slot, id_rng.x) last left:
-// 0 without the option, and for kNoReceiverPath (a camera ray).  The callees below read it themselves, out of line, so that the
-// shade kernels hold nothing for it but the path's slot, which they hold anyway.
+// 0 without the option, and for kNoReceiverPath (a camera ray).  The light functions below read it themselves, out of line, so that
+// the shade kernels hold nothing for it but the path's slot, which they hold anyway.  RCV: the instantiation of the option
+// "light_receiver"; the others read no word and take the constant 0, which leaves them the expressions without the option.
 constexpr uint32_t kNoReceiverPath = 0xffffffffu;
+template<bool RCV>
 __device__ __forceinline__ uint32_t receiver_word_of(const DeviceScene &sc, uint32_t path) {
+    if (!RCV) return 0u;
     const uint32_t *words = light_tree_of(sc).receiver;
     return words != nullptr && path != kNoReceiverPath ? words[path] : 0u;
 }
 
 // The descents of the light tree, out of line so that the shade kernels' register allocation does not grow with them.  `path`: as
 // receiver_word_of, whose word is decoded here for both the sample and the pmf.
-__device__ __noinline__ inline uint32_t light_tree_sample_receiver(const DeviceScene &sc, const LightTreeNode *nodes, V3 p, float u, float &pmf, float &u_left,
+template<bool RCV>
+__device__ __noinline__ inline uint32_t light_tree_sample(const DeviceScene &sc, const LightTreeNode *nodes, V3 p, float u, float &pmf, float &u_left,
                                                           uint32_t path) {
-    return light_tree_walk<true>(nodes, p.x, p.y, p.z, u, 0ull, pmf, &u_left, receiver_decode(receiver_word_of(sc, path)));
+    return light_tree_walk<true>(nodes, p.x, p.y, p.z, u, 0ull, pmf, &u_left, receiver_decode(receiver_word_of<RCV>(sc, path)));
 }
-__device__ __noinline__ inline float light_tree_pmf_receiver(const DeviceScene &sc, const LightTreeNode *nodes, const uint32_t *inst_light,
+template<bool RCV>
+__device__ __noinline__ inline float light_tree_pmf(const DeviceScene &sc, const LightTreeNode *nodes, const uint32_t *inst_light,
                                                     const unsigned long long *trail, V3 p, uint32_t inst, uint32_t path) {
     const uint32_t l = __ldg(inst_light + inst);
     if (l == kLightTreeNone) return 0.f;// an emitter without power
     float pmf;
-    light_tree_walk<false>(nodes, p.x, p.y, p.z, 0.f, __ldg(trail + l), pmf, nullptr, receiver_decode(receiver_word_of(sc, path)));
+    light_tree_walk<false>(nodes, p.x, p.y, p.z, 0.f, __ldg(trail + l), pmf, nullptr, receiver_decode(receiver_word_of<RCV>(sc, path)));
     return pmf;
 }
 
@@ -293,44 +286,32 @@ __device__ __forceinline__ V3 light_tree_to_object(const DeviceScene &sc, uint32
     light_tree_object_point(w2o, p.x, p.y, p.z, q.x, q.y, q.z);
     return q;
 }
-__device__ __noinline__ inline uint32_t light_tree_sample_triangle(const DeviceScene &sc, uint32_t inst, V3 p, float u, float &pmf) {
-    const DeviceLightTree &lt = light_tree_of(sc);
-    const uint32_t root = __ldg(lt.inst_bottom + inst).x;
-    pmf = 0.f;
-    if (root == kLightTreeNone) return kLightTreeNone;
-    const V3 q = light_tree_to_object(sc, inst, p);
-    return light_tree_walk<true>(lt.bottom_nodes + root, q.x, q.y, q.z, u, 0ull, pmf);
-}
-__device__ __noinline__ inline float light_tree_triangle_pmf(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p) {
-    const DeviceLightTree &lt = light_tree_of(sc);
-    const uint2 b = __ldg(lt.inst_bottom + inst);
-    if (b.x == kLightTreeNone) return 0.f;
-    const V3 q = light_tree_to_object(sc, inst, p);
-    return light_tree_triangle_pmf_at(lt.bottom_nodes + b.x, q.x, q.y, q.z, __ldg(lt.bottom_trail + b.y + prim), prim);
-}
 // the receiver word decoded and mapped to the object space of instance inst (receiver_to_object: the transpose of object-to-world)
+template<bool RCV>
 __device__ __forceinline__ Receiver light_tree_object_receiver(const DeviceScene &sc, uint32_t inst, uint32_t path) {
-    const Receiver r = receiver_decode(receiver_word_of(sc, path));
+    const Receiver r = receiver_decode(receiver_word_of<RCV>(sc, path));
     if (r.kind == kReceiverNone) return r;
     const Mat34 m = load_o2w(sc, inst);
     const float o2w[9] = {m.r0.x, m.r0.y, m.r0.z, m.r1.x, m.r1.y, m.r1.z, m.r2.x, m.r2.y, m.r2.z};
     return receiver_to_object(o2w, r);
 }
-__device__ __noinline__ inline uint32_t light_tree_sample_triangle_receiver(const DeviceScene &sc, uint32_t inst, V3 p, float u, float &pmf, uint32_t path) {
+template<bool RCV>
+__device__ __noinline__ inline uint32_t light_tree_sample_triangle(const DeviceScene &sc, uint32_t inst, V3 p, float u, float &pmf, uint32_t path) {
     const DeviceLightTree &lt = light_tree_of(sc);
     const uint32_t root = __ldg(lt.inst_bottom + inst).x;
     pmf = 0.f;
     if (root == kLightTreeNone) return kLightTreeNone;
     const V3 q = light_tree_to_object(sc, inst, p);
-    return light_tree_walk<true>(lt.bottom_nodes + root, q.x, q.y, q.z, u, 0ull, pmf, nullptr, light_tree_object_receiver(sc, inst, path));
+    return light_tree_walk<true>(lt.bottom_nodes + root, q.x, q.y, q.z, u, 0ull, pmf, nullptr, light_tree_object_receiver<RCV>(sc, inst, path));
 }
-__device__ __noinline__ inline float light_tree_triangle_pmf_receiver(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p, uint32_t path) {
+template<bool RCV>
+__device__ __noinline__ inline float light_tree_triangle_pmf(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p, uint32_t path) {
     const DeviceLightTree &lt = light_tree_of(sc);
     const uint2 b = __ldg(lt.inst_bottom + inst);
     if (b.x == kLightTreeNone) return 0.f;
     const V3 q = light_tree_to_object(sc, inst, p);
     return light_tree_triangle_pmf_at(lt.bottom_nodes + b.x, q.x, q.y, q.z, __ldg(lt.bottom_trail + b.y + prim), prim,
-                                      light_tree_object_receiver(sc, inst, path));
+                                      light_tree_object_receiver<RCV>(sc, inst, path));
 }
 
 // Point sampling of next-event estimation: the reference's area sampling of the chosen triangle, or, with the option
@@ -357,22 +338,16 @@ __device__ __noinline__ inline float light_triangle_solid_angle(const DeviceScen
     light_triangle_world(sc, inst, prim, v0, v1, v2);
     return solid_angle({p.x, p.y, p.z}, v0, v1, v2);
 }
-__device__ __noinline__ inline V3 light_triangle_sample_spherical(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p, float omega, float u0,
-                                                                  float u1) {
-    SphVec v0, v1, v2;
-    light_triangle_world(sc, inst, prim, v0, v1, v2);
-    const SphVec b = sample_spherical_triangle({p.x, p.y, p.z}, v0, v1, v2, omega, u0, u1);
-    return v3(b.x, b.y, b.z);
-}
 // `path`: as receiver_word_of; where its word is not 0 (option "light_receiver"), (u0, u1) go through the receiver-cosine warp first,
-// and `warp` receives the warp's pdf factor (spherical_warp_pdf) at the point made, taken with the expression of make_interaction's
-// pg (hit_position), which is the point an emitter hit evaluates it at; else 1.
-__device__ __noinline__ inline V3 light_triangle_sample_spherical_receiver(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p, float omega,
-                                                                           float u0, float u1, uint32_t path, float &warp) {
+// and `*warp` receives the warp's pdf factor (spherical_warp_pdf) at the point made, taken with the expression of make_interaction's
+// pg (hit_position), which is the point an emitter hit evaluates it at; else 1.  `warp` is written by the RCV instantiation only.
+template<bool RCV>
+__device__ __noinline__ inline V3 light_triangle_sample_spherical(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p, float omega, float u0,
+                                                                  float u1, uint32_t path, float *warp) {
     SphVec v0, v1, v2;
     light_triangle_world(sc, inst, prim, v0, v1, v2);
-    const Receiver r = receiver_decode(receiver_word_of(sc, path));
-    warp = 1.f;
+    const Receiver r = receiver_decode(receiver_word_of<RCV>(sc, path));
+    if (RCV) *warp = 1.f;
     if (r.kind == kReceiverNone) {
         const SphVec b = sample_spherical_triangle({p.x, p.y, p.z}, v0, v1, v2, omega, u0, u1);
         return v3(b.x, b.y, b.z);
@@ -381,14 +356,14 @@ __device__ __noinline__ inline V3 light_triangle_sample_spherical_receiver(const
     sample_bilinear(spherical_warp_weights(pp, n, v0, v1, v2), u0, u1);
     const SphVec b = sample_spherical_triangle(pp, v0, v1, v2, omega, u0, u1);
     const V3 x = hit_position(sc, inst, prim, v3(b.x, b.y, b.z));
-    warp = spherical_warp_pdf(pp, n, v0, v1, v2, omega, {x.x, x.y, x.z});
+    *warp = spherical_warp_pdf(pp, n, v0, v1, v2, omega, {x.x, x.y, x.z});
     return v3(b.x, b.y, b.z);
 }
 // the warp's factor of the pdf of point x (spherical_warp_pdf) for the receiver word of `path`; 1 for the word 0.  The emitter hit's
 // half of the one pdf: light_triangle_sample_spherical computes the sample's with the same function at the point it made.
 __device__ __noinline__ inline float light_triangle_warp_pdf(const DeviceScene &sc, uint32_t inst, uint32_t prim, V3 p, uint32_t path, float omega,
                                                              V3 x) {
-    const Receiver r = receiver_decode(receiver_word_of(sc, path));
+    const Receiver r = receiver_decode(receiver_word_of<true>(sc, path));
     if (r.kind == kReceiverNone) return 1.f;
     SphVec v0, v1, v2;
     light_triangle_world(sc, inst, prim, v0, v1, v2);
@@ -398,7 +373,7 @@ __device__ __noinline__ inline float light_triangle_warp_pdf(const DeviceScene &
 // spherical sampler serves the triangle there, else area_pdf, the reference's area pdf in solid angle (diffuse_light_evaluate;
 // 0 for a point that emits nothing there, which stays 0; triangle_selected as in diffuse_light_evaluate: 1 / omega).  With the
 // option "light_receiver", the pdf of the point is this times the warp's factor (spherical_warp_pdf at the point): an emitter hit takes
-// it from light_triangle_warp_pdf, a light sample from light_triangle_sample_spherical_receiver, both through the one function.
+// it from light_triangle_warp_pdf, a light sample from light_triangle_sample_spherical, both through the one function.
 __device__ __forceinline__ float light_point_pdf(const DeviceScene &sc, const Interaction &it_light, float area_pdf, float omega,
                                                  bool triangle_selected = false) {
     if (area_pdf == 0.f || !use_spherical(omega)) return area_pdf;
@@ -417,19 +392,12 @@ __device__ __forceinline__ LightEval evaluate_hit(const DeviceScene &sc, const I
     if (PT == kLightPointSolidAngle && e.pdf != 0.f) {
         const float omega = light_triangle_solid_angle(*sc.self, inst, it.prim, p_from);
         e.pdf = light_point_pdf(sc, it, e.pdf, omega, tri_sel);
-        if constexpr (RCV)
-            if (e.pdf != 0.f && use_spherical(omega)) e.pdf *= light_triangle_warp_pdf(*sc.self, inst, it.prim, p_from, path, omega, it.pg);
+        if (RCV && e.pdf != 0.f && use_spherical(omega)) e.pdf *= light_triangle_warp_pdf(*sc.self, inst, it.prim, p_from, path, omega, it.pg);
     }
     if (SEL == kLightSelectTree) {
         const DeviceLightTree &lt = light_tree_of(sc);
-        float pmf;
-        if constexpr (RCV) {
-            pmf = light_tree_pmf_receiver(*sc.self, lt.nodes, lt.inst_light, lt.trail, p_from, inst, path);
-            if (tri_sel && pmf != 0.f) pmf *= light_tree_triangle_pmf_receiver(*sc.self, inst, it.prim, p_from, path);
-        } else {
-            pmf = light_tree_pmf(lt.nodes, lt.inst_light, lt.trail, p_from, inst);
-            if (tri_sel && pmf != 0.f) pmf *= light_tree_triangle_pmf(*sc.self, inst, it.prim, p_from);
-        }
+        float pmf = light_tree_pmf<RCV>(*sc.self, lt.nodes, lt.inst_light, lt.trail, p_from, inst, path);
+        if (tri_sel && pmf != 0.f) pmf *= light_tree_triangle_pmf<RCV>(*sc.self, inst, it.prim, p_from, path);
         e.pdf *= (1.f - sc.env_prob) * pmf;
         return e;
     }
@@ -446,6 +414,15 @@ struct LightSample {
     LightEval eval;
     float4 ray_o_tmin, ray_d_tmax;
 };
+// the light sample of no light: no radiance, pdf 0 and an empty shadow ray
+__device__ __forceinline__ LightSample no_light_sample() {
+    LightSample s;
+    s.eval.L = v3(0.f);
+    s.eval.pdf = 0.f;
+    s.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
+    s.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
+    return s;
+}
 
 // `p_shading`: it_from.p_shading(), the point the light's emission and pdf are evaluated from (diffuse.cpp:62-86) - the hit point
 // for a surface interaction, but the WORLD ORIGIN for the volume integrator's Interaction{ray->origin()}, whose shading point is
@@ -475,25 +452,16 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
             const DeviceLightTree &lt = light_tree_of(sc);
             const LightTreeNode *nodes = lt.nodes;
             float pmf = 0.f, u_left = 0.f;
-            uint32_t l = kLightTreeNone;
-            if constexpr (RCV) l = nodes != nullptr ? light_tree_sample_receiver(*sc.self, nodes, it_from.pg, uu, pmf, u_left, path) : kLightTreeNone;
-            else l = nodes != nullptr ? light_tree_sample(nodes, it_from.pg, uu, pmf, u_left) : kLightTreeNone;
+            uint32_t l = nodes != nullptr ? light_tree_sample<RCV>(*sc.self, nodes, it_from.pg, uu, pmf, u_left, path) : kLightTreeNone;
             if (l != kLightTreeNone) tag = __ldg(lt.light_inst + l);// the instance itself
             tri_sel = lt.bottom_nodes != nullptr;
             if (tri_sel && l != kLightTreeNone) {// one selection number for the whole descent: the top walk's u continues
                 float tri_pmf;
-                if constexpr (RCV) tree_tri = light_tree_sample_triangle_receiver(*sc.self, tag, it_from.pg, u_left, tri_pmf, path);
-                else tree_tri = light_tree_sample_triangle(*sc.self, tag, it_from.pg, u_left, tri_pmf);
+                tree_tri = light_tree_sample_triangle<RCV>(*sc.self, tag, it_from.pg, u_left, tri_pmf, path);
                 if (tree_tri == kLightTreeNone) l = kLightTreeNone;
                 pmf *= tri_pmf;
             }
-            if (l == kLightTreeNone) {// no emitter can reach the point: nothing to trace
-                s.eval.L = v3(0.f);
-                s.eval.pdf = 0.f;
-                s.ray_o_tmin = make_float4(0.f, 0.f, 0.f, 0.f);
-                s.ray_d_tmax = make_float4(0.f, 0.f, 1.f, 0.f);
-                return s;
-            }
+            if (l == kLightTreeNone) return no_light_sample();// no emitter can reach the point: nothing to trace
             sel_prob = ep == 0.f ? pmf : (1.f - ep) * pmf;
         }
     } else if (ep == 0.f) {
@@ -537,21 +505,16 @@ __device__ __forceinline__ LightSample sample_light_from(const DeviceScene &sc, 
     float omega = 0.f, warp = 1.f;
     if (PT == kLightPointSolidAngle) {// the same two numbers drive either sampler
         omega = light_triangle_solid_angle(*sc.self, handle.instance_id, triangle_id, p_shading);
-        if constexpr (RCV)
-            uvw = use_spherical(omega) ? light_triangle_sample_spherical_receiver(*sc.self, handle.instance_id, triangle_id, p_shading, omega, ux, u1,
-                                                                                  path, warp)
-                                       : sample_uniform_triangle(ux, u1);
-        else
-            uvw = use_spherical(omega) ? light_triangle_sample_spherical(*sc.self, handle.instance_id, triangle_id, p_shading, omega, ux, u1)
-                                       : sample_uniform_triangle(ux, u1);
+        uvw = use_spherical(omega) ? light_triangle_sample_spherical<RCV>(*sc.self, handle.instance_id, triangle_id, p_shading, omega, ux, u1, path,
+                                                                          RCV ? &warp : nullptr)
+                                   : sample_uniform_triangle(ux, u1);
     } else {
         uvw = sample_uniform_triangle(ux, u1);
     }
     Interaction it_light = make_interaction(sc, handle.instance_id, triangle_id, uvw);
     it_light.back_facing = dot(it_light.ng, it_from.pg - it_light.pg) < 0.f;
     s.eval = diffuse_light_evaluate<TEX>(sc, it_light, p_shading, tri_sel);
-    if (PT == kLightPointSolidAngle) s.eval.pdf = RCV ? light_point_pdf(sc, it_light, s.eval.pdf, omega, tri_sel) * warp
-                                                                  : light_point_pdf(sc, it_light, s.eval.pdf, omega, tri_sel);
+    if (PT == kLightPointSolidAngle) s.eval.pdf = light_point_pdf(sc, it_light, s.eval.pdf, omega, tri_sel) * warp;
     s.eval.pdf *= sel_prob;
     // Interaction::spawn_ray_to, src/base/interaction.cpp:25-30
     V3 p_from = p_robust(it_from, it_light.pg - it_from.pg);
