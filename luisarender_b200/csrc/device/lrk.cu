@@ -76,11 +76,21 @@ struct DeviceArrays {
         lt_bottom_trail, update_staging, mesh_staging, mesh_refit, refit_starts, refit_scratch, refit_visits, node_runs;
 };
 
-enum KernelCategory { CAT_TRACE_CLOSEST = 0, CAT_TRACE_SHADOW = 1, CAT_SHADE = 2, CAT_OTHER = 3, CAT_COUNT = 4 };
+// CAT_NONE: counted in stats.kernel_launches, never timed
+enum KernelCategory { CAT_NONE = -1, CAT_TRACE_CLOSEST = 0, CAT_TRACE_SHADOW = 1, CAT_SHADE = 2, CAT_OTHER = 3 };
 
 struct TimedLaunch {
     int cat;
     cudaEvent_t start, stop;
+};
+
+// The persistent grid of every kernel that a pass launches over a path queue (blocks_for caps the launch there): resident blocks per
+// SM x SM count, measured by measure_grids at lrk_create so that no occupancy query runs inside a timed render.  Each grid is
+// measured on the kernel's untextured, uniform/area, non-counting, non-alpha instantiation and launches all of its instantiations.
+// [v]: 0 = fast, 1 = strict arithmetic (shade.cu).
+struct Grids {
+    int closest, query, shadow, classify, miss, shade[2][kHitKinds];
+    int medium_shadow, volume_medium[2], volume_surface[2][3], volume_nee;
 };
 
 // The host state of the uploaded scene that the scene updates (lrk_update_*, lrk_replace_meshes) read and keep, set whole by
@@ -147,15 +157,13 @@ struct lrk_ctx {
     cudaEvent_t ev_begin{}, ev_end{};
     std::vector<TimedLaunch> timed;
     std::vector<cudaEvent_t> event_pool;
-    int grid_trace{0}, grid_shade[2][kHitKinds]{}, grid_shadow{0}, grid_classify{0};// grid_shade[variant]: 0 = fast, 1 = strict arithmetic
+    Grids grids{};
     uint32_t used_kinds{1u};     // bit k: an instance of the scene has hit kind k (bit 0 always: emitter-only hits of an image emission)
     uint32_t allocated_kinds{0u};// bit k: hit_index[k] is allocated
     bool volume{false};
     bool strict_math{false};// option strict_math: every closure kernel from shade.cu's IEEE-arithmetic compilation
     bool volume_general{false};// the volume integrator's per-thread kernel (volume_general.cuh) instead of the wavefront one
-    int grid_vgeneral{0};
     uint64_t volume_capacity{0};
-    int grid_vshade[2][3]{}, grid_vmedium[2]{0, 0}, grid_vshadow{0};
     // adaptive mode (lrk_render_adaptive); the device buffers are allocated on its first call
     std::vector<uint32_t> block_start;// offsets of the 8x4 pixel blocks in the pixel list, closed by npix_owned (build_pixel_list)
     float2 *pass_moments{nullptr};// set while lrk_render_adaptive runs: the film accumulation also adds the luminance moments here
@@ -343,75 +351,86 @@ cudaEvent_t take_event(lrk_ctx *ctx) {
     return e;
 }
 
-struct ScopedTimer {
-    lrk_ctx *ctx;
-    TimedLaunch t{};
-    bool on;
-    ScopedTimer(lrk_ctx *c, int cat) : ctx{c}, on{c->time_kernels} {
-        if (on) {
-            t.cat = cat;
-            t.start = take_event(ctx);
-            t.stop = take_event(ctx);
-            cudaEventRecord(t.start, ctx->stream);
+// A stage of a pass: launches its kernels on ctx->stream and counts each in stats.kernel_launches (stats.kernel_launches counts the
+// kernels of lrk_render and lrk_render_adaptive: a cub call there counts itself as one).  With the option time_kernels a stage with
+// a category is one timed interval, the gaps between its kernels included.  A stage of one launch can be a temporary:
+// Stage(ctx, CAT_OTHER).launch(...) records its end after the launch.
+class Stage {
+public:
+    Stage(lrk_ctx *ctx, int cat) : ctx_{ctx}, on_{cat != CAT_NONE && ctx->time_kernels} {
+        if (on_) {
+            t_.cat = cat;
+            t_.start = take_event(ctx_);
+            t_.stop = take_event(ctx_);
+            cudaEventRecord(t_.start, ctx_->stream);
         }
     }
-    ~ScopedTimer() {
-        if (on) {
-            cudaEventRecord(t.stop, ctx->stream);
-            ctx->timed.push_back(t);
+    ~Stage() {
+        if (on_) {
+            cudaEventRecord(t_.stop, ctx_->stream);
+            ctx_->timed.push_back(t_);
         }
     }
+    template<typename... Params, typename... Args>
+    void launch(void (*kernel)(Params...), unsigned blocks, int block, Args &&...args) {
+        kernel<<<blocks, block, 0, ctx_->stream>>>(std::forward<Args>(args)...);
+        ctx_->stats.kernel_launches++;
+    }
+
+private:
+    lrk_ctx *ctx_;
+    bool on_;
+    TimedLaunch t_{};
 };
 
-int blocks_for(lrk_ctx *ctx, uint64_t n, int persistent_grid) {
+int blocks_for(lrk_ctx *ctx, uint64_t n, int grid) {
     uint64_t need = (n + kBlock - 1u) / kBlock;
-    return static_cast<int>(std::max<uint64_t>(1u, std::min<uint64_t>(need, static_cast<uint64_t>(persistent_grid))));
+    return static_cast<int>(std::max<uint64_t>(1u, std::min<uint64_t>(need, static_cast<uint64_t>(grid))));
 }
 
-// Every traversal kernel family is launched from one place, which also picks its instantiation: traversal counters (option
-// count_traversal) or any-hit queries x the stochastic alpha test (scenes with non-opaque surfaces).  The kernels are named directly
-// rather than through a generic lambda, so that they are instantiated in source order and the cubin's function order stays put.
-void launch_query(lrk_ctx *ctx, int g, bool any_hit, const float4 *d_rays, uint4 *d_hits, uint32_t n) {
-    const auto kernel = ctx->any_non_opaque ? (any_hit ? trace_query_kernel<true, true> : trace_query_kernel<false, true>)
-                                            : (any_hit ? trace_query_kernel<true, false> : trace_query_kernel<false, false>);
-    kernel<<<g, kTraceBlock, 0, ctx->stream>>>(ctx->scene, d_rays, d_hits, n, ctx->d_query_cursor.get<uint32_t>());
+// The instantiation of every kernel template that lrk.cu launches, picked from the context's flags: any-hit queries, traversal
+// counters (option count_traversal), the stochastic alpha test (scenes with non-opaque surfaces) and the film accumulation's
+// luminance moments (adaptive renders, G-buffer films).  The kernels are named directly rather than through a generic lambda, so
+// that they are instantiated in source order and the cubin's function order stays put.
+auto query_kernel(const lrk_ctx *ctx, bool any_hit) {
+    return ctx->any_non_opaque ? (any_hit ? trace_query_kernel<true, true> : trace_query_kernel<false, true>)
+                               : (any_hit ? trace_query_kernel<true, false> : trace_query_kernel<false, false>);
 }
-
-// stats.kernel_launches counts the kernels of lrk_render and lrk_render_adaptive (a cub call counts as one): each launch there adds
-// itself where it is issued.
-
-// The film accumulation of a pass; with the adaptive mode's moments while lrk_render_adaptive runs.
-void launch_accumulate(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp) {
-    ScopedTimer t{ctx, CAT_OTHER};
-    const auto kernel = ctx->pass_moments != nullptr ? accumulate_kernel<true> : accumulate_kernel<false>;
-    kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->scene, ctx->pb.li, ctx->d_film.get<float4>(), pixel_list, pixel_offset, npix, spp,
-                                                                    ctx->pb.counts, ctx->pb.stats, ctx->pass_moments);
-    ctx->stats.kernel_launches++;
+auto accumulation_kernel(const lrk_ctx *ctx) { return ctx->pass_moments != nullptr ? accumulate_kernel<true> : accumulate_kernel<false>; }
+auto closest_kernel(const lrk_ctx *ctx, bool alpha) {
+    return alpha ? (ctx->count_traversal ? trace_closest_kernel<true, true> : trace_closest_kernel<false, true>)
+                 : (ctx->count_traversal ? trace_closest_kernel<true, false> : trace_closest_kernel<false, false>);
 }
+auto shadow_kernel(const lrk_ctx *ctx) {
+    return ctx->any_non_opaque ? (ctx->count_traversal ? trace_shadow_kernel<true, true> : trace_shadow_kernel<false, true>)
+                               : (ctx->count_traversal ? trace_shadow_kernel<true, false> : trace_shadow_kernel<false, false>);
+}
+auto general_kernel(const lrk_ctx *ctx) { return ctx->any_non_opaque ? volume_general_kernel<true> : volume_general_kernel<false>; }
+auto medium_shadow_kernel(const lrk_ctx *ctx) { return ctx->count_traversal ? trace_medium_shadow_kernel<true> : trace_medium_shadow_kernel<false>; }
+auto volume_nee_kernel(const lrk_ctx *ctx) { return ctx->count_traversal ? trace_volume_nee_kernel<true> : trace_volume_nee_kernel<false>; }
 
-// The G-buffer sums of a pass (G-buffer films only): after depth 0's closest-hit trace, while pb.hit and ray_o / ray_d[0] still hold
-// the camera samples' hits and rays.
-void launch_gbuffer(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp) {
-    ScopedTimer t{ctx, CAT_OTHER};
-    const auto &pb = ctx->pb;
-    gbuffer_kernel<<<(npix + kBlock - 1u) / kBlock, kBlock, 0, ctx->stream>>>(ctx->scene, pb.ray_o[0], pb.ray_d[0], pb.hit, pixel_list, pixel_offset, npix, spp,
-                                                                            ctx->d_gb_albedo.get<float4>(), ctx->d_gb_normal.get<float4>(),
-                                                                            ctx->d_gb_hits.get<float>());
-    ctx->stats.kernel_launches++;
+// lrk_trace / lrk_trace_device: not a render's kernel, so not counted
+void launch_query(lrk_ctx *ctx, bool any_hit, const float4 *d_rays, uint4 *d_hits, uint32_t n) {
+    query_kernel(ctx, any_hit)<<<blocks_for(ctx, n, ctx->grids.query), kTraceBlock, 0, ctx->stream>>>(ctx->scene, d_rays, d_hits, n,
+                                                                                                      ctx->d_query_cursor.get<uint32_t>());
 }
 
 // Closest-hit traversal of the path queue of `depth`.  The volume pass launches it with alpha = false: the volume integrator rejects
 // non-opaque surfaces at upload.
 void launch_trace_closest(lrk_ctx *ctx, bool alpha, uint64_t n, uint32_t depth) {
-    ScopedTimer t{ctx, CAT_TRACE_CLOSEST};
     const auto &pb = ctx->pb;
-    const bool count = ctx->count_traversal;
-    const auto kernel = alpha ? (count ? trace_closest_kernel<true, true> : trace_closest_kernel<false, true>)
-                              : (count ? trace_closest_kernel<true, false> : trace_closest_kernel<false, false>);
     const int in = depth & 1u;
-    kernel<<<blocks_for(ctx, n, ctx->grid_trace), kTraceBlock, 0, ctx->stream>>>(ctx->scene, pb.ray_o[in], pb.ray_d[in], pb.hit, path_count(pb.counts, depth),
-                                                                                 closest_cursor(pb.counts, depth), pb.stats);
-    ctx->stats.kernel_launches++;
+    Stage(ctx, CAT_TRACE_CLOSEST).launch(closest_kernel(ctx, alpha), blocks_for(ctx, n, ctx->grids.closest), kTraceBlock, ctx->scene, pb.ray_o[in],
+                                         pb.ray_d[in], pb.hit, path_count(pb.counts, depth), closest_cursor(pb.counts, depth), pb.stats);
+}
+
+// The end of every pass: the film accumulation, with the adaptive mode's moments while lrk_render_adaptive runs.
+int finish_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp) {
+    Stage(ctx, CAT_OTHER).launch(accumulation_kernel(ctx), (npix + kBlock - 1u) / kBlock, kBlock, ctx->scene, ctx->pb.li, ctx->d_film.get<float4>(),
+                                 pixel_list, pixel_offset, npix, spp, ctx->pb.counts, ctx->pb.stats, ctx->pass_moments);
+    ctx->stats.passes++;
+    LRK_CUDA(cudaGetLastError());
+    return LRK_OK;
 }
 
 // One pass: sample indices [spp_begin, spp_begin + spp) of the pixels pixel_list[pixel_offset .. pixel_offset + npix).
@@ -426,116 +445,73 @@ int render_pass(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset,
     pb.tile_cost_size = ctx->tile_size;
     pb.tile_cost_tiles_x = (ctx->scene.width + ctx->tile_size - 1u) / ctx->tile_size;
     const auto &sc = ctx->scene;
-    {
-        ScopedTimer t{ctx, CAT_OTHER};
-        generate_rays_kernel<<<static_cast<unsigned>((n + kBlock - 1u) / kBlock), kBlock, 0, ctx->stream>>>(
-            sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
-        ctx->stats.kernel_launches++;
-    }
+    const auto &grids = ctx->grids;
+    Stage(ctx, CAT_OTHER).launch(generate_rays_kernel, static_cast<unsigned>((n + kBlock - 1u) / kBlock), kBlock, sc, pb, pixel_list, pixel_offset,
+                                 npix, spp_begin, static_cast<uint32_t>(n));
     // upper bound of the live queue at depth d is n; launch persistent-size grids and let kernels read *count
     for (uint32_t depth = 0; depth < sc.max_depth; depth++) {
         launch_trace_closest(ctx, ctx->any_non_opaque, n, depth);
-        if (depth == 0u && ctx->gbuffer_film) launch_gbuffer(ctx, pixel_list, pixel_offset, npix, spp);
+        // the G-buffer sums (G-buffer films only): pb.hit and ray_o / ray_d[0] still hold the camera samples' hits and rays
+        if (depth == 0u && ctx->gbuffer_film)
+            Stage(ctx, CAT_OTHER).launch(gbuffer_kernel, (npix + kBlock - 1u) / kBlock, kBlock, sc, pb.ray_o[0], pb.ray_d[0], pb.hit, pixel_list,
+                                         pixel_offset, npix, spp, ctx->d_gb_albedo.get<float4>(), ctx->d_gb_normal.get<float4>(),
+                                         ctx->d_gb_hits.get<float>());
         {
-            ScopedTimer t{ctx, CAT_SHADE};
-            if (sc.env_present) {
-                shade_miss_kernel<<<blocks_for(ctx, n, ctx->grid_classify), kBlock, 0, ctx->stream>>>(sc, pb, depth);
-                ctx->stats.kernel_launches++;
-            }
-            classify_hits_kernel<<<blocks_for(ctx, n, ctx->grid_classify), kBlock, 0, ctx->stream>>>(sc, pb, depth);
-            ctx->stats.kernel_launches++;
+            Stage shade{ctx, CAT_SHADE};
+            if (sc.env_present) shade.launch(shade_miss_kernel, blocks_for(ctx, n, grids.miss), kBlock, sc, pb, depth);
+            shade.launch(classify_hits_kernel, blocks_for(ctx, n, grids.classify), kBlock, sc, pb, depth);
             // one kernel per closure kind over its own hit bucket (shade.cu); TEXTURED variants only for scenes with image-textured
             // parameters / normal maps
             for (uint32_t kind = 0; kind < kHitKinds; kind++) {
                 if (!(ctx->used_kinds & (1u << kind))) continue;
                 const bool strict = ctx->strict_math || hit_kind_always_strict(kind);
-                const int blocks = blocks_for(ctx, n, ctx->grid_shade[strict ? 1 : 0][kind]);
-                if (strict) strict::launch_shade(kind, ctx->textured, ctx->light_active, blocks, ctx->stream, sc, pb, depth);
-                else fast::launch_shade(kind, ctx->textured, ctx->light_active, blocks, ctx->stream, sc, pb, depth);
-                ctx->stats.kernel_launches++;
+                const ShadeKernel kernel = strict ? strict::shade_kernel_for(kind, ctx->textured, ctx->light_active)
+                                                  : fast::shade_kernel_for(kind, ctx->textured, ctx->light_active);
+                shade.launch(kernel, blocks_for(ctx, n, grids.shade[strict][kind]), kShadeBlock, sc, pb, depth);
             }
         }
-        {
-            ScopedTimer t{ctx, CAT_TRACE_SHADOW};
-            const bool count = ctx->count_traversal;
-            const auto kernel = ctx->any_non_opaque ? (count ? trace_shadow_kernel<true, true> : trace_shadow_kernel<false, true>)
-                                                    : (count ? trace_shadow_kernel<true, false> : trace_shadow_kernel<false, false>);
-            kernel<<<blocks_for(ctx, n, ctx->grid_shadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, shadow_count(pb.counts, depth), shadow_cursor(pb.counts, depth));
-            ctx->stats.kernel_launches++;
-        }
+        Stage(ctx, CAT_TRACE_SHADOW).launch(shadow_kernel(ctx), blocks_for(ctx, n, grids.shadow), kTraceBlock, sc, pb, shadow_count(pb.counts, depth),
+                                            shadow_cursor(pb.counts, depth));
     }
-    launch_accumulate(ctx, pixel_list, pixel_offset, npix, spp);
-    ctx->stats.passes++;
-    LRK_CUDA(cudaGetLastError());
-    return LRK_OK;
+    return finish_pass(ctx, pixel_list, pixel_offset, npix, spp);
 }
 
-// One pass of the volume path integrator (config C4); schedule described in kernels.cuh.
-// the general volume path: one thread per camera sample (volume_general.cuh), then the common film accumulation
-int render_pass_volume_general(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp_begin, uint32_t spp) {
-    const uint64_t n = static_cast<uint64_t>(npix) * spp;
-    auto &pb = ctx->pb;
-    const auto &sc = ctx->scene;
-    {
-        ScopedTimer t{ctx, CAT_SHADE};
-        const unsigned blocks = static_cast<unsigned>((n + kGeneralBlock - 1u) / kGeneralBlock);
-        const auto kernel = ctx->any_non_opaque ? volume_general_kernel<true> : volume_general_kernel<false>;
-        kernel<<<blocks, kGeneralBlock, 0, ctx->stream>>>(sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
-        ctx->stats.kernel_launches++;
-    }
-    launch_accumulate(ctx, pixel_list, pixel_offset, npix, spp);
-    ctx->stats.passes++;
-    LRK_CUDA(cudaGetLastError());
-    return LRK_OK;
-}
-
+// One pass of the volume path integrator.  Media bound to shapes and the other scenes beyond config C4 (SceneCheck::volume_general):
+// one thread per camera sample (volume_general.cuh).  Config C4: the wavefront schedule described in kernels.cuh.
 int render_pass_volume(lrk_ctx *ctx, const uint32_t *pixel_list, uint32_t pixel_offset, uint32_t npix, uint32_t spp_begin, uint32_t spp) {
-    if (ctx->volume_general) return render_pass_volume_general(ctx, pixel_list, pixel_offset, npix, spp_begin, spp);
     const uint64_t n = static_cast<uint64_t>(npix) * spp;
     auto &pb = ctx->pb;
     const auto &sc = ctx->scene;
-    {
-        ScopedTimer t{ctx, CAT_OTHER};
-        generate_rays_volume_kernel<<<static_cast<unsigned>((n + kBlock - 1u) / kBlock), kBlock, 0, ctx->stream>>>(
-            sc, pb, pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
-        ctx->stats.kernel_launches++;
+    const auto &grids = ctx->grids;
+    if (ctx->volume_general) {
+        Stage(ctx, CAT_SHADE).launch(general_kernel(ctx), static_cast<unsigned>((n + kGeneralBlock - 1u) / kGeneralBlock), kGeneralBlock, sc, pb,
+                                     pixel_list, pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
+        return finish_pass(ctx, pixel_list, pixel_offset, npix, spp);
     }
+    Stage(ctx, CAT_OTHER).launch(generate_rays_volume_kernel, static_cast<unsigned>((n + kBlock - 1u) / kBlock), kBlock, sc, pb, pixel_list,
+                                 pixel_offset, npix, spp_begin, static_cast<uint32_t>(n));
     for (uint32_t depth = 0; depth < sc.max_depth; depth++) {
         const int out = (depth & 1u) ^ 1;
-        {
-            ScopedTimer t{ctx, CAT_TRACE_SHADOW};
-            // the in-medium shadow rays share the depth's path-queue size
-            const auto kernel = ctx->count_traversal ? trace_medium_shadow_kernel<true> : trace_medium_shadow_kernel<false>;
-            kernel<<<blocks_for(ctx, n, ctx->grid_vshadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, path_count(pb.counts, depth), medium_shadow_cursor(pb.counts, depth));
-            ctx->stats.kernel_launches++;
-        }
+        // the in-medium shadow rays share the depth's path-queue size
+        Stage(ctx, CAT_TRACE_SHADOW).launch(medium_shadow_kernel(ctx), blocks_for(ctx, n, grids.medium_shadow), kTraceBlock, sc, pb,
+                                            path_count(pb.counts, depth), medium_shadow_cursor(pb.counts, depth));
         launch_trace_closest(ctx, false, n, depth);
         {
-            ScopedTimer t{ctx, CAT_SHADE};
+            Stage shade{ctx, CAT_SHADE};
             const int v = ctx->strict_math ? 1 : 0;
-            if (v) strict::launch_volume_medium(blocks_for(ctx, n, ctx->grid_vmedium[v]), ctx->stream, sc, pb, depth);
-            else fast::launch_volume_medium(blocks_for(ctx, n, ctx->grid_vmedium[v]), ctx->stream, sc, pb, depth);
-            ctx->stats.kernel_launches++;
+            const ShadeKernel medium = v ? strict::volume_medium_kernel_for() : fast::volume_medium_kernel_for();
+            shade.launch(medium, blocks_for(ctx, n, grids.volume_medium[v]), kBlock, sc, pb, depth);
             for (uint32_t kind = 0; kind <= kHitDisney; kind++) {
                 if (!(ctx->used_kinds & (1u << kind))) continue;
-                const int blocks = blocks_for(ctx, n, ctx->grid_vshade[v][kind]);
-                if (v) strict::launch_volume_surface(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
-                else fast::launch_volume_surface(kind, ctx->textured, blocks, ctx->stream, sc, pb, depth);
-                ctx->stats.kernel_launches++;
+                const ShadeKernel kernel = v ? strict::volume_surface_kernel_for(kind, ctx->textured)
+                                             : fast::volume_surface_kernel_for(kind, ctx->textured);
+                shade.launch(kernel, blocks_for(ctx, n, grids.volume_surface[v][kind]), kBlock, sc, pb, depth);
             }
         }
-        {
-            ScopedTimer t{ctx, CAT_TRACE_SHADOW};
-            const auto kernel = ctx->count_traversal ? trace_volume_nee_kernel<true> : trace_volume_nee_kernel<false>;
-            kernel<<<blocks_for(ctx, n, ctx->grid_vshadow), kTraceBlock, 0, ctx->stream>>>(sc, pb, shadow_count(pb.counts, depth), shadow_cursor(pb.counts, depth),
-                                                                                         pb.occl2[out]);
-            ctx->stats.kernel_launches++;
-        }
+        Stage(ctx, CAT_TRACE_SHADOW).launch(volume_nee_kernel(ctx), blocks_for(ctx, n, grids.volume_nee), kTraceBlock, sc, pb,
+                                            shadow_count(pb.counts, depth), shadow_cursor(pb.counts, depth), pb.occl2[out]);
     }
-    launch_accumulate(ctx, pixel_list, pixel_offset, npix, spp);
-    ctx->stats.passes++;
-    LRK_CUDA(cudaGetLastError());
-    return LRK_OK;
+    return finish_pass(ctx, pixel_list, pixel_offset, npix, spp);
 }
 
 // Scratch of the device hierarchy build (bvh_build.cuh) for sets of at most max_n primitives, carved out of a.build_scratch: boxes,
@@ -1114,6 +1090,37 @@ int write_scene_record(lrk_ctx *ctx) {
     return LRK_OK;
 }
 
+// The blocks of one persistent grid: as many as are resident at once, (blocks per SM at full occupancy) x SM count.
+template<typename... Params>
+int persistent_grid(void (*kernel)(Params...), int block, int sm_count) {
+    int per_sm = 0;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0);
+    return std::max(1, per_sm) * sm_count;
+}
+
+// The grid table (Grids).  Three kernels borrow another kernel's grid instead of being measured themselves.
+Grids measure_grids(int sm_count) {
+    Grids g{};
+    g.closest = persistent_grid(trace_closest_kernel<false, false>, kTraceBlock, sm_count);
+    g.query = g.closest;// lrk_trace's queries: the same trace_queue walk at the same block size
+    g.shadow = persistent_grid(trace_shadow_kernel<false, false>, kTraceBlock, sm_count);
+    for (uint32_t kind = 0; kind < kHitKinds; kind++) {// the fast variant has no kernel for the kinds that are always strict
+        if (!hit_kind_always_strict(kind)) g.shade[0][kind] = persistent_grid(fast::shade_kernel_for(kind, false, LightSampling{}), kShadeBlock, sm_count);
+        g.shade[1][kind] = persistent_grid(strict::shade_kernel_for(kind, false, LightSampling{}), kShadeBlock, sm_count);
+    }
+    g.classify = persistent_grid(classify_hits_kernel, kBlock, sm_count);
+    g.miss = g.classify;// the escaped rays: a loop over the same depth's queue at the same block size, launched just before classification
+    g.volume_medium[0] = persistent_grid(fast::volume_medium_kernel_for(), kBlock, sm_count);
+    g.volume_medium[1] = persistent_grid(strict::volume_medium_kernel_for(), kBlock, sm_count);
+    for (uint32_t kind = 0; kind < 3u; kind++) {
+        g.volume_surface[0][kind] = persistent_grid(fast::volume_surface_kernel_for(kind, false), kBlock, sm_count);
+        g.volume_surface[1][kind] = persistent_grid(strict::volume_surface_kernel_for(kind, false), kBlock, sm_count);
+    }
+    g.volume_nee = persistent_grid(trace_volume_nee_kernel<false>, kTraceBlock, sm_count);
+    g.medium_shadow = g.volume_nee;// the in-medium shadow rays: the same any-hit trace_queue walk as the surface NEE rays
+    return g;
+}
+
 }// namespace
 
 // The one teardown of a context, run with its device current and its stream idle (lrk_destroy, or a failed lrk_create).  The device
@@ -1159,25 +1166,7 @@ int lrk_create(const lrk_device_cfg *cfg, lrk_ctx **out) {
     cudaEventCreate(&ctx->ev_begin);
     cudaEventCreate(&ctx->ev_end);
     if (ctx->d_query_cursor.reserve(64u * sizeof(uint32_t)) != cudaSuccess) return LRK_ERR_OUT_OF_MEMORY;
-    auto grid_for = [&](const void *fn, int block = kBlock) {
-        int per_sm = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, block, 0);
-        return std::max(1, per_sm) * ctx->sm_count;
-    };
-    ctx->grid_trace = grid_for(reinterpret_cast<const void *>(trace_closest_kernel<false, false>), kTraceBlock);
-    ctx->grid_shadow = grid_for(reinterpret_cast<const void *>(trace_shadow_kernel<false, false>), kTraceBlock);
-    for (uint32_t kind = 0; kind < kHitKinds; kind++) {
-        if (!hit_kind_always_strict(kind)) ctx->grid_shade[0][kind] = fast::shade_grid(kind, ctx->sm_count);
-        ctx->grid_shade[1][kind] = strict::shade_grid(kind, ctx->sm_count);
-    }
-    ctx->grid_classify = grid_for(reinterpret_cast<const void *>(classify_hits_kernel));
-    ctx->grid_vmedium[0] = fast::volume_medium_grid(ctx->sm_count);
-    ctx->grid_vmedium[1] = strict::volume_medium_grid(ctx->sm_count);
-    for (uint32_t kind = 0; kind < 3u; kind++) {
-        ctx->grid_vshade[0][kind] = fast::volume_surface_grid(kind, ctx->sm_count);
-        ctx->grid_vshade[1][kind] = strict::volume_surface_grid(kind, ctx->sm_count);
-    }
-    ctx->grid_vshadow = grid_for(reinterpret_cast<const void *>(trace_volume_nee_kernel<false>), kTraceBlock);
+    ctx->grids = measure_grids(ctx->sm_count);
     *out = ctx.release();
     return LRK_OK;
 }
@@ -1987,16 +1976,15 @@ int lrk_render_adaptive(lrk_ctx *ctx, const lrk_adaptive *p) {
         c = next;
         const bool last = c >= p->max_spp;
         const unsigned grid = static_cast<unsigned>((static_cast<uint64_t>(nblocks + 1u) * 32u + kAdaptiveBlock - 1u) / kAdaptiveBlock);
-        adaptive_test_kernel<<<grid, kAdaptiveBlock, 0, ctx->stream>>>(ctx->scene.width, ctx->d_film.get<float4>(), ctx->d_moments.get<float2>(), list, blocks,
-                                                                        nblocks, p->threshold, c, last, ctx->d_sample_counts.get<uint32_t>(), keep);
-        ctx->stats.kernel_launches++;
+        Stage stage{ctx, CAT_NONE};
+        stage.launch(adaptive_test_kernel, grid, kAdaptiveBlock, ctx->scene.width, ctx->d_film.get<float4>(), ctx->d_moments.get<float2>(), list, blocks,
+                     nblocks, p->threshold, c, last, ctx->d_sample_counts.get<uint32_t>(), keep);
         if (last) break;
         size_t temp = ctx->d_scan_temp.bytes();
         LRK_CUDA(cub::DeviceScan::ExclusiveSum(ctx->d_scan_temp.get(), temp, keep, offsets, static_cast<int>(nblocks + 1u), ctx->stream));
         ctx->stats.kernel_launches++;
         uint32_t *list_out = ctx->d_active[round & 1u].get<uint32_t>(), *blocks_out = ctx->d_block_start[1u + (round & 1u)].get<uint32_t>();
-        adaptive_compact_kernel<<<grid, kAdaptiveBlock, 0, ctx->stream>>>(list, blocks, nblocks, keep, offsets, list_out, blocks_out);
-        ctx->stats.kernel_launches++;
+        stage.launch(adaptive_compact_kernel, grid, kAdaptiveBlock, list, blocks, nblocks, keep, offsets, list_out, blocks_out);
         LRK_CUDA(cudaGetLastError());
         unsigned long long total = 0ull;
         LRK_CUDA(cudaMemcpyAsync(&total, offsets + nblocks, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
@@ -2137,9 +2125,8 @@ int lrk_trace(lrk_ctx *ctx, const lrk_ray *rays, uint64_t n, int any_hit, lrk_hi
     LRK_CUDA(d_rays.reserve(n * sizeof(lrk_ray)));
     if (d_hits.reserve(n * sizeof(lrk_hit)) != cudaSuccess) return fail(ctx, LRK_ERR_OUT_OF_MEMORY, "lrk_trace: out of device memory");
     cudaMemcpyAsync(d_rays.get(), rays, n * sizeof(lrk_ray), cudaMemcpyHostToDevice, ctx->stream);
-    int g = blocks_for(ctx, n, ctx->grid_trace);
     cudaMemsetAsync(ctx->d_query_cursor.get(), 0, sizeof(uint32_t), ctx->stream);
-    launch_query(ctx, g, any_hit != 0, d_rays.get<float4>(), d_hits.get<uint4>(), static_cast<uint32_t>(n));
+    launch_query(ctx, any_hit != 0, d_rays.get<float4>(), d_hits.get<uint4>(), static_cast<uint32_t>(n));
     cudaMemcpyAsync(hits, d_hits.get(), n * sizeof(lrk_hit), cudaMemcpyDeviceToHost, ctx->stream);
     cudaMemcpyAsync(&ctx->h_overflow, ctx->scene.traversal_overflow, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
@@ -2153,11 +2140,10 @@ int lrk_trace_device(lrk_ctx *ctx, const void *d_rays, uint64_t n, int any_hit, 
     if (!ctx || !ctx->has_scene) return fail(ctx, LRK_ERR_NO_SCENE, "lrk_trace_device: no scene");
     if (!d_rays || !d_hits || n == 0u || n > 0xffffffffull || repeat == 0u) return fail(ctx, LRK_ERR_INVALID_ARGUMENT, "lrk_trace_device: bad argument");
     LRK_CUDA(cudaSetDevice(ctx->device));
-    int g = blocks_for(ctx, n, ctx->grid_trace);
     LRK_CUDA(cudaEventRecord(ctx->ev_begin, ctx->stream));
     for (uint32_t r = 0; r < repeat; r++) {
         LRK_CUDA(cudaMemsetAsync(ctx->d_query_cursor.get(), 0, sizeof(uint32_t), ctx->stream));
-        launch_query(ctx, g, any_hit != 0, static_cast<const float4 *>(d_rays), static_cast<uint4 *>(d_hits), static_cast<uint32_t>(n));
+        launch_query(ctx, any_hit != 0, static_cast<const float4 *>(d_rays), static_cast<uint4 *>(d_hits), static_cast<uint32_t>(n));
     }
     LRK_CUDA(cudaEventRecord(ctx->ev_end, ctx->stream));
     LRK_CUDA(cudaStreamSynchronize(ctx->stream));

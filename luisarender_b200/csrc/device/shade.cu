@@ -30,13 +30,6 @@ namespace {
 #define LRK_SHADE_IS_FAST(v) LRK_SHADE_IS_FAST_OF(v)
 constexpr bool kFastVariant = LRK_SHADE_IS_FAST(LRK_SHADE_VARIANT);
 
-template<typename Kernel>
-int grid_of(Kernel kernel, int block, int sm_count) {
-    int per_sm = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0);
-    return (per_sm > 0 ? per_sm : 1) * sm_count;
-}
-
 // calls f(std::bool_constant<b>{}): the run-time flag as a compile-time one
 template<typename F>
 void with_flag(bool b, F &&f) {
@@ -44,66 +37,63 @@ void with_flag(bool b, F &&f) {
     else f(std::false_type{});
 }
 
-// calls f(kernel) with the shade kernel instantiation of (kind, textured, light selection, light point sampling), or with the
-// kind's resampling instantiation (RESAMPLE; none for emitter-only hits).  The fast variant has none for the kinds that always run
-// in strict arithmetic (hit_kind_always_strict): render_pass never launches them there.
-template<uint32_t SEL, uint32_t PT, bool RESAMPLE = false, bool RECEIVER = false, typename F>
-void with_shade_kernel(uint32_t kind, bool textured, F &&f) {
+// The shade kernel instantiation of (kind, textured, light selection, light point sampling), or the kind's resampling instantiation
+// (RESAMPLE; none for emitter-only hits).  The fast variant has none for the kinds that always run in strict arithmetic
+// (hit_kind_always_strict): render_pass never launches them there.
+template<uint32_t SEL, uint32_t PT, bool RESAMPLE = false, bool RECEIVER = false>
+ShadeKernel shade_kernel_of(uint32_t kind, bool textured) {
+    ShadeKernel kernel = nullptr;
     with_hit_kind(kind, [&](auto k) {
         constexpr uint32_t K = decltype(k)::value;
         if constexpr (!(kFastVariant && hit_kind_always_strict(K)) && !(RESAMPLE && K == kHitEmitter))
-            textured ? f(shade_kernel<K, true, SEL, PT, RESAMPLE, RECEIVER>) : f(shade_kernel<K, false, SEL, PT, RESAMPLE, RECEIVER>);
+            kernel = textured ? shade_kernel<K, true, SEL, PT, RESAMPLE, RECEIVER> : shade_kernel<K, false, SEL, PT, RESAMPLE, RECEIVER>;
     });
+    return kernel;
 }
-// the volume integrator's surface step exists for the kinds of config C4's closures: emitter-only, Matte and Disney
-template<typename F>
-void with_volume_surface_kernel(uint32_t kind, bool textured, F &&f) {
-    with_hit_kind(kind, [&](auto k) {
-        constexpr uint32_t K = decltype(k)::value;
-        if constexpr (K <= kHitDisney) textured ? f(volume_surface_kernel<K, true>) : f(volume_surface_kernel<K, false>);
-    });
-}
+
+// Defined below the volume steps' lookups: the kernels are instantiated in source order, and the cubin keeps its function order.
+ShadeKernel light_option_kernel(uint32_t kind, bool textured, bool resample, bool tree, bool solid_angle, bool receiver);
 
 }// namespace
-
-int shade_grid(uint32_t kind, int sm_count) {
-    int g = 1;
-    with_shade_kernel<kLightSelectUniform, kLightPointArea>(kind, false, [&](auto kernel) { g = grid_of(kernel, kShadeBlock, sm_count); });
-    return g;
-}
-
-int volume_medium_grid(int sm_count) { return grid_of(volume_medium_kernel, kBlock, sm_count); }
-
-int volume_surface_grid(uint32_t kind, int sm_count) {
-    int g = 1;
-    with_volume_surface_kernel(kind, false, [&](auto kernel) { g = grid_of(kernel, kBlock, sm_count); });
-    return g;
-}
 
 // The light sampling as the kernels' <SEL, PT, RESAMPLE, RECEIVER>.  The triangle-level trees need no instantiation of their own: the
 // kernels find them through light_tree_of(sc).bottom_nodes.  Resampling (candidates >= 2) has one instantiation per kind, which reads
 // the selection, the point sampling and the candidate count from light_tree_of(sc); emitter-only hits sample no light and keep
 // theirs.  The receiver refines the tree, the solid-angle sampler and the resampling only: uniform area sampling keeps its kernel.
-void launch_shade(uint32_t kind, bool textured, const LightSampling &light, int blocks, cudaStream_t stream, const DeviceScene &sc,
-                  const PathBuffers &pb, uint32_t depth) {
+ShadeKernel shade_kernel_for(uint32_t kind, bool textured, const LightSampling &light) {
     const bool resample = light.candidates >= 2u && kind != kHitEmitter;
     const bool tree = light.tree && !resample, solid_angle = light.solid_angle && !resample;
-    const bool receiver = light.receiver && (resample || tree || solid_angle);
+    if (!resample && !tree && !solid_angle) return shade_kernel_of<kLightSelectUniform, kLightPointArea>(kind, textured);
+    return light_option_kernel(kind, textured, resample, tree, solid_angle, light.receiver);
+}
+
+ShadeKernel volume_medium_kernel_for() { return volume_medium_kernel; }
+
+// the volume integrator's surface step exists for the kinds of config C4's closures: emitter-only, Matte and Disney
+ShadeKernel volume_surface_kernel_for(uint32_t kind, bool textured) {
+    ShadeKernel kernel = nullptr;
+    with_hit_kind(kind, [&](auto k) {
+        constexpr uint32_t K = decltype(k)::value;
+        if constexpr (K <= kHitDisney) kernel = textured ? volume_surface_kernel<K, true> : volume_surface_kernel<K, false>;
+    });
+    return kernel;
+}
+
+namespace {
+
+// shade_kernel_for's flags when resample, tree or solid_angle is set
+ShadeKernel light_option_kernel(uint32_t kind, bool textured, bool resample, bool tree, bool solid_angle, bool receiver) {
+    ShadeKernel kernel = nullptr;
     with_flag(resample, [&](auto r) { with_flag(tree, [&](auto t) { with_flag(solid_angle, [&](auto s) { with_flag(receiver, [&](auto v) {
         constexpr bool RESAMPLE = decltype(r)::value, TREE = decltype(t)::value, SOLID_ANGLE = decltype(s)::value, RECEIVER = decltype(v)::value;
-        if constexpr (!(RESAMPLE && (TREE || SOLID_ANGLE)) && (!RECEIVER || RESAMPLE || TREE || SOLID_ANGLE))// the flags' combinations above
-            with_shade_kernel<TREE ? kLightSelectTree : kLightSelectUniform, SOLID_ANGLE ? kLightPointSolidAngle : kLightPointArea, RESAMPLE, RECEIVER>(
-                    kind, textured, [&](auto kernel) { kernel<<<blocks, kShadeBlock, 0, stream>>>(sc, pb, depth); });
+        if constexpr (!(RESAMPLE && (TREE || SOLID_ANGLE)) && (!RECEIVER || RESAMPLE || TREE || SOLID_ANGLE))// the combinations shade_kernel_for passes
+            kernel = shade_kernel_of<TREE ? kLightSelectTree : kLightSelectUniform, SOLID_ANGLE ? kLightPointSolidAngle : kLightPointArea, RESAMPLE,
+                                     RECEIVER>(kind, textured);
     }); }); }); });
+    return kernel;
 }
 
-void launch_volume_medium(int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth) {
-    volume_medium_kernel<<<blocks, kBlock, 0, stream>>>(sc, pb, depth);
-}
-
-void launch_volume_surface(uint32_t kind, bool textured, int blocks, cudaStream_t stream, const DeviceScene &sc, const PathBuffers &pb, uint32_t depth) {
-    with_volume_surface_kernel(kind, textured, [&](auto kernel) { kernel<<<blocks, kBlock, 0, stream>>>(sc, pb, depth); });
-}
+}// namespace
 
 }// namespace LRK_SHADE_VARIANT
 }// namespace lrk

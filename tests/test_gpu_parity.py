@@ -214,7 +214,7 @@ def test_render_is_deterministic_and_independent_of_scheduling(cornell_small, gp
     assert st["closest_xforms"] + st["shadow_xforms"] <= cnt["xforms"]
 
 
-SURFACE_DISNEY, SURFACE_LAYERED, SURFACE_DISNEY_THIN, INTEGRATOR_VOLUME_PATH = 1, 7, 64, 1  # include/lrk.h
+SURFACE_DISNEY, SURFACE_LAYERED, SURFACE_DISNEY_THIN, INTEGRATOR_VOLUME_PATH, SHAPE_HAS_MEDIUM = 1, 7, 64, 1, 16  # include/lrk.h
 
 
 def _hit_buckets(d):
@@ -235,24 +235,29 @@ def _hit_buckets(d):
     return used
 
 
-@pytest.mark.parametrize("name", ["environment", "layered", "disney_thin", "c4_medium"])
+@pytest.mark.parametrize("name", ["environment", "layered", "disney_thin", "c4_medium", "shape_media"])
 def test_kernel_launch_count_follows_the_scene(name, gpu_renderer):
     """stats()["kernel_launches"] restated from the scene.  Surface path, per pass: ray generation and film accumulation, and per depth
     closest hit, classification, bucket 0's shade kernel, the shadow rays, the miss kernel when an environment light is present, and
     one shade kernel per further hit bucket in use.  Volume path (C4), per depth: in-medium shadow rays, closest hit, the medium step,
-    bucket 0's surface step, the surface NEE rays, and the surface steps of buckets 1 and 2 when used."""
+    bucket 0's surface step, the surface NEE rays, and the surface steps of buckets 1 and 2 when used.  Volume path with media bound
+    to shapes, per pass: the per-thread kernel and film accumulation."""
     if name in ("disney_thin", "c4_medium"):  # the reference-render fixtures' scene texts (tests/test_ref_render.py)
         key = {"disney_thin": "spheres_disney_thin", "c4_medium": "config_c4_full_scene"}[name]
         src = bytes(np.load(REPO / "tests" / "golden" / "ref_renders.npz")[f"{key}/scene"]).decode()
     else:
-        src = scenes.environment_scene() if name == "environment" else scenes.layered_box()
+        src = {"environment": scenes.environment_scene, "layered": scenes.layered_box, "shape_media": scenes.media_box}[name]()
     scene = Scene.from_source(src, REPO)
     d = scene.desc()
     buckets, depth = _hit_buckets(d), d.integrator.max_depth
     volume = d.integrator.type == INTEGRATOR_VOLUME_PATH
+    shape_media = any(inst.handle[0] & SHAPE_HAS_MEDIUM for inst in d.instances[:d.instance_count])
     # each scene exercises what it is here for
-    assert {"environment": d.environment.present, "layered": 9 in buckets, "disney_thin": 10 in buckets, "c4_medium": volume}[name]
-    if volume:
+    assert {"environment": d.environment.present, "layered": 9 in buckets, "disney_thin": 10 in buckets, "c4_medium": volume and not shape_media,
+            "shape_media": volume and shape_media}[name]
+    if shape_media:
+        per_pass = 2
+    elif volume:
         per_pass = 2 + depth * (5 + (1 in buckets) + (2 in buckets))
     else:
         per_pass = 2 + depth * (4 + bool(d.environment.present) + len(buckets))
