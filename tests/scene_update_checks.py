@@ -183,6 +183,70 @@ def with_hierarchies(b, blas, mesh_table):
     return h, keep
 
 
+def refit_frame(a, b, lib):
+    """A description that renders frame b with frame a's mesh hierarchies refit to b's vertices (what lrk_update_meshes leaves on
+    the device): a's refit BLAS nodes and mesh table, a's slot order with b's positions, b's vertices and instances, and b's
+    instance level appended behind a's meshes.  Returns the description, the arrays it points into and the refit meshes' pads."""
+    nodes_a = S.array(a.bvh_nodes, a.bvh_node_count, F.BvhNode, np.uint32, 16)
+    blas = np.ascontiguousarray(nodes_a[:a.tlas_root])
+    # a's slot order, b's positions: every slot's primitive re-read through b's triangles and vertices
+    tv = S.array(a.tri_verts, a.tri_slot_count, C.c_float * 12).copy()
+    vb, tris = S.vertices(b), S.triangles(b)
+    m = S.meshes(a)
+    for vo, vc, to, tc, _root, so, *_ in m:
+        prim = tv[so:so + tc, 3].view(np.uint32)
+        t = tris[to + prim]
+        for c in range(3):
+            tv[so:so + tc, 4 * c:4 * c + 3] = vb[vo + t[:, c], :3]
+    ids, _ = S.deformed_meshes(a, b)
+    pads = {}
+    for k in ids:
+        root, end = node_ranges(a)[k]
+        pad = C.c_float()
+        assert lib.refit_mesh(blas.ctypes.data, root, end, tv.ctypes.data, int(m[k][5]), int(m[k][3]), C.byref(pad)) == 0
+        pads[k] = pad.value
+    h, keep = with_hierarchies(b, blas, m)
+    h.tri_verts = tv.ctypes.data_as(C.POINTER(C.c_float))
+    return h, keep + [tv], pads, blas, tv, ids
+
+
+def move_nodes(lib, nodes, node_delta, slot_delta):
+    out = np.zeros_like(nodes)
+    lib.relayout_nodes(nodes.ctypes.data, out.ctypes.data, len(nodes), node_delta % 2**32, slot_delta % 2**32)
+    return out
+
+
+def relaid_frame(a, b, lib):
+    """The hierarchy lrk_replace_meshes leaves for frame a replaced by frame b's meshes, built on the host: in mesh order, every
+    unchanged mesh's node range of a moved to its new place, every replaced mesh's range of max(n - 1, 1) nodes starting with b's
+    own hierarchy of it (moved), and b's instance level behind them.  Returns the description (b's with these nodes and roots),
+    the arrays it points into, and the new ranges."""
+    ids, _, _ = S.replaced_meshes(a, b)
+    nodes_a = S.array(a.bvh_nodes, a.bvh_node_count, F.BvhNode, np.uint32, 16)
+    nodes_b = S.array(b.bvh_nodes, b.bvh_node_count, F.BvhNode, np.uint32, 16)
+    ma, mb = S.meshes(a), S.meshes(b).copy()
+    ra, rb = node_ranges(a), node_ranges(b)
+    parts, ranges, base = [], [], 0
+    for k in range(b.mesh_count):
+        if k in ids:
+            first, end = rb[k]
+            size = max(int(mb[k, 3]) - 1, 1)
+            assert end - first <= size  # the host's hierarchy never has more nodes than the device builder's
+            part = np.zeros((size, 16), np.uint32)
+            part[:end - first] = move_nodes(lib, nodes_b[first:end], base - first, 0)
+        else:
+            first, end = ra[k]
+            part = move_nodes(lib, nodes_a[first:end], base - first, int(mb[k, 5]) - int(ma[k, 5]))
+            # the same mesh's hierarchy in b (the host build is deterministic), moved from b's place to the new one
+            assert np.array_equal(part, move_nodes(lib, nodes_b[rb[k][0]:rb[k][1]], base - rb[k][0], 0))
+        mb[k, 4] = base
+        ranges.append((base, base + len(part)))
+        parts.append(part)
+        base += len(part)
+    h, keep = with_hierarchies(b, np.concatenate(parts), mb)
+    return h, keep, ranges, ids
+
+
 def recording_renderer(call, record=lambda *args: args):
     """A Renderer over a stand-in for the device library whose function `call` appends record(*its arguments) to the returned
     list and succeeds; record runs while the call's arrays are alive."""

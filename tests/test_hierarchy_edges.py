@@ -7,386 +7,30 @@ CPU: the oracle's BVH walk against its brute-force loop (bit for bit), and the b
 Moeller-Trumbore wherever the float64 answer is unambiguous.  GPU: lrk_trace with the host-built and the device-built (LBVH)
 hierarchy against the same brute force, under every warp-scheduling setting and queue length, and the films of both hierarchies.
 The only rays exempt from bit-exactness are those whose hit the triangle test itself places outside the triangle's padded box
-(outside_own_box): no box test can keep them, and they are counted and bounded.
+(outside_own_box) or, along the world ray, outside its instance's box (outside_instance_box): no box test can keep them, and they
+are counted and bounded.  The catalogue, the rays and the float64 reference are in hierarchy_edge_cases.py.
 """
 from __future__ import annotations
-
-from pathlib import Path
 
 import numpy as np
 import pytest
 
-from luisarender_b200 import scenes
-from luisarender_b200.api import Scene
+from hierarchy_edge_cases import (CATALOGUE, F64_RAYS, FAR_FACTORS, MISS, SEEDS, Case as _Case, assert_equal_hits as _assert_equal_hits,
+                                  differ as _differ, f64_check)
 from oracle import binding as O
-
-REPO = Path(__file__).resolve().parents[1]
-MISS = 0xFFFFFFFF
-FMAX = np.finfo(np.float32).max
-FAR_FACTORS = (3, 30, 100, 1000)
-FAR_RAYS = 20_000  # per distance factor and scene: the BVH-vs-brute-force comparison is cheap, missed hits are rare events
-F64_RAYS = 3_000   # rays per scene that also go through the float64 reference
-
-
-# ---- scene catalogue --------------------------------------------------------------------------------------------------------
-
-def _affine(linear=np.eye(3), translate=(0.0, 0.0, 0.0)):
-    return np.concatenate([np.asarray(linear, np.float64), np.asarray(translate, np.float64)[:, None]], axis=1)
-
-
-def _random_tris(rng, n, center=(0.0, 0.0, 0.0), radius=0.5):
-    p = rng.normal(size=(n * 3, 3))
-    p /= np.linalg.norm(p, axis=1, keepdims=True)
-    return p * radius + np.asarray(center), np.arange(n * 3).reshape(n, 3)
-
-
-def _fan(n, radius=0.5):
-    a = np.linspace(0.0, 2.0 * np.pi, n, endpoint=False)
-    ring = np.stack([radius * np.cos(a), 0.1 * np.sin(3 * a), radius * np.sin(a)], axis=1)
-    p = np.concatenate([[[0.0, 0.0, 0.0]], ring])
-    return p, np.array([[0, 1 + k, 1 + (k + 1) % n] for k in range(n)])
-
-
-def _grid(n=6, size=1.0):
-    xs = np.linspace(-size / 2, size / 2, n + 1)
-    p = np.array([[x, 0.0, z] for z in xs for x in xs])
-    idx = []
-    for j in range(n):
-        for i in range(n):
-            a, b, c, d = j * (n + 1) + i, j * (n + 1) + i + 1, (j + 1) * (n + 1) + i, (j + 1) * (n + 1) + i + 1
-            idx += [[a, b, d], [a, d, c]]
-    return p, np.array(idx)
-
-
-def _graded(kmax=40):
-    """Self-similar triangles of size 2^-k at x = 2^-k: a hierarchy as deep as the number of triangles."""
-    base = np.array([[1.0, 0.0, 0.0], [1.5, 1.0, 0.2], [1.2, 0.3, 1.0]])
-    p = np.concatenate([base * 2.0 ** -k for k in range(kmax + 1)])
-    return p, np.arange(len(p)).reshape(-1, 3)
-
-
-def _rotation(axis, angle):
-    axis = np.asarray(axis, np.float64) / np.linalg.norm(axis)
-    k = np.array([[0, -axis[2], axis[1]], [axis[2], 0, -axis[0]], [-axis[1], axis[0], 0]])
-    return np.eye(3) + np.sin(angle) * k + (1 - np.cos(angle)) * k @ k
-
-
-def catalogue():
-    """name -> (meshes [(positions, indices)], instances [(mesh, 3x4 object_to_world, visible)])."""
-    rng = np.random.default_rng(2024)
-    I = _affine()
-    cat = {}
-    for n in (1, 2, 3, 4, 5, 8, 9, 33):
-        cat[f"tris_{n}"] = ([_random_tris(rng, n)], [(0, I, True)])
-    tri = np.array([[-0.4, -0.3, 0.1], [0.5, -0.2, -0.1], [0.0, 0.45, 0.05]])
-    cat["copies_12"] = ([(np.tile(tri, (12, 1)), np.arange(36).reshape(12, 3))], [(0, I, True)])
-    cat["fan_8"] = ([_fan(8)], [(0, I, True)])
-    cat["fan_64"] = ([_fan(64)], [(0, I, True)])
-    blob = _random_tris(rng, 40)
-    cat["same_transform_twice"] = ([blob], [(0, _affine(_rotation((1, 2, 3), 0.7), (0.1, 0.2, 0.3)), True)] * 2)
-    cat["flat_grid"] = ([_grid()], [(0, I, True)])
-    cat["graded"] = ([_graded()], [(0, I, True)])
-    cat["size_1e-4"] = ([_random_tris(rng, 30, radius=1e-4)], [(0, I, True)])
-    cat["size_1e4"] = ([_random_tris(rng, 30, radius=1e4)], [(0, I, True)])
-    cat["offset_1e4"] = ([_random_tris(rng, 30, center=(1e4, -3e3, 5e3))], [(0, I, True)])
-    far = (3000.0, -2000.0, 5000.0)
-    cat["cancelling_instance"] = ([_random_tris(rng, 60, center=far)], [(0, _affine(translate=-np.asarray(far)), True)])
-    cat["scaled_instance"] = ([_random_tris(rng, 60)], [(0, _affine(0.05 * np.eye(3)), True)])
-    skew = _rotation((0.3, -1.0, 0.5), 1.1) @ np.diag([-1.0, 0.25, 3.0])  # rotation, mirroring, non-uniform scale
-    cat["rotated_mirrored_instance"] = ([_random_tris(rng, 60)], [(0, _affine(skew, (0.2, -0.1, 0.4)), True)])
-    small = _random_tris(rng, 4, radius=0.05)
-    cat["one_instance"] = ([small], [(0, _affine(translate=(0.3, 0.1, -0.2)), True)])
-    cat["two_instances"] = ([small], [(0, _affine(translate=(0.3, 0.1, -0.2)), True), (0, _affine(translate=(-0.3, 0.0, 0.1)), True)])
-    grid = np.stack(np.meshgrid(*[np.linspace(-1.0, 1.0, 10)] * 3, indexing="ij"), axis=-1).reshape(-1, 3)
-    cat["instances_1000"] = ([small], [(0, _affine(_rotation(rng.normal(size=3), rng.uniform(0, 6)), t), True) for t in grid])
-    # invisible instances between and in front of visible ones: rays along z cross both kinds
-    cat["invisible_interleaved"] = ([blob], [(0, _affine(0.3 * np.eye(3), (0.15 * (k % 5), 0.0, 0.4 * k - 2.0)), k % 2 == 1) for k in range(10)])
-    return cat
-
-
-def _world_triangles(meshes, instances):
-    """float64 world-space triangles [(inst, prim, p0, p1, p2)] of the visible instances (the ray generator's view)."""
-    out = []
-    for i, (m, xf, vis) in enumerate(instances):
-        if vis:
-            p, idx = meshes[m]
-            w = p @ xf[:, :3].T + xf[:, 3]
-            out.append(w[idx])
-    return np.concatenate(out)
-
-
-def scene_text(meshes, instances):
-    f = scenes._fmt
-    tris = _world_triangles(meshes, instances)
-    lo, hi = tris.reshape(-1, 3).min(axis=0), tris.reshape(-1, 3).max(axis=0)
-    c, r = (lo + hi) / 2, float((hi - lo).max())
-    ly, s = hi[1] + 0.05 * r, 0.05 * r
-    lamp = [c[0] - s, ly, c[2] - s, c[0] + s, ly, c[2] - s, c[0] + s, ly, c[2] + s, c[0] - s, ly, c[2] + s]
-    eye = c + r * np.array([0.4, 0.9, 2.2])
-    front = (c - eye) / np.linalg.norm(c - eye)
-    lines = ['Surface white : Matte { Kd : Constant { v { 0.6, 0.5, 0.4 } } }',
-             'Light lamp_light : Diffuse { emission : Constant { v { 8.0, 8.0, 8.0 } } }']
-    for k, (p, idx) in enumerate(meshes):
-        lines.append(f"Shape m{k} : InlineMesh {{ positions {{ {', '.join(f(v) for v in p.ravel())} }} "
-                     f"indices {{ {', '.join(str(int(v)) for v in idx.ravel())} }} }}")
-    for k, (m, xf, vis) in enumerate(instances):
-        mat = np.concatenate([xf, [[0.0, 0.0, 0.0, 1.0]]]).ravel()
-        lines.append(f"Shape i{k} : Instance {{ shape {{ @m{m} }} surface {{ @white }} visible {{ {'true' if vis else 'false'} }} "
-                     f"transform : Matrix {{ m {{ {', '.join(f(v) for v in mat)} }} }} }}")
-    lines.append(f"Shape lamp : InlineMesh {{ positions {{ {', '.join(f(v) for v in lamp)} }} indices {{ 0, 1, 2, 0, 2, 3 }} "
-                 "light { @lamp_light } }")
-    shapes = ", ".join([f"@i{k}" for k in range(len(instances))] + ["@lamp"])
-    lines.append(f"Camera camera : Pinhole {{ position {{ {', '.join(f(v) for v in eye)} }} front {{ {', '.join(f(v) for v in front)} }} "
-                 "up { 0.0, 1.0, 0.0 } fov { 45.0 } spp { 4 } film : Color { resolution { 24, 24 } } filter : Box { radius { 0.5 } } "
-                 'file { "edges.exr" } }')
-    lines.append("render { integrator : WavePath { depth { 3 } sampler : Independent { seed { 7 } } } cameras { @camera } "
-                 f"shapes {{ {shapes} }} }}")
-    return "\n".join(lines)
-
-
-# ---- rays ---------------------------------------------------------------------------------------------------------------------
-
-def _desc_triangles(d):
-    """float64 world-space triangles of the flattened scene, with their (instance, primitive) - what the oracle intersects - and the
-    size of their object-space coordinates in world units (what the float32 test's rounding is relative to)."""
-    tris, ids, mags = [], [], []
-    for i in range(d.instance_count):
-        inst = d.instances[i]
-        if not inst.visible:
-            continue
-        mesh = d.meshes[inst.mesh]
-        m = np.array(inst.object_to_world, np.float64).reshape(3, 4)
-        v = np.array([d.vertices[mesh.vertex_offset + k].p[:] for k in range(mesh.vertex_count)], np.float64)
-        t = np.array([[d.triangles[mesh.triangle_offset + k].i0, d.triangles[mesh.triangle_offset + k].i1,
-                       d.triangles[mesh.triangle_offset + k].i2] for k in range(mesh.triangle_count)])
-        tris.append((v @ m[:, :3].T + m[:, 3])[t])
-        ids.append(np.stack([np.full(len(t), i), np.arange(len(t))], axis=1))
-        mags.append(np.abs(v[t]).max(axis=(1, 2)) * np.linalg.norm(m[:, :3], 2))
-    return np.concatenate(tris), np.concatenate(ids).astype(np.uint32), np.concatenate(mags)
-
-
-def _pack(o, d, tmax=FMAX, tmin=0.0):
-    rays = np.zeros((len(o), 8), np.float32)
-    rays[:, :3], rays[:, 3], rays[:, 4:7], rays[:, 7] = o, tmin, d, tmax
-    return rays
-
-
-def _unit(v):
-    return v / np.linalg.norm(v, axis=1, keepdims=True)
-
-
-def _aimed(rng, targets, dist):
-    d = _unit(rng.normal(size=targets.shape))
-    return _pack(targets - d * dist[:, None] if np.ndim(dist) else targets - d * dist, d)
-
-
-def make_rays(d, tris, ids, seed):
-    """The ray set of one scene (fixed seed): [base rays (checked against float64 too) ..., far rays]."""
-    rng = np.random.default_rng(seed)
-    pts = tris.reshape(-1, 3)
-    lo, hi = pts.min(axis=0), pts.max(axis=0)
-    c, r = (lo + hi) / 2, float((hi - lo).max())
-    pick = lambda a, n: a[rng.integers(0, len(a), n)]  # noqa: E731
-    cent = tris.mean(axis=1)
-    mids = np.concatenate([(tris[:, 0] + tris[:, 1]) / 2, (tris[:, 1] + tris[:, 2]) / 2, (tris[:, 2] + tris[:, 0]) / 2])
-    feats = np.concatenate([pts, mids])
-    jitter = lambda p: p + rng.normal(size=p.shape) * 1e-4 * r  # noqa: E731
-    parts = []
-    # one ray per triangle (at most 400) at its centroid, from around the scene
-    parts.append(_aimed(rng, pick(cent, min(len(cent), 400)), rng.uniform(0.5, 2.0, min(len(cent), 400)) * r))
-    # vertices and edge midpoints, jittered: silhouettes, shared edges and corners
-    parts.append(_aimed(rng, jitter(pick(feats, 800)), rng.uniform(0.5, 2.0, 800) * r))
-    # random rays through the scene's box (as in test_gpu_parity._random_rays), a third of them short
-    o = rng.uniform(lo - 0.5 * r, hi + 0.5 * r, size=(600, 3))
-    rand = _pack(o, _unit(rng.uniform(lo, hi, size=(600, 3)) - o))
-    rand[::3, 7] = rng.uniform(0.05, 1.0, size=len(rand[::3])) * r
-    parts.append(rand)
-    # axis-aligned directions and negative-zero components through vertices and edge midpoints (on the flat grid: rays in its
-    # plane, along its grid lines)
-    ax = _aimed(rng, jitter(pick(feats, 300)), 1.5 * r)
-    ax[:100, 4:7] = np.eye(3)[rng.integers(0, 3, 100)] * rng.choice([-1.0, 1.0], size=(100, 1))
-    ax[100:, 4 + rng.integers(0, 3)] = -0.0
-    ax[:, :3] = pick(feats, 300) - ax[:, 4:7] * (1.5 * r)
-    parts.append(ax)
-    base = np.concatenate(parts)
-    # rays that start on surfaces: points on the hit triangles (rounded to float32, so on either side), random directions
-    ref, _ = O.trace(d, base, brute=True)
-    hit = np.flatnonzero(ref["inst"] != MISS)[:600]
-    key = {(int(a), int(b)): k for k, (a, b) in enumerate(ids)}
-    bary = ref["bary"][hit].astype(np.float64)
-    tri = tris[[key[(int(a), int(b))] for a, b in zip(ref["inst"][hit], ref["prim"][hit])]]
-    p = (1 - bary.sum(axis=1))[:, None] * tri[:, 0] + bary[:, :1] * tri[:, 1] + bary[:, 1:] * tri[:, 2]
-    dirs = _unit(rng.normal(size=p.shape))
-    dirs[::5, 1] = -0.0
-    bounce = _pack(p, dirs)
-    bounce[1::4, 7] = 1e-3 * r
-    base = np.concatenate([base, bounce])
-    # distant origins aimed at vertices and edge midpoints (with a tiny jitter: silhouettes)
-    far = [_aimed(rng, pick(feats, FAR_RAYS) + rng.normal(size=(FAR_RAYS, 3)) * 1e-5 * r, k * r) for k in FAR_FACTORS]
-    return base, far
-
-
-# ---- float64 reference ----------------------------------------------------------------------------------------------------------
-
-def f64_check(rays, tris, ids, mags, brute, scale):
-    """Independent float64 Moeller-Trumbore over every visible triangle.  Where the answer is unambiguous - the nearest hit is more
-    than 1e-4 relative ahead of every other candidate and of the ray's ends, and at least 1e-5 inside its triangle (more for distant
-    origins, large object-space coordinates and grazing rays) - the brute force must hit the same (instance, primitive) at the same
-    point (1e-5 of the distance); a ray that passes every triangle by more than 1e-3 in the barycentrics must miss.  Returns the
-    number of rays with an unambiguous answer."""
-    p0, e1, e2 = tris[:, 0], tris[:, 1] - tris[:, 0], tris[:, 2] - tris[:, 0]
-    size = np.sqrt(np.linalg.norm(np.cross(e1, e2), axis=1))
-    kept = 0
-    for s in range(0, len(rays), 128):
-        with np.errstate(divide="ignore", invalid="ignore"):
-            kept += _f64_chunk(rays[s:s + 128], brute[s:s + 128], s, tris, ids, mags, scale, p0, e1, e2, size)
-    return kept
-
-
-def _f64_chunk(rays, b, first, tris, ids, mags, scale, p0, e1, e2, size):
-    o, dd = rays[:, :3].astype(np.float64), rays[:, 4:7].astype(np.float64)
-    tmin, tmax = rays[:, 3].astype(np.float64), rays[:, 7].astype(np.float64)
-    pvec = np.cross(dd[:, None, :], e2[None])
-    det = np.einsum("tk,rtk->rt", e1, pvec)
-    tvec = o[:, None, :] - p0[None]
-    u = np.einsum("rtk,rtk->rt", tvec, pvec) / det
-    q = np.cross(tvec, e1[None])
-    v = np.einsum("rk,rtk->rt", dd, q) / det
-    t = np.einsum("tk,rtk->rt", e2, q) / det
-    inside = np.minimum(np.minimum(u, v), 1.0 - u - v)
-    # candidates include those just outside the ray's ends: a ray that starts on a surface meets it again near t = 0, on either
-    # side of tmin (by up to 1e-4 x the scene size for grazing rays and large object-space coordinates)
-    in_range = (t > tmin[:, None] - 1e-3 * scale) & (t < tmax[:, None] * (1 + 1e-4)) & np.isfinite(t)
-    # 1e-5 of the barycentrics, more from far away, for large object-space coordinates and for grazing rays: the float32 test's
-    # barycentrics err by ~1e-7 x (distance or coordinate size) / (triangle size x |cos| of the angle to the normal)
-    dn = np.linalg.norm(dd, axis=1)[:, None]
-    reach = np.nan_to_num(np.abs(t), posinf=0.0) * dn + mags[None]
-    cos = np.abs(det) / (dn * size[None] ** 2)
-    margin = 1e-5 * np.maximum(1.0, np.nan_to_num(reach / size[None] / cos / 10.0, nan=np.inf))
-    cand_t = np.where(in_range & (inside >= -margin), t, np.inf)
-    order = np.argsort(cand_t, axis=1)[:, :2]
-    rows = np.arange(len(rays))
-    best = order[:, 0]
-    t1, t2 = cand_t[rows, best], cand_t[rows, order[:, 1]] if cand_t.shape[1] > 1 else np.full(len(rays), np.inf)
-    # a clear miss: no triangle within 1e-3 of its edges anywhere on the line before tmax (rays that start on a surface and
-    # rays from far away are decided by the float32 rounding of their own triangle)
-    miss = ~((t < tmax[:, None]) & (inside >= -np.maximum(1e-3, 10 * margin))).any(axis=1)
-    assert (b["inst"][miss] == MISS).all(), f"brute force hit where float64 finds no candidate: rays {(first + np.flatnonzero(miss & (b['inst'] != MISS)))[:5]}"
-    tol = 1e-4 * np.abs(t1) + 1e-5 * scale + 1e-6 * mags[best] / dn[:, 0]  # t rounds with the object-space coordinates too
-    clear = np.isfinite(t1) & (inside[rows, best] >= margin[rows, best]) & (t2 - t1 > tol) & (t1 - tmin > tol) & (tmax - t1 > tol)
-    k = np.flatnonzero(clear)
-    wrong = k[(b["inst"][k] != ids[best[k], 0]) | (b["prim"][k] != ids[best[k], 1])]
-    assert not len(wrong), f"brute force disagrees with float64 on unambiguous hits: rays {(first + wrong)[:5].tolist()}, " \
-        f"brute {b[wrong[:3]].tolist()}, float64 {ids[best[wrong[:3]]].tolist()} at t {t1[wrong[:3]].tolist()}"
-    # the hit point: 1e-5 of the distance, or what the barycentric margin allows
-    tb, bu = best[k], b["bary"][k].astype(np.float64)
-    ph = (1 - bu.sum(axis=1))[:, None] * tris[tb, 0] + bu[:, :1] * tris[tb, 1] + bu[:, 1:] * tris[tb, 2]
-    gap = np.linalg.norm(ph - (o[k] + t1[k, None] * dd[k]), axis=1)
-    assert (gap <= 1e-5 * t1[k] * dn[k, 0] + 4 * margin[k, tb] * size[tb]).all(), "brute-force hit point disagrees with float64"
-    return int(miss.sum()) + len(k)
-
-
-# ---- hits the triangle test takes outside its own box ----------------------------------------------------------------------------
-
-def _fma(a, b, c):
-    """fmaf on float32 arrays: the product of two float32 is exact in float64."""
-    return (a.astype(np.float64) * b + c).astype(np.float32)
-
-
-def _fdot(a, b):
-    return _fma(a[:, 0], b[:, 0], _fma(a[:, 1], b[:, 1], a[:, 2] * b[:, 2]))
-
-
-def _fcross(a, b):
-    return np.stack([_fma(a[:, 1], b[:, 2], -(a[:, 2] * b[:, 1])), _fma(a[:, 2], b[:, 0], -(a[:, 0] * b[:, 2])),
-                     _fma(a[:, 0], b[:, 1], -(a[:, 1] * b[:, 0]))], axis=1)
-
-
-def outside_own_box(d, rays, hits):
-    """Rays whose hit the float32 triangle test places outside the hit triangle's own padded box.
-
-    The Moeller-Trumbore test rounds too, by an amount that grows with the distance from the ray origin to the triangle and with how
-    grazing the ray is: rays from far away that pass a silhouette edge by a few 1e-7 of their length, or that graze a fan of
-    triangles through a shared vertex, can be accepted at a point that lies outside every box holding the triangle.  Whether such a
-    hit is found then depends on the hierarchy - no box test can be made to contain it - so these rays are the ones exempt from
-    the bit-exact comparison with the brute force.  This restates the test's arithmetic (object-space ray by fma, edges, t) and
-    flags the rays that miss the triangle's bounds, padded like bvh.cpp pads a leaf box, in exact arithmetic, and the rays whose t
-    lies outside the exact entry and exit distances of those bounds by more than the box test's own margin (kSlabExitScale)."""
-    out = np.zeros(len(rays), bool)
-    hit = np.flatnonzero(hits["inst"] != MISS)
-    if not len(hit):
-        return out
-    inst = hits["inst"][hit].astype(np.int64)
-    w = np.array([d.instances[i].world_to_object[:] for i in range(d.instance_count)], np.float32).reshape(-1, 3, 4)[inst]
-    o, dd = rays[hit, :3], rays[hit, 4:7]
-    oo = np.stack([_fma(w[:, a, 0], o[:, 0], _fma(w[:, a, 1], o[:, 1], _fma(w[:, a, 2], o[:, 2], w[:, a, 3]))) for a in range(3)], axis=1)
-    od = np.stack([_fma(w[:, a, 0], dd[:, 0], _fma(w[:, a, 1], dd[:, 1], w[:, a, 2] * dd[:, 2])) for a in range(3)], axis=1)
-    verts = np.array([v.p[:] for v in d.vertices[:d.vertex_count]], np.float32)
-    tris = np.array([(t.i0, t.i1, t.i2) for t in d.triangles[:d.triangle_count]], np.int64)
-    meshes = [d.meshes[d.instances[i].mesh] for i in range(d.instance_count)]
-    pad = np.zeros(d.instance_count, np.float32)
-    for i, m in enumerate(meshes):
-        v = verts[m.vertex_offset:m.vertex_offset + m.vertex_count]
-        pad[i] = np.float32(5e-7) * np.float32(max(np.abs(v).max(), (v.max(axis=0) - v.min(axis=0)).max()))
-    first = np.array([m.triangle_offset for m in meshes])[inst] + hits["prim"][hit]
-    voff = np.array([m.vertex_offset for m in meshes])[inst]
-    p = verts[tris[first] + voff[:, None]]
-    e1, e2 = p[:, 1] - p[:, 0], p[:, 2] - p[:, 0]
-    pvec = _fcross(od, e2)
-    with np.errstate(divide="ignore"):
-        inv_det = np.float32(1.0) / _fdot(e1, pvec)
-    t = _fdot(e2, _fcross(oo - p[:, 0], e1)) * inv_det
-    lo = (p.min(axis=1) - pad[inst][:, None]).astype(np.float64)
-    hi = (p.max(axis=1) + pad[inst][:, None]).astype(np.float64)
-    o64, d64 = oo.astype(np.float64), od.astype(np.float64)
-    with np.errstate(divide="ignore", invalid="ignore"):
-        t0, t1 = (lo - o64) / d64, (hi - o64) / d64
-    inside = (o64 >= lo) & (o64 <= hi)  # axes the ray is parallel to: all or nothing
-    near = np.where(d64 == 0, np.where(inside, -np.inf, np.inf), np.minimum(t0, t1)).max(axis=1)
-    far = np.where(d64 == 0, np.where(inside, np.inf, -np.inf), np.maximum(t0, t1)).min(axis=1)
-    t = t.astype(np.float64)
-    out[hit] = (near > far) | (t < near - 2.0 ** -20 * np.abs(near)) | (t > far + 2.0 ** -20 * np.abs(far))
-    return out
-
 
 # ---- fixtures -------------------------------------------------------------------------------------------------------------------
 
-CATALOGUE = catalogue()
 NAMES = list(CATALOGUE)
+# the 1000 clusters of far_mesh_instances_1000 are 0.1 wide and 2.4e4 apart: rays jittered by 1e-5 of the scene pass most of them
+MIN_HITS = {"far_mesh_instances_1000": 0.002}
+_CASES: dict[str, _Case] = {}
 
 
-class Case:
-    def __init__(self, name):
-        meshes, instances = CATALOGUE[name]
-        self.scene = Scene.from_source(scene_text(meshes, instances), REPO)
-        self.desc = self.scene.desc()
-        self.tris, self.ids, self.mags = _desc_triangles(self.desc)
-        self.base, self.far = make_rays(self.desc, self.tris, self.ids, seed=NAMES.index(name) + 1)
-        self.rays = np.concatenate([self.base] + self.far)
-        self.brute, _ = O.trace(self.desc, self.rays, brute=True)
-        self.occ_brute, _ = O.trace(self.desc, self.rays, any_hit=True, brute=True)
-        self.loose = outside_own_box(self.desc, self.rays, self.brute)
-
-
-_CASES: dict[str, Case] = {}
-
-
-def case(name) -> Case:
+def case(name) -> _Case:
     if name not in _CASES:
-        _CASES[name] = Case(name)
+        _CASES[name] = _Case(*CATALOGUE[name], seed=SEEDS.get(name, NAMES.index(name) + 1))
     return _CASES[name]
-
-
-def _differ(got, ref):
-    return ((got["inst"] != ref["inst"]) | (got["prim"] != ref["prim"])
-            | (got["bary"].view(np.uint32) != ref["bary"].view(np.uint32)).any(axis=1))
-
-
-def _assert_equal_hits(got, ref, loose, what):
-    """Bit-identical hit records, except on the rays whose reference hit the triangle test takes outside its own box."""
-    bad = np.flatnonzero(_differ(got, ref) & ~loose)
-    lost = int(((got["inst"] == MISS) & (ref["inst"] != MISS))[bad].sum())
-    assert not len(bad), f"{what}: {len(bad)} of {len(got)} rays differ from the brute force ({lost} lost a hit), first: {bad[:5].tolist()}"
 
 
 @pytest.mark.parametrize("name", NAMES)
@@ -397,7 +41,7 @@ def test_oracle_bvh_equals_brute_force(name):
     occ, _ = O.trace(c.desc, c.rays, any_hit=True)
     assert not (occ["inst"] != c.occ_brute["inst"])[~c.loose].any()
     assert np.array_equal(c.occ_brute["inst"] == 1, c.brute["inst"] != MISS)
-    assert (c.brute["inst"] != MISS).mean() > 0.2 and cnt["nodes_visited"] > 0
+    assert (c.brute["inst"] != MISS).mean() > MIN_HITS.get(name, 0.2) and cnt["nodes_visited"] > 0
     near = slice(0, len(c.base))
     print(f"{name}: {len(c.rays)} rays, {int(c.loose.sum())} exempt ({int(c.loose[near].sum())} of the {len(c.base)} near ones), "
           f"{int(_differ(got, c.brute).sum())} of those differ")
@@ -415,8 +59,18 @@ def test_oracle_bvh_equals_brute_force_from_far_away(name):
         sl = slice(begin, begin + len(rays))
         begin += len(rays)
         got, _ = O.trace(c.desc, rays)
-        assert (c.brute["inst"][sl] != MISS).mean() > 0.2  # aimed at silhouettes: many pass by
+        assert (c.brute["inst"][sl] != MISS).mean() > MIN_HITS.get(name, 0.2)  # aimed at silhouettes: many pass by
         _assert_equal_hits(got, c.brute[sl], c.loose[sl], f"origins {k}x the scene size away")
+
+
+@pytest.mark.parametrize("name", list(SEEDS))
+def test_seeded_scenes_draw_a_hit_the_instance_level_loses(name):
+    """The reproductions of outside_instance_box stay reproductions: their rays include one whose hit the oracle's walk of the
+    host-built hierarchy does not return and that only outside_instance_box exempts (its hit is inside its triangle's own box)."""
+    c = case(name)
+    got, _ = O.trace(c.desc, c.rays)
+    lost = _differ(got, c.brute) & c.instance & ~c.own
+    assert lost.any() and not (_differ(got, c.brute) & ~c.loose).any()
 
 
 @pytest.mark.parametrize("name", NAMES)
@@ -494,7 +148,7 @@ def test_gpu_films_of_host_and_device_hierarchies_are_identical(name, gpu_render
             r.clear()
             r.render(0, 3)  # raises on a traversal stack overflow
             films.append(r.film(raw=True).copy())
-        assert (films[0][..., 3] == 3).all() and films[0][..., :3].max() > 0
+        assert (films[0][..., 3] == 3).all() and (films[0][..., :3].max() > 0 or name in MIN_HITS)  # the sparse scene is black
         assert np.array_equal(films[0], films[1])
     finally:
         r.set_option("device_bvh", 0)

@@ -69,43 +69,6 @@ def test_frames_differ_only_in_the_replaced_meshes(name):
             assert bytes(x) == bytes(y)
 
 
-def _move(lib, nodes, node_delta, slot_delta):
-    out = np.zeros_like(nodes)
-    lib.relayout_nodes(nodes.ctypes.data, out.ctypes.data, len(nodes), node_delta % 2**32, slot_delta % 2**32)
-    return out
-
-
-def _relaid(a, b, lib):
-    """The hierarchy lrk_replace_meshes leaves for frame a replaced by frame b's meshes, built on the host: in mesh order, every
-    unchanged mesh's node range of a moved to its new place, every replaced mesh's range of max(n - 1, 1) nodes starting with b's
-    own hierarchy of it (moved), and b's instance level behind them.  Returns the description (b's with these nodes and roots),
-    the arrays it points into, and the new ranges."""
-    ids, _, _ = S.replaced_meshes(a, b)
-    nodes_a = S.array(a.bvh_nodes, a.bvh_node_count, F.BvhNode, np.uint32, 16)
-    nodes_b = S.array(b.bvh_nodes, b.bvh_node_count, F.BvhNode, np.uint32, 16)
-    ma, mb = S.meshes(a), S.meshes(b).copy()
-    ra, rb = U.node_ranges(a), U.node_ranges(b)
-    parts, ranges, base = [], [], 0
-    for k in range(b.mesh_count):
-        if k in ids:
-            first, end = rb[k]
-            size = max(int(mb[k, 3]) - 1, 1)
-            assert end - first <= size  # the host's hierarchy never has more nodes than the device builder's
-            part = np.zeros((size, 16), np.uint32)
-            part[:end - first] = _move(lib, nodes_b[first:end], base - first, 0)
-        else:
-            first, end = ra[k]
-            part = _move(lib, nodes_a[first:end], base - first, int(mb[k, 5]) - int(ma[k, 5]))
-            # the same mesh's hierarchy in b (the host build is deterministic), moved from b's place to the new one
-            assert np.array_equal(part, _move(lib, nodes_b[rb[k][0]:rb[k][1]], base - rb[k][0], 0))
-        mb[k, 4] = base
-        ranges.append((base, base + len(part)))
-        parts.append(part)
-        base += len(part)
-    h, keep = U.with_hierarchies(b, np.concatenate(parts), mb)
-    return h, keep, ranges, ids
-
-
 def test_relayout_rules(refit_host):
     leaf = lambda count, slot: 0x80000000 | ((count - 1) << 28) | slot
     node = np.zeros((3, 16), np.uint32)
@@ -113,7 +76,7 @@ def test_relayout_rules(refit_host):
     node[:, 12:15] = [[5, leaf(3, 40), 0xFFFFFFFF], [0xFFFFFFFF, leaf(4, 0x0FFFFFF0), 9], [leaf(1, 7), 12, 2]]
     node[:, 15] = 77
     for nd, sd in ((7, 3), (-4, -7), (0, 0x10)):
-        out = _move(refit_host, node, nd, sd)
+        out = U.move_nodes(refit_host, node, nd, sd)
         assert np.array_equal(out[:, :12], node[:, :12]) and np.array_equal(out[:, 15], node[:, 15])  # boxes stay
         for got, ref in zip(out[:, 12:14].reshape(-1), node[:, 12:14].reshape(-1)):
             if ref == 0xFFFFFFFF:
@@ -130,7 +93,7 @@ def test_relayout_rules(refit_host):
 def test_relaid_hierarchies_trace_like_the_replaced_frame(name, refit_host):
     for fa, fb in _pairs(name):
         a, b = fa.desc(), fb.desc()
-        h, keep, ranges, ids = _relaid(a, b, refit_host)
+        h, keep, ranges, ids = U.relaid_frame(a, b, refit_host)
         rays = U.random_rays(fb, 100_000, seed=5)
         for any_hit in (False, True):
             want, _ = O.trace(b, rays, any_hit=any_hit)

@@ -85,33 +85,6 @@ def test_shared_alias_tables_reproduce_the_flattened_ones(name, refit_host):
             assert np.array_equal(table, alias[to:to + tc]) and np.array_equal(p, pdf[to:to + tc, 0])
 
 
-def _hybrid(a, b, lib):
-    """A description that renders frame b with frame a's mesh hierarchies refit to b's vertices (what lrk_update_meshes leaves on
-    the device): a's refit BLAS nodes and mesh table, a's slot order with b's positions, b's vertices and instances, and b's
-    instance level appended behind a's meshes.  Returns the description, the arrays it points into and the refit meshes' pads."""
-    nodes_a = S.array(a.bvh_nodes, a.bvh_node_count, F.BvhNode, np.uint32, 16)
-    blas = np.ascontiguousarray(nodes_a[:a.tlas_root])
-    # a's slot order, b's positions: every slot's primitive re-read through b's triangles and vertices
-    tv = S.array(a.tri_verts, a.tri_slot_count, C.c_float * 12).copy()
-    vb, tris = S.vertices(b), S.triangles(b)
-    m = S.meshes(a)
-    for vo, vc, to, tc, _root, so, *_ in m:
-        prim = tv[so:so + tc, 3].view(np.uint32)
-        t = tris[to + prim]
-        for c in range(3):
-            tv[so:so + tc, 4 * c:4 * c + 3] = vb[vo + t[:, c], :3]
-    ids, _ = S.deformed_meshes(a, b)
-    pads = {}
-    for k in ids:
-        root, end = U.node_ranges(a)[k]
-        pad = C.c_float()
-        assert lib.refit_mesh(blas.ctypes.data, root, end, tv.ctypes.data, int(m[k][5]), int(m[k][3]), C.byref(pad)) == 0
-        pads[k] = pad.value
-    h, keep = U.with_hierarchies(b, blas, m)
-    h.tri_verts = tv.ctypes.data_as(C.POINTER(C.c_float))
-    return h, keep + [tv], pads, blas, tv, ids
-
-
 def _check_refit_boxes(a, blas, tv, ids, pads):
     """Every reachable leaf child's stored box is its slots' triangle box padded by exactly 5e-7 x the deformed mesh's extent."""
     m = S.meshes(a)
@@ -146,7 +119,7 @@ def test_refit_hierarchies_trace_like_the_deformed_frame(name, refit_host):
     a = frames[0].desc()
     for f in frames[1:]:
         b = f.desc()
-        h, keep, pads, blas, tv, ids = _hybrid(a, b, refit_host)
+        h, keep, pads, blas, tv, ids = U.refit_frame(a, b, refit_host)
         _check_refit_boxes(a, blas, tv, ids, pads)
         rays = U.random_rays(f, 100_000, seed=5)
         for any_hit in (False, True):
