@@ -469,7 +469,7 @@ typedef struct lrk_scene_desc {
 typedef struct lrk_device_cfg {
     int32_t device_index;      /* -1: current device */
     uint32_t reserved;
-    uint64_t max_paths_per_pass; /* 0: default (8 Mi) */
+    uint64_t max_paths_per_pass; /* 0: default (136 Mi) */
 } lrk_device_cfg;
 
 typedef struct lrk_stats {

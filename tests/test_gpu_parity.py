@@ -199,8 +199,10 @@ def test_render_is_deterministic_and_independent_of_scheduling(cornell_small, gp
     assert np.array_equal(a, gpu_renderer.film(raw=True))
     gpu_renderer.clear()
     gpu_renderer.set_option("max_paths_per_pass", 1024)  # many small passes, pixel chunks smaller than the film
-    gpu_renderer.render(0, 8)
-    gpu_renderer.set_option("max_paths_per_pass", 8 << 20)
+    try:
+        gpu_renderer.render(0, 8)
+    finally:
+        gpu_renderer.set_option("max_paths_per_pass", 136 << 20)  # the default of lrk_create
     assert np.array_equal(a, gpu_renderer.film(raw=True))
     # traversal counting does not change the result and counts the oracle's numbers
     gpu_renderer.clear()

@@ -16,13 +16,14 @@ import pytest
 from luisarender_b200 import _ffi as F
 from luisarender_b200 import scenes
 from luisarender_b200.api import Renderer, Scene
-from luisarender_b200.distributed import owned_pixel_mask, tile_owner
+from luisarender_b200.distributed import owned_pixel_mask
 from oracle import binding as O
+from oracle_shards import TILE, shard, with_depth
 
 pytestmark = pytest.mark.gpu
 REPO = Path(__file__).resolve().parents[1]
 TABLE_SAMPLERS = ("PMJ02BN", "Sobol", "PaddedSobol", "ZSobol")
-TILE = 32
+DEFAULT_PATHS_PER_PASS = 136 << 20  # the default of lrk_create
 REDUCED = dict(big_subdivision=3, small_subdivision=2)
 FRAMES = {
     "c2_cornell_1024x1024_4096": lambda: scenes.cornell_box(resolution=(1024, 1024), spp=4096),
@@ -47,21 +48,6 @@ def scene(frame: str, sampler: str) -> Scene:
             src = src.replace("sampler : Independent", f"sampler : {sampler}")
         _scenes[(frame, sampler)] = Scene.from_source(src, REPO)
     return _scenes[(frame, sampler)]
-
-
-def with_depth(d, depth: int):
-    """A copy of the description with another max_depth (the arrays stay the scene's)."""
-    c = F.SceneDesc.from_buffer_copy(d)
-    c.integrator.max_depth = depth
-    return c
-
-
-def shard(d):
-    """(rank, world): a shard of about 32 tiles that owns the frame's last tile, so it holds tiles of the last row and column."""
-    w, h = d.camera.resolution[0], d.camera.resolution[1]
-    tiles = ((w + TILE - 1) // TILE) * ((h + TILE - 1) // TILE)
-    world = max(tiles // 32, 1)
-    return int(tile_owner(tiles - 1, world)), world
 
 
 def oracle(frame, sampler, d, depth, begin, end):
@@ -157,7 +143,7 @@ def test_range_ends_match_oracle(frame, sampler, gpu_renderer):
         gpu_renderer.render(spp - 4, spp - 2)
         gpu_renderer.render(spp - 2, spp)
     finally:
-        gpu_renderer.set_option("max_paths_per_pass", 8 << 20)
+        gpu_renderer.set_option("max_paths_per_pass", DEFAULT_PATHS_PER_PASS)
     assert np.array_equal(gpu_renderer.film(raw=True), whole)
 
 
